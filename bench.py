@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — registrations/sec of the scan-matching hot path on B200 (BASELINE.json metric).
+"""bench.py — registrations/sec of the scan-matching hot path on H100 (BASELINE.json metric).
 
 Default workload = BASELINE.json configs[1]: GICP odometry over a synthetic VLP-16 sequence (65 536 pts/scan,
 fast_gicp defaults of the reference's launch file: k=20, max_corr 2.5 m, eps 0.01, <=64 LM iterations; keyframe rule of
@@ -22,6 +22,12 @@ config.strict_chain_value.
 Other workloads: --workload ndt_odometry_hdl32e_128k (configs[2]), --workload loop_batch (configs[3]), --workload gicp_odometry_vlp16_64k,
 --workload voxelgrid (SURVEY §8 row a5 alone), --workload kitti_pipeline (configs[4]'s per-scan chain: prefilter -> odometry in HBM); the last
 two live in bench_workloads.py.
+
+--dump-outputs DIR writes what the GPU arm's headline pass returned to its caller in the last timed step as DIR/<name>.npy
+(float32 clouds and poses, float64 otherwise, at most 64 MB): odometry workloads the b2r_odometry_status (odom / trans 4x4 poses,
+converged / iterations / keyframe_updated / frame_rejected); kitti_pipeline the same plus the filtered point count; loop_batch every
+pair's record as rank 0 holds it after the all-gather (T, fitness, converged, iterations) and the per-group best candidate; voxelgrid the
+downsampled cloud.  Inputs are seeded synthetic scans, so equal arguments give equal inputs on every run.
 """
 import argparse
 import json
@@ -29,6 +35,7 @@ import os
 import statistics
 import subprocess
 import sys
+import tempfile
 import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
@@ -43,10 +50,10 @@ WORKLOADS = {
 }
 
 
-def parse():
+def parse(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--steps", type=int, default=None, help="timed steps (default: 5 passes of the batch for loop_batch, 200 otherwise)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default=None, choices=list(WORKLOADS) + ["loop_batch", "voxelgrid", "kitti_pipeline"],
@@ -59,16 +66,8 @@ def parse():
     ap.add_argument("--no-anchor", action="store_true", help="N = 1 odometry line: skip the loop_batch_n1 / strict-chain extras")
     ap.add_argument("--no-profile", action="store_true")
     ap.add_argument("--no-prefetch", action="store_true", help="strict call-by-call chain: do not announce the next frame (no software pipelining)")
-    return ap.parse_args()
-
-
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` capture (profiles/), or None"""
-    p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    try:
-        return json.load(open(p)).get(kernel)
-    except Exception:  # noqa: BLE001
-        return None
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as DIR/<name>.npy (GPU arm)")
+    return ap.parse_args(argv)
 
 
 def peaks():
@@ -78,7 +77,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "fallback"  # H100 SXM data sheet: 3.35 TB/s of HBM3
 
 
 class ClockSampler:
@@ -92,7 +91,7 @@ class ClockSampler:
     MIN_WINDOW_S = 0.7
 
     def __init__(self, dev):
-        self.dev, self.p, self.path = dev, None, f"/tmp/b2r_clocks_{os.getpid()}.csv"
+        self.dev, self.p, self.path = dev, None, os.path.join(tempfile.gettempdir(), f"b2r_clocks_{os.getpid()}.csv")
         self.t0 = self.t1 = None
         self.extra_steps = 0
 
@@ -339,7 +338,7 @@ def run_reference(args, wl, rank):
     print(json.dumps(line), flush=True)
 
 
-# ------------------------------------------------------------------------------------------------ B200 arm
+# ------------------------------------------------------------------------------------------------ GPU arm
 def algorithmic_bytes(cls, n, m, stride_bytes):
     """SURVEY.md §8(d): compulsory bytes per launch of each kernel class (N source points, M target points)."""
     return {
@@ -369,6 +368,27 @@ def whole_step_algorithmic_gbs(calls, n, m, stride_bytes, total_ms, steps):
     if total_ms <= 0 or steps <= 0:
         return None
     return total / (total_ms * 1e-3) / 1e9, total / steps, unknown
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def odometry_outputs(status):
+    """the b2r_odometry_status of one step as the Python caller receives it.  matching_error / inlier_fraction are left out: the
+    bench runs with publish_status off, so the engine reports them as NaN."""
+    return {k: v for k, v in status.items() if k not in ("matching_error", "inlier_fraction")}
+
+
+def dump_outputs(out_dir, outputs):
+    """outputs: name -> array-like.  float32 arrays stay float32, everything else is written as float64; refuses more than 64 MB."""
+    arrays = {k: np.asarray(v) for k, v in outputs.items()}
+    arrays = {k: (a if a.dtype == np.float32 else a.astype(np.float64)) for k, a in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise ValueError(f"--dump-outputs: {total} bytes of outputs exceed the {DUMP_LIMIT_BYTES}-byte limit")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def run_b200(args, wl, rank, world, local_rank):
@@ -461,7 +481,7 @@ def run_b200(args, wl, rank, world, local_rank):
             sampler.hold(lambda k: step(W + 1 + (k % K)), reg.synchronize)
             clocks = sampler.stop()
         results[arm] = dict(ms=float(t.item()), per_rank_ms=per_rank, wall_ms=wall * 1e3, stats=stats, iters=iters, conv=conv, kf=kf, clocks=clocks,
-                            last_odom=st["odom"])
+                            last=st)
         odo.close()
         reg.close()
 
@@ -470,6 +490,8 @@ def run_b200(args, wl, rank, world, local_rank):
             dist.destroy_process_group()
         return
     rv, re_ = results["value"], results["e2e"]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, odometry_outputs(rv["last"]))
     value = world * K / (rv["ms"] * 1e-3)
     e2e = world * K / (re_["ms"] * 1e-3)
     launches = int(sum(rv["stats"]["launches"].values()))
@@ -484,8 +506,8 @@ def run_b200(args, wl, rank, world, local_rank):
         ab = algorithmic_bytes(top, n, n, stride_bytes)
         if ab:
             achieved = ab / (per_launch_ms * 1e-3) / 1e9
-            roofline = {"bound": "hbm", "kernel": top, "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm, "traffic": ncu_traffic(top),
-                        "peak_source": f"of {how} (MEASURED_PEAKS.json hbm_gbs)" if how == "measured" else "of fallback (6.65 TB/s)",
+            roofline = {"bound": "hbm", "kernel": top, "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm,
+                        "peak_source": f"of {how} (MEASURED_PEAKS.json hbm_gbs)" if how == "measured" else "of fallback (3.35 TB/s, H100 SXM data sheet)",
                         "algorithmic_bytes_per_launch": ab, "avg_launch_us": per_launch_ms * 1e3, "launches_timed": st["calls"][top],
                         "share_of_step": st["ms"][top] / prof_ms,
                         "note": "single-pair working set (~9 MB) is L2-resident: this is the odometry chain's latency-bound figure; see DESIGN.md"}
@@ -551,20 +573,27 @@ def run_b200(args, wl, rank, world, local_rank):
         dist.destroy_process_group()
 
 
-def main():
-    args = parse()
-    rank = int(os.environ.get("RANK", "0"))
-    world = int(os.environ.get("WORLD_SIZE", "1"))
-    local_rank = int(os.environ.get("LOCAL_RANK", "0"))
+def resolve_args(args, world):
+    """fills in the workload- and world-dependent defaults; an explicit --steps is never changed"""
     if args.workload is None:
         # the odometry chain cannot shard (frame k's guess is frame k-1's pose): at N > 1 measure the path that does
         args.workload = "loop_batch" if max(world, args.gpus) > 1 else "gicp_odometry_vlp16_64k"
+    if args.steps is None:
+        args.steps = 5 if args.workload == "loop_batch" else 200  # loop_batch: one step is a pass over the whole candidate batch
+    if args.dump_outputs and args.impl != "b200":
+        raise SystemExit("--dump-outputs: only the GPU arm (--impl b200) writes outputs")
+    return args
+
+
+def main():
+    rank = int(os.environ.get("RANK", "0"))
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    local_rank = int(os.environ.get("LOCAL_RANK", "0"))
+    args = resolve_args(parse(), world)
     if args.workload == "loop_batch":
         if args.impl == "reference":
             return run_reference_loop(args, rank)
         from hdl_graph_slam_b200 import batch
-        if args.steps == 200:
-            args.steps = 5  # default: 5 timed passes of the whole batch
         args.warmup = max(args.warmup, 3) if args.warmup != 5 else 3
         return batch.bench_loop_batch(args, rank, world, local_rank)
     if args.workload in ("voxelgrid", "kitti_pipeline"):

@@ -19,7 +19,7 @@ KITTI_PREFILTER = dict(use_distance_filter=1, distance_near_thresh=0.1, distance
 KITTI_ODOMETRY = {"registration_method": "FAST_GICP", "reg_transformation_epsilon": 0.1, "reg_maximum_iterations": 64,
                   "reg_max_correspondence_distance": 2.0, "reg_correspondence_randomness": 20}
 KITTI_KEYFRAME = dict(keyframe_delta_trans=5.0, keyframe_delta_angle=2.0, keyframe_delta_time=10000.0)
-N_FRAMES = 40  # 40 x 3.84 MB of raw scans = 154 MB > the 126 MB L2: consecutive steps never find their input in cache
+N_FRAMES = 40  # 40 x 3.84 MB of raw scans = 154 MB > the 50 MB L2: consecutive steps never find their input in cache
 
 
 def _setup(args, rank, world, local_rank):
@@ -44,7 +44,8 @@ def _frames(torch, dev, rank, count=N_FRAMES):
     return host, devbuf, int(n), int(stride_f)
 
 
-def _timed(torch, dist, dev, world, stream, K, body, sampler=None, stats_fn=None):
+def _timed(torch, dist, dev, world, stream, K, body, sampler=None, stats_fn=None, after=None):
+    """K timed calls of body; `after` (if given) runs once the timed region has drained, before any untimed hold step"""
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
@@ -60,6 +61,8 @@ def _timed(torch, dist, dev, world, stream, K, body, sampler=None, stats_fn=None
     wall = time.perf_counter() - t0
     clocks = None
     stats = stats_fn() if stats_fn else None  # counters of the timed region only (the hold steps below are not part of it)
+    if after:
+        after()
     if sampler:  # untimed steps of the same workload until nvidia-smi has sampled the load (bench.ClockSampler)
         sampler.hold(lambda k: body(k % K), torch.cuda.synchronize)
         clocks = sampler.stop()
@@ -69,6 +72,13 @@ def _timed(torch, dist, dev, world, stream, K, body, sampler=None, stats_fn=None
         dist.barrier()
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     return float(t.item()), wall * 1e3, clocks, stats
+
+
+def _device_floats(torch, dev, ptr, rows, cols):
+    """copy of a float32 (rows, cols) array the engine left in device memory"""
+    class _View:
+        __cuda_array_interface__ = {"shape": (rows, cols), "typestr": "<f4", "data": (ptr, False), "version": 2, "strides": None}
+    return torch.as_tensor(_View(), device=dev).cpu().numpy().copy()
 
 
 def _cpu_voxelgrid(host, leaf, budget_s=10.0):
@@ -91,10 +101,16 @@ def bench_voxelgrid(args, rank, world, local_rank, leaf=0.25):
     stream = torch.cuda.ExternalStream(reg.getStream(), device=dev)
     fbytes = n * stride_f * 4
     counts = []
+    last = {}
 
     def dev_step(k):
-        _, m, _ = reg.voxelGridFilterDevice(devbuf.data_ptr() + (k % N_FRAMES) * fbytes, n, stride_f * 4, leaf)
+        last["ptr"], m, _ = reg.voxelGridFilterDevice(devbuf.data_ptr() + (k % N_FRAMES) * fbytes, n, stride_f * 4, leaf)
         counts.append(m)
+
+    def keep_last_cloud():  # the downsampled cloud of the last timed step, before the hold steps reuse the output buffer
+        if args.dump_outputs and rank == 0:
+            reg.synchronize()
+            last["cloud"] = _device_floats(torch, dev, last["ptr"], counts[-1], stride_f)
 
     def host_step(k):
         out = reg.voxelGridFilter(host[k % N_FRAMES].numpy(), leaf)
@@ -109,12 +125,14 @@ def bench_voxelgrid(args, rank, world, local_rank, leaf=0.25):
         reg.setProfiling(arm == "profile")
         counts.clear()
         sampler = bench.ClockSampler(local_rank) if (rank == 0 and arm == "value") else None
-        ms, wall, clocks, stats = _timed(torch, dist, dev, world, stream, K, body, sampler, reg.getStats)
+        ms, wall, clocks, stats = _timed(torch, dist, dev, world, stream, K, body, sampler, reg.getStats, keep_last_cloud if arm == "value" else None)
         res[arm] = dict(ms=ms, wall=wall, clocks=clocks, stats=stats, n_ds=float(np.mean(counts)))
         reg.setProfiling(False)
     reg.close()
     if rank != 0:
         return
+    if args.dump_outputs:
+        bench.dump_outputs(args.dump_outputs, {"cloud": last["cloud"]})
     hbm, how = bench.peaks()
     n_ds = res["value"]["n_ds"]
     ab = 2 * 16 * n + 16 * n_ds  # SURVEY §8d: N_raw x 16 x 2 (read for the key + read for the sum) + N_ds x 16
@@ -133,11 +151,11 @@ def bench_voxelgrid(args, rank, world, local_rank, leaf=0.25):
                 "d2h_bytes_per_step": res["e2e"]["stats"]["d2h_bytes"] / K, "ms_per_step": res["e2e"]["ms"] / K},
         "gpu_launches": int(sum(res["value"]["stats"]["launches"].values())),
         "clocks": res["value"]["clocks"],
-        "roofline": {"bound": "hbm", "kernel": "k_voxelgrid_cluster<8> (keys + cluster radix sort + centroids + compaction in one launch)", "achieved": ab / (per_launch_ms * 1e-3) / 1e9,
-                     "peak": hbm, "unit": "GB/s", "frac": ab / (per_launch_ms * 1e-3) / 1e9 / hbm, "traffic": bench.ncu_traffic("voxelgrid_cluster"),
-                     "peak_source": f"of {how} (MEASURED_PEAKS.json hbm_gbs)" if how == "measured" else "of fallback (6.65 TB/s)",
+        "roofline": {"bound": "hbm", "kernel": "k_voxelgrid_cluster (keys + cluster radix sort + centroids + compaction in one launch)", "achieved": ab / (per_launch_ms * 1e-3) / 1e9,
+                     "peak": hbm, "unit": "GB/s", "frac": ab / (per_launch_ms * 1e-3) / 1e9 / hbm,
+                     "peak_source": f"of {how} (MEASURED_PEAKS.json hbm_gbs)" if how == "measured" else "of fallback (3.35 TB/s, H100 SXM data sheet)",
                      "algorithmic_bytes_per_launch": ab, "avg_launch_us": per_launch_ms * 1e3, "launches_timed": st["calls"][cls],
-                     "note": "one 8-CTA cluster per scan: latency bound on 8 of 148 SMs (8 cluster barriers per scan); concurrent scans on other streams fill the rest"},
+                     "note": "one cluster per scan (16 CTAs where the device accepts that size, else 8): latency bound on a few of 132 SMs; concurrent scans on other streams fill the rest"},
         "cpu_baseline": {"value": cpu_v, "unit": "scans/s", "cores": 1, "kind": "port", "sample": f"{cpu_n} scans of the same workload through the oracle's pcl::VoxelGrid restatement"},
     }
     print(json.dumps(line), flush=True)
@@ -189,7 +207,7 @@ def bench_kitti_pipeline(args, rank, world, local_rank):
         reg = pkg.select_registration_method(dict(KITTI_ODOMETRY), device_id=local_rank)
         odo = pkg.ScanMatchingOdometry(reg, **KITTI_KEYFRAME)
         stream = torch.cuda.ExternalStream(reg.getStream(), device=dev)
-        state = dict(m=[], iters=[], conv=0, kf=0, odom=None)
+        state = dict(m=[], iters=[], conv=0, kf=0, last=None)
 
         def step(k, arm=arm, reg=reg, odo=odo, state=state):
             f = k % N_FRAMES
@@ -202,7 +220,7 @@ def bench_kitti_pipeline(args, rank, world, local_rank):
             state["iters"].append(st["iterations"])
             state["conv"] += int(st["converged"])
             state["kf"] += int(st["keyframe_updated"])
-            state["odom"] = st["odom"]
+            state["last"] = dict(bench.odometry_outputs(st), filtered_points=m)
 
         for k in range(W):
             step(k)
@@ -213,16 +231,20 @@ def bench_kitti_pipeline(args, rank, world, local_rank):
             state[key].clear()
         state["conv"] = state["kf"] = 0
         sampler = bench.ClockSampler(local_rank) if (rank == 0 and arm == "value") else None
-        ms, wall, clocks, stats = _timed(torch, dist, dev, world, stream, K, lambda k: step(k + W), sampler, reg.getStats)
+        kept = {}
+        ms, wall, clocks, stats = _timed(torch, dist, dev, world, stream, K, lambda k: step(k + W), sampler, reg.getStats,
+                                         lambda: kept.update(state["last"]))
         res[arm] = dict(ms=ms, wall=wall, clocks=clocks, stats=stats, m=float(np.mean(state["m"])), iters=float(np.mean(state["iters"])),
-                        conv=state["conv"], kf=state["kf"])
+                        conv=state["conv"], kf=state["kf"], last=kept)
         reg.setProfiling(False)
         odo.close()
         reg.close()
     if rank != 0:
         return
-    hbm, how = bench.peaks()
     rv = res["value"]
+    if args.dump_outputs:
+        bench.dump_outputs(args.dump_outputs, rv["last"])
+    hbm, how = bench.peaks()
     st = res["profile"]["stats"]
     m = int(rv["m"])
     cls = max(st["ms"], key=lambda c: st["ms"][c])
@@ -231,8 +253,8 @@ def bench_kitti_pipeline(args, rank, world, local_rank):
     roofline = None
     if ab:
         roofline = {"bound": "hbm", "kernel": cls, "achieved": ab / (per_launch_ms * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s",
-                    "frac": ab / (per_launch_ms * 1e-3) / 1e9 / hbm, "traffic": None,
-                    "peak_source": f"of {how} (MEASURED_PEAKS.json hbm_gbs)" if how == "measured" else "of fallback (6.65 TB/s)",
+                    "frac": ab / (per_launch_ms * 1e-3) / 1e9 / hbm,
+                    "peak_source": f"of {how} (MEASURED_PEAKS.json hbm_gbs)" if how == "measured" else "of fallback (3.35 TB/s, H100 SXM data sheet)",
                     "algorithmic_bytes_per_launch": ab, "avg_launch_us": per_launch_ms * 1e3, "launches_timed": st["calls"][cls],
                     "share_of_step": st["ms"][cls] / res["profile"]["ms"],
                     "note": f"filtered scans are ~{m} points: a pair's working set sits in L2, latency-bound single chain"}

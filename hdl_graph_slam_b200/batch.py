@@ -272,14 +272,19 @@ def run_loop_batch(args, rank, world, local_rank, quiet=False):
         achieved = bytes_per_pair_round * prof["pair_rounds"] / (round_ms * 1e-3) / 1e9
         launches = st["calls"].get("gicp_correspondences", 0) + st["calls"].get("gicp_linearize", 0)
         roofline = {"bound": "hbm", "kernel": "k_pair_search + k_pair_accumulate (one batched LM round = update_correspondences + linearize + compute_error of every pair in flight)",
-                    "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm, "traffic": bench.ncu_traffic("pair_round"),
-                    "peak_source": f"of {how} (MEASURED_PEAKS.json hbm_gbs)" if how == "measured" else "of fallback (6.65 TB/s)",
+                    "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm,
+                    "peak_source": f"of {how} (MEASURED_PEAKS.json hbm_gbs)" if how == "measured" else "of fallback (3.35 TB/s, H100 SXM data sheet)",
                     "algorithmic_bytes_per_pair_round": bytes_per_pair_round, "pair_rounds": prof["pair_rounds"], "rounds": prof["rounds"],
                     "avg_round_us": round_ms * 1e3 / max(prof["rounds"], 1), "launches_timed": launches,
                     "us_per_pair_round": round_ms * 1e3 / prof["pair_rounds"],
                     "share_of_step": round_ms / prof["ms"],
-                    "working_set": f"{per_gpu} pairs in flight x {117 * N / 1e6:.1f} MB of per-pair workspace + {len(needed)} clouds x {(16 + 48 + 8) * N / 1e6:.1f} MB >> 126 MB L2"}
+                    "working_set": f"{per_gpu} pairs in flight x {117 * N / 1e6:.1f} MB of per-pair workspace + {len(needed)} clouds x {(16 + 48 + 8) * N / 1e6:.1f} MB >> 50 MB L2"}
     kernel_ms = {k: round(v, 3) for k, v in st["ms"].items() if v > 0}
+    if getattr(args, "dump_outputs", None):  # every pair's gathered record of the last timed pass + the per-group best candidate
+        bench.dump_outputs(args.dump_outputs, {
+            "T": np.array([np.array(res[i].T, np.float32).reshape(4, 4).T for i in range(n_pairs)], np.float32),
+            "fitness": [res[i].fitness for i in range(n_pairs)], "converged": [res[i].converged for i in range(n_pairs)],
+            "iterations": [res[i].iterations for i in range(n_pairs)], "best": rv["best"]})
     line = {
         "metric": "registrations/sec", "value": value, "unit": "registrations/s", "n_gpus": world, "steps": K, "warmup": W,
         "ms_per_step": rv["ms"] / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -289,7 +294,7 @@ def run_loop_batch(args, rank, world, local_rank, quiet=False):
                    "unique_clouds_per_gpu": len(needed),
                    "shards": ("distinct keyframe groups per rank (per-GPU work varies with the shard's iteration counts)" if distinct else
                               "every rank's shard is the same keyframe groups and guesses: per-GPU work exactly fixed (weak scaling); --distinct-shards gives every rank "
-                              "different places of the circuit, where the MAX over ranks follows the heaviest shard (r2i: 2 x B200 = 1.65 x with identical kernel time on rank 0)"), "cloud_cache": "each keyframe cloud is uploaded and preprocessed once per pass and shared by the pairs that name it",
+                              "different places of the circuit, where the MAX over ranks follows the heaviest shard"), "cloud_cache": "each keyframe cloud is uploaded and preprocessed once per pass and shared by the pairs that name it",
                    "step": "one pass = register the rank's keyframe clouds (upload + search structure + covariances), align + fitness of all its pairs, one ncclAllGather, argmin",
                    "collective": "one ncclAllGather of 80-byte records, issued by libb200reg (in-library NCCL)", "fitness_max_range": max_range,
                    "l2": "inputs larger than L2: a pass streams the rank's keyframe clouds (2 MiB each) and ~7.7 MB of workspace per pair",

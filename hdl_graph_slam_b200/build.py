@@ -1,6 +1,6 @@
 """In-tree build of the engine's native libraries (no JIT cache: the .so files travel with the repo snapshot).
 
-  _lib/libb200reg.so     CUDA engine + C ABI (sm_100a)                 <- csrc/api.cu
+  _lib/libb200reg.so     CUDA engine + C ABI (sm_90a)                  <- csrc/api.cu
   _lib/libb2r_synth.so   synthetic LiDAR workload generator (C/OpenMP)  <- synth/lidar_synth.c
 """
 import os
@@ -10,7 +10,7 @@ import shutil
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "_lib")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 

@@ -92,7 +92,7 @@ struct b2r_handle {
   int* pf_h_total = nullptr; int* pf_h_total_dev = nullptr;
   BuildCtx bc[2];                   // per-stream build scratch (main stream, prefetch stream)
   bool knn_smem_attr = false, stat_smem_attr = false;
-  int n_sm = 148;
+  int n_sm = 132;
   // last result
   float final_T[16];                // row-major
   bool has_final = false;
@@ -106,7 +106,7 @@ static Cloud& SRC(b2r_handle* h) { return h->clouds[h->src]; }
 static Cloud& TGT(b2r_handle* h) { return h->clouds[h->tgt]; }
 
 extern "C" const char* b2r_last_error(void) { return g_last_error.c_str(); }
-extern "C" const char* b2r_version(void) { return "b200reg 0.1 (sm_100a)"; }
+extern "C" const char* b2r_version(void) { return "b200reg 0.1 (sm_90a)"; }
 
 extern "C" int b2r_config_default(b2r_config* c, int method) {
   if (!c) return fail(B2R_EINVAL, "cfg is NULL");
@@ -191,7 +191,7 @@ extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
   }
   auto bail = [&](int code) { b2r_destroy(h); return code; };
   cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, cfg->device_id);
-  if (h->n_sm <= 0) h->n_sm = 148;
+  if (h->n_sm <= 0) h->n_sm = 132;
   {  // the align path (latency-critical chain of small kernels) outranks the prefetch path (throughput work for the NEXT frame)
     int lo = 0, hi = 0;
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
@@ -488,8 +488,8 @@ static int build_cov(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
     TEL_BEGIN(&h->tel, st);
     if (k == kKnnRegK) {  // the reference's default reg_correspondence_randomness: lists live in registers
       // On the PREFETCH stream the kernel works for the NEXT frame while the align chain of the current one runs beside it.  All of its
-      // 512 blocks become resident at once (104 registers x 128 threads x 3.5 blocks per SM = 70 % of the register file) and stay for
-      // ~170 us — stream priorities only order PENDING blocks, so the chain's search kernels then run in the remaining third of each SM.
+      // 512 blocks become resident at once (104 registers x 128 threads x ~3.9 blocks per SM on 132 SMs = 80 % of the register file) and
+      // stay for the kernel's whole run — stream priorities only order PENDING blocks, so the chain's search kernels then run in what is left of each SM.
       // Capping the prefetch kernel's residency with unused dynamic shared memory keeps most of every SM for the chain.
       static const int cap = [] { const char* e = getenv("B2R_PREFETCH_KNN_BLOCKS"); return e ? atoi(e) : B2R_PREFETCH_KNN_BLOCKS_DEFAULT; }();
       size_t pad_smem = 0;
@@ -799,7 +799,7 @@ static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, co
     // The source's covariances do not exist yet (strict call-by-call chain: no prefetch).  The first round's correspondence search
     // reads only the source's sorted points and the target's structure, so it runs on the SECOND (low-priority) stream while the
     // k-NN covariance kernel runs on the main one: that kernel's grid is under one wave with a long tail of single heavy warps
-    // (profiles/r01_g), and the search's blocks fill the SMs as its blocks retire.  The accumulate kernel, the first reader of the
+    // and the search's blocks fill the SMs as its blocks retire.  The accumulate kernel, the first reader of the
     // covariances, waits for both.
     B2R_CUDA(cudaEventRecord(h->ev_fork, h->st));  // behind the structure build and whatever the previous align left on the main stream
     B2R_CUDA(cudaStreamWaitEvent(h->st2, h->ev_fork, 0));
@@ -1404,7 +1404,7 @@ static int ingest_device(b2r_handle* h, const unsigned char* d_blob, size_t n, c
   A.data = d_blob; A.n = (long long)n; A.point_step = L.point_step; A.off_x = L.off_x; A.off_y = L.off_y; A.off_z = L.off_z;
   A.off_i = L.off_intensity; A.type_i = L.intensity_datatype; A.bigendian = L.is_bigendian; A.out = h->ingest_out.p;
   { TEL_BEGIN(&h->tel, h->st);
-    k_unpack_points<<<(unsigned)std::min<size_t>((n + 255) / 256, 148 * 16), 256, 0, h->st>>>(A);
+    k_unpack_points<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)h->n_sm * 16), 256, 0, h->st>>>(A);
     TEL_END(&h->tel, KC_MISC, 1, h->st); }
   B2R_CUDA(cudaGetLastError());
   *d_out = h->ingest_out.p;
@@ -1542,7 +1542,7 @@ extern "C" int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot
   B2R_CUDA(cudaMemcpyAsync(h->map_kf.p, kf2.data(), kf2.size() * sizeof(MapKf), cudaMemcpyHostToDevice, st));
   B2R_CUDA(cudaStreamSynchronize(st));  // kf2 is pageable host memory on the stack of this call
   const long long T = (long long)total;
-  unsigned nb = (unsigned)std::min<size_t>((total + 255) / 256, 148 * 16);
+  unsigned nb = (unsigned)std::min<size_t>((total + 255) / 256, (size_t)h->n_sm * 16);
   { TEL_BEGIN(&h->tel, st);
     k_map_transform<<<nb, 256, 0, st>>>(reinterpret_cast<const MapKf*>(h->map_kf.p), (int)kf2.size(), sf, T, cloud.p);
     TEL_END(&h->tel, KC_MISC, 1, st); }

@@ -23,7 +23,7 @@ struct b2r_batch {
   std::vector<Cloud*> recycled;  // removed clouds keep their device buffers for the next add (no cudaMalloc churn per keyframe)
   // pair slots.  A chunk of pairs can be split over kLanes independent round sequences ("lanes"), each on its own stream, so that a
   // lane's search kernel (instruction-issue bound) runs beside the other lane's accumulate kernel and a lane's thin tail rounds
-  // overlap the other's fat ones.  Measured on B200 (256 pairs x 64k points): 6688 pairs/s with two lanes, 6713 with one — the block
+  // overlap the other's fat ones.  Two lanes did not beat one on 256 pairs x 64k points — the block
   // scheduler drains one kernel's grid before it starts the next stream's, so the overlap is confined to the tails; the default
   // is ONE lane (B2R_BATCH_LANES=2 enables the second).  Lane 0 runs on the engine's main stream.
   static constexpr int kLanes = 2;

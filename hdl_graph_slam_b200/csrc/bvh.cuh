@@ -6,7 +6,7 @@
 //
 // Structure (per cloud): points sorted by (30-bit Hilbert key, original index); leaf L = sorted[32L .. 32L+31] with a tight
 // AABB; super-node S = leaves [32S .. 32S+31] with a tight AABB.  LiDAR density varies by 3 orders of magnitude between the
-// near and the far field; fixed-size leaves adapt to it (profiles/r01_b shows why a uniform grid does not).
+// near and the far field; fixed-size leaves adapt to it (a uniform grid does not).
 //
 // Search = "warp group": the 32 lanes of a warp hold 32 queries that are neighbours in space (a leaf of the query cloud).
 // A leaf of the target is visited if ANY lane still needs it; its 32 points are then tested by all lanes (all-pairs tile).
@@ -278,7 +278,7 @@ __global__ void __launch_bounds__(1024) k_bvh_leaves(const float* __restrict__ r
 
 // ------------------------------------------------------------------------------------------------ warp-group traversal
 // Group-level masks are cheap but only as good as the group's box: a group that straddles a jump of the Hilbert curve has a box
-// of tens of metres and would send every leaf in range to bvh_try_leaf (profiles/r01_g: one such warp, 900 leaf tests, set the
+// of tens of metres and would send every leaf in range to bvh_try_leaf (one such warp, with hundreds of leaf tests, can set the
 // kernel time).  When a group mask keeps more than kRefineAbove nodes, every lane re-tests the survivors against ITS OWN query
 // (uniform loads, no ballot in the loop) and the warp keeps the union.
 constexpr int kRefineAbove = 4;
@@ -302,7 +302,7 @@ __device__ __forceinline__ unsigned refine_node_mask(unsigned gmask, const float
 // All 32 lanes call this together.  Lane l holds query (qx,qy,qz) (active) and its own visitor.
 //   own_leaf >= 0 : the queries ARE that leaf of this same structure (k-NN of a cloud against itself): visited first.
 // Order: own leaf, then the super-node nearest to the group's AABB, then all remaining super-nodes by index.
-// Visit one leaf for the lanes flagged `pass`.  Two modes (profiles/r01_c: a Morton leaf at a curve discontinuity can
+// Visit one leaf for the lanes flagged `pass`.  Two modes (a Morton leaf at a curve discontinuity can
 // span 100 m; its 32 queries then want DIFFERENT leaves and a pure all-pairs tile wastes 31/32 of the work):
 //   tile mode  (>= kTileLanes lanes interested): every lane tests all 32 candidates (broadcast loads);
 //   coop mode  (few lanes interested): for each interested lane L the 32 lanes evaluate the leaf's 32 candidates in ONE
@@ -311,7 +311,7 @@ __device__ __forceinline__ unsigned refine_node_mask(unsigned gmask, const float
 
 // C > 1: the warp carries Q = 32/C queries; lanes q, q+Q, q+2Q, ... hold the SAME query and identical visitor state between
 // visits.  In tile mode each copy scans 1/C of the leaf and the copies merge afterwards: C times the warps, 1/C of the chain per
-// warp — the searches are latency-bound and their kernel time is the slowest warp, i.e. the heaviest query (profiles/r01_g).
+// warp — the searches are latency-bound and their kernel time is the slowest warp, i.e. the heaviest query.
 // Candidates and tie rule are unchanged, so results are identical.
 template <int C = 1, class Visitor>
 __device__ __forceinline__ bool bvh_visit_leaf(const Bvh& b, int l, float qx, float qy, float qz, bool pass, Visitor& v) {
@@ -335,7 +335,7 @@ __device__ __forceinline__ bool bvh_visit_leaf(const Bvh& b, int l, float qx, fl
 #endif
   if (__popc(mask) >= kTile) {
     // (dynamic regrouping of sparse visits — the r-th interested query served by 2 or 4 adjacent lanes sweeping a half / a quarter of the
-    // leaf each — is exact but measured neutral out of line and 44 % slower inlined at every visit site: profiles/r02_ac, r02_ad)
+    // leaf each — is exact but was no faster out of line and slower inlined at every visit site)
     if constexpr (C > 1) {
       const int t0 = (lane / Q) * (kLeaf / C);
       if constexpr (keyed_visitor<Visitor>::value) {
@@ -378,8 +378,8 @@ __device__ __forceinline__ bool bvh_visit_leaf(const Bvh& b, int l, float qx, fl
       }
     } else {
       // (a minimum-first variant — one sweep that keeps only the smallest distance, the exact (d2, index) sweep only when some lane can
-      // improve — was measured: neutral on the 4-lane odometry search, 15 % slower on the 1-lane batch search, where some lane of
-      // the 32 nearly always needs the second sweep: profiles/r02_n)
+      // improve — was no faster on the 4-lane odometry search and slower on the 1-lane batch search, where some lane of
+      // the 32 nearly always needs the second sweep)
       if constexpr (keyed_visitor<Visitor>::value) {
         unsigned long long k = v.tile_begin(pass);
 #pragma unroll Visitor::kTileUnroll
@@ -517,7 +517,7 @@ __device__ __forceinline__ void bvh_group_search(const Bvh& b, float qx, float q
   // pass 1: the window of 32 leaves CENTRED on the already-visited leaf, in order of index distance from it (Hilbert order:
   // index neighbours are space neighbours), so the bound is tight before anything else is looked at.  The window ignores
   // super-node borders: a leaf that straddles a jump of the curve at the end of its super-node has half of its true
-  // neighbours in the next one (profiles/r01_g: that leaf alone set the kernel time).
+  // neighbours in the next one (such a leaf alone can set the kernel time).
   int win0 = -1;  // first leaf of the pass-1 window
   if (own_leaf >= 0) {
     win0 = own_leaf - kSuper / 2;

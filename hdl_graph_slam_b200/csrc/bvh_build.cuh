@@ -5,7 +5,7 @@
 // 172,177,246 and /root/reference/include/hdl_graph_slam/loop_detector.hpp:122,136) — and, in this engine, a chain of eleven
 // launches (bbox, fill, keys, six cub::DeviceRadixSort kernels, leaves).
 //
-// B200-first design: a cloud of up to 131 072 points lives ENTIRELY in the distributed shared memory of one cluster
+// Design: a cloud of up to 131 072 points lives ENTIRELY in the distributed shared memory of one cluster
 // (CL = 1/2/4/8 CTAs x PER = 1..16 (key, index) pairs per thread, at most 128 KB per CTA).  The cluster computes the bounding box, the 30-bit Hilbert
 // keys, runs a stable 4-pass LSD radix sort whose scatter writes straight into the PEER CTAs' shared memory (DSMEM stores,
 // cluster barriers between passes — no global-memory round trip, no histogram/offset kernels), and finally each CTA emits its
@@ -26,8 +26,7 @@ constexpr int kBuildMaxPer = 16;                        // (key, index) pairs pe
 constexpr int kBuildMaxPoints = 8 * kBuildMaxPer * kBuildThreads;  // 131 072: the largest cloud a cluster of 8 holds
 // PER pairs per thread => a CTA holds PER * 1024 pairs.  The kernels are latency bound (one cluster per cloud), so a cloud is spread over
 // as MANY CTAs as the portable cluster size allows (8) with as FEW pairs per thread as that needs: 65 536 points = 8 CTAs x 8 per
-// thread, 24 000 points = 8 x 4 (measured phase cycles, profiles/r02_o_build_phase_cycles.txt: every phase except the barriers scales
-// with the pairs per thread).
+// thread, 24 000 points = 8 x 4 (every phase except the barriers scales with the pairs per thread).
 template <int PER>
 struct BuildGeom {
   static_assert(PER == 1 || PER == 2 || PER == 4 || PER == 8 || PER == 16, "pairs per thread: a power of two up to 16");
@@ -165,8 +164,8 @@ __device__ __forceinline__ void cluster_radix_sort(cg::cluster_group& cluster, c
     // every warp ranks its own contiguous 32 * PER elements in order, 32 at a time: rank inside (warp, digit) = running count of the
     // digit in this warp + number of equal digits in lower lanes (stable).  The MATCH.ANY of a step does not depend on the running
     // counts, so the masks of up to 8 steps are taken first (independent, pipelined) and only the count updates — a shared-memory
-    // read-modify-write by the digit's leader lane — run one after the other (measured: the serial match + update chain was 13 us
-    // of a 31 us pass at 16 pairs per thread).
+    // read-modify-write by the digit's leader lane — run one after the other (the serial match + update chain was a large share of a pass
+    // at 16 pairs per thread).
     uint2 e[PER];
     unsigned short off[PER];
     unsigned short* mywh = wh + warp * 256;

@@ -1,4 +1,4 @@
-// common.cuh — shared definitions of the B200 scan-matching engine (libb200reg).
+// common.cuh — shared definitions of the scan-matching engine (libb200reg).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

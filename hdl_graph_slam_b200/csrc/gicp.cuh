@@ -1,6 +1,6 @@
 // gicp.cuh — GICP kernels: k-NN covariances, and the block / grid reductions shared by every reducing kernel.
 //
-// Re-creates, B200-first, the arithmetic of fast_gicp::FastGICP (SURVEY.md A.4) that the reference selects at
+// Re-creates, GPU-first, the arithmetic of fast_gicp::FastGICP (SURVEY.md A.4) that the reference selects at
 // /root/reference/src/hdl_graph_slam/registrations.cpp:27-36 and runs from apps/scan_matching_odometry_nodelet.cpp:177,210
 // and include/hdl_graph_slam/loop_detector.hpp:136,143:
 //   k_knn_cov_reg<20>  <- FastGICP::calculate_covariances (k = 20 exact NN in registers, PLANE regularisation); k_knn_cov: any k
@@ -16,7 +16,7 @@ namespace b2r {
 
 constexpr int kKnnThreads = 128;
 // resident blocks per SM: the single-cloud kernel is bound by its slowest warp (4 blocks, 104 registers, no spills); the batched one by
-// throughput (5 blocks, 96 registers: +4 % on the k-NN share of the loop batch, profiles/r02_y; the same setting costs the odometry chain 2 %)
+// throughput (5 blocks, 96 registers: faster on the k-NN share of the loop batch; the same setting slows the odometry chain)
 #ifndef B2R_KNN_MINBLOCKS
 #define B2R_KNN_MINBLOCKS 4
 #endif
@@ -147,7 +147,7 @@ __global__ void __launch_bounds__(kKnnThreads, 4) k_knn_cov(Bvh b, int k, const 
   }, cov + (size_t)s * 6);
 }
 
-// ---- register-resident lists (K fixed at compile time).  profiles/r01_g: with the lists in shared memory a warp spends ~400
+// ---- register-resident lists (K fixed at compile time).  With the lists in shared memory a warp spends hundreds of
 // cycles per candidate step, the latency of a data-dependent LDS -> compare -> STS chain (max over lanes of the shift count);
 // in registers every slot is recomputed branch-free from the OLD neighbours (new[j] = old[j-1] > q ? old[j-1] : old[j] > q ? q :
 // old[j]), so the K slot updates are independent instructions.  Same candidates, same (d2, idx) order => identical lists.

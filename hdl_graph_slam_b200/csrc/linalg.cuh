@@ -67,7 +67,7 @@ B2R_HD void sym_eigen3(const double* Ain, double* w, double* V) {
 // root that is well separated — the smallest when det(B) <= 0, the largest otherwise.  In the first case the wanted vector is
 // the best-conditioned cross product of two rows of (A - lambda0 I).  In the second case the largest eigenvector is deflated
 // and the remaining 2x2 problem in its orthogonal complement is solved by one exact Jacobi rotation.
-// ~250 flops against ~6 sweeps of 3x3 Jacobi (profiles/r01_e: the iterative solver was 30 % of k_knn_cov's instructions).
+// ~250 flops against ~6 sweeps of 3x3 Jacobi (the iterative solver was a large share of k_knn_cov's instructions).
 B2R_HD void sym_cross_eigvec3(double a00, double a01, double a02, double a11, double a12, double a22, double lam, double* v) {
   const double m00 = a00 - lam, m11 = a11 - lam, m22 = a22 - lam;
   const double x0 = a01 * a12 - a02 * m11, y0 = a02 * a01 - m00 * a12, z0 = m00 * m11 - a01 * a01;  // r0 x r1

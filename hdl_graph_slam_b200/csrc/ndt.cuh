@@ -1,6 +1,6 @@
 // ndt.cuh — NDT kernels and host driver.
 //
-// Re-creates, B200-first, pclomp::NormalDistributionsTransform + pclomp::VoxelGridCovariance (koide3/ndt_omp; SURVEY.md
+// Re-creates, GPU-first, pclomp::NormalDistributionsTransform + pclomp::VoxelGridCovariance (koide3/ndt_omp; SURVEY.md
 // A.2/A.3) — the reference factory's default engine (/root/reference/src/hdl_graph_slam/registrations.cpp:26,101-120):
 //   ndt_build_map (k_vox_*)   <- setInputTarget -> VoxelGridCovariance::filter/applyFilter (voxel Gaussians: mean, cov, icov)
 //   k_ndt_derivatives         <- computeDerivatives + computePointDerivatives + updateDerivatives, DIRECT1 / DIRECT7
@@ -301,12 +301,12 @@ __device__ __forceinline__ int ndt_find(const unsigned long long* __restrict__ t
 // counter (a resident block takes the next chunk when it is done with its own), every chunk reduces to its OWN row of 43
 // float64 sums, and the rows are added by a fixed two-level tree (32 chunk rows -> one group row by whichever block completes
 // the group, group rows -> result by whichever block completes the last group).  The sums therefore do not depend on which
-// block processed which chunk — bitwise reproducible — while no SM waits for a statically assigned heavy block (ncu, static
-// persistent grid: slowest SM sub-partition 99 k cycles against a mean of 56 k, a quarter of it the single last block adding 592
-// rows of partials in 38 dependent memory round trips; profiles/r02_t).
-// (Measured and dropped, profiles/r02_w: fully warp-autonomous 32-point sub-chunks with warp tickets and a three-level tree — no block
-// barrier at all — 40.1 us per pass against 36.9 us for this version: the barrier stalls turn into long-scoreboard and fence stalls, and
-// the tail does not shrink because it is set by work units per resident slot (1.73 in both versions), not by the unit's size.)
+// block processed which chunk — bitwise reproducible — while no SM waits for a statically assigned heavy block (with a static
+// persistent grid the slowest SM sub-partition ran far longer than the mean, much of it the single last block adding its rows of
+// partials in a chain of dependent memory round trips).
+// (Tried and dropped: fully warp-autonomous 32-point sub-chunks with warp tickets and a three-level tree — no block barrier at
+// all — was slower per pass than this version: the barrier stalls turn into long-scoreboard and fence stalls, and the tail does
+// not shrink because it is set by work units per resident slot, not by the unit's size.)
 constexpr int kNdtRow = 136;  // float64 elements per shared-memory row of per-thread values (128 + 8: half-warps hit distinct banks)
 
 // sums of R (<= 16) rows of 128 per-thread values -> dst[0..R): thread (row = tid >> 3, part = tid & 7) adds the elements part,
@@ -946,7 +946,7 @@ inline unsigned ndt_resident_blocks(bool hess) {
   static unsigned cached[2] = {0, 0};
   unsigned& c = cached[hess ? 1 : 0];
   if (c == 0) {
-    int dev = 0, sms = 148, per = 4;
+    int dev = 0, sms = 132, per = 4;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (hess) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_ndt_derivatives<true>, kNdtThreads, 0);

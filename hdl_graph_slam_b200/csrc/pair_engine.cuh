@@ -5,7 +5,7 @@
 // /root/reference/apps/scan_matching_odometry_nodelet.cpp:210 and /root/reference/include/hdl_graph_slam/loop_detector.hpp:143,
 // plus the `getFitnessScore(max_range)` that follows every loop-closure align (loop_detector.hpp:146).
 //
-// Design (B200-first, SURVEY.md §0.5 / §7 "iteration control on device"):
+// Design (GPU-first, SURVEY.md §0.5 / §7 "iteration control on device"):
 //   * every pair in flight owns a PairDev record in HBM: the two clouds' search structures, its double-buffered
 //     correspondence sets, and the COMPLETE Levenberg-Marquardt state (pose, H, b, lambda, nu, counters);
 //   * ONE round = three launches that cover ALL active pairs (blockIdx.y = slot): k_pair_search (exact seeded 1-NN of every
@@ -360,7 +360,7 @@ __device__ __forceinline__ void red_emit(double v, double* tile, double* red, in
 // linearize (float64) at xe into the write set + compute_error of the previous set, per active pair.  Every block leaves its
 // 29 partial sums in the pair's `partials`; k_pair_lm (next launch) adds them in a fixed order and takes the LM step.
 #ifndef B2R_ACC_MINBLOCKS
-#define B2R_ACC_MINBLOCKS 4  // 64 registers, 32 warps per SM: the pass is bound by gather latency (profiles/r02_x: 33.2 -> 28.0 ms per 5 passes of 256 pairs)
+#define B2R_ACC_MINBLOCKS 4  // 64 registers, 32 warps per SM: the pass is bound by gather latency
 #endif
 __global__ void __launch_bounds__(kAccThreads, B2R_ACC_MINBLOCKS) k_pair_accumulate(PairDev* pairs, const int* __restrict__ active, const __grid_constant__ LmCfg cfg) {
   __shared__ double red[kAcc * 8];

@@ -1,4 +1,4 @@
-/* b200reg.h — C ABI of libb200reg.so, the B200-native scan-matching engine that drops in behind the
+/* b200reg.h — C ABI of libb200reg.so, the GPU-native (H100, sm_90a) scan-matching engine that drops in behind the
  * pcl::Registration<pcl::PointXYZI, pcl::PointXYZI> handle of koide3/hdl_graph_slam.
  *
  * Every entry point names the reference interface it replaces (paths relative to /root/reference).  The seam is

@@ -8,7 +8,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 _HAS_GPU = None
@@ -39,7 +39,7 @@ def pytest_collection_modifyitems(config, items):
     if not gpu_items:
         return
     if not has_gpu():
-        skip = pytest.mark.skip(reason="no CUDA device in this container (run under gpurun)")
+        skip = pytest.mark.skip(reason="no CUDA device on this machine")
         for it in gpu_items:
             it.add_marker(skip)
 

@@ -116,3 +116,44 @@ def test_clock_sampler_window_and_hold(tmp_path, monkeypatch):
     out = s.stop()
     assert out["samples"] == 2 and out["sm_mhz"] == 1957.5 and out["sm_max_mhz"] == 1965.0 and out["reasons"] == ["sw_power_cap"]
     assert "untimed steps" in out["window"]
+
+
+def test_dump_outputs_writes_the_callers_arrays(tmp_path):
+    """odometry status -> one .npy per field a caller gets; poses as 4x4, float64 scalars; the NaN-only status fields left out"""
+    import numpy as np
+    b = _bench()
+    T = np.arange(16, dtype=np.float64).reshape(4, 4)
+    status = dict(odom=T, trans=T + 1, converged=True, iterations=5, keyframe_updated=False, frame_rejected=False,
+                  matching_error=float("nan"), inlier_fraction=float("nan"))
+    b.dump_outputs(str(tmp_path / "d"), b.odometry_outputs(status))
+    names = sorted(p.name for p in (tmp_path / "d").iterdir())
+    assert names == ["converged.npy", "frame_rejected.npy", "iterations.npy", "keyframe_updated.npy", "odom.npy", "trans.npy"]
+    odom = np.load(tmp_path / "d" / "odom.npy")
+    assert odom.dtype == np.float64 and np.array_equal(odom, T)
+    assert np.load(tmp_path / "d" / "iterations.npy").dtype == np.float64 and float(np.load(tmp_path / "d" / "iterations.npy")) == 5.0
+    cloud = np.ones((3, 8), np.float32)  # float32 outputs (clouds, batch poses) stay float32
+    b.dump_outputs(str(tmp_path / "c"), {"cloud": cloud})
+    assert np.load(tmp_path / "c" / "cloud.npy").dtype == np.float32
+
+
+def test_dump_outputs_refuses_more_than_64_mb(tmp_path):
+    import numpy as np
+    import pytest
+    b = _bench()
+    with pytest.raises(ValueError):
+        b.dump_outputs(str(tmp_path / "d"), {"big": np.zeros(b.DUMP_LIMIT_BYTES // 8 + 1, np.float64)})
+    assert not (tmp_path / "d").exists()
+
+
+def test_steps_argument_is_the_number_of_timed_steps():
+    import pytest
+    b = _bench()
+    r = lambda argv, world=1: b.resolve_args(b.parse(argv), world)  # noqa: E731
+    assert r(["--workload", "loop_batch", "--steps", "200"]).steps == 200
+    assert r(["--steps", "7"]).steps == 7 and r(["--steps", "7"]).workload == "gicp_odometry_vlp16_64k"
+    assert r(["--gpus", "2", "--steps", "200"], world=2).steps == 200
+    assert r(["--workload", "loop_batch"]).steps == 5 and r([]).steps == 200
+    assert r(["--gpus", "2"], world=2).workload == "loop_batch"
+    assert r(["--workload", "voxelgrid", "--dump-outputs", "x"]).dump_outputs == "x"
+    with pytest.raises(SystemExit):
+        r(["--impl", "reference", "--dump-outputs", "x"])

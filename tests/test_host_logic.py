@@ -93,7 +93,7 @@ def test_result_message_protocol(tmp_path):
 def lm_harness(oracle):
     os.makedirs(os.path.join(ROOT, "build"), exist_ok=True)
     exe = os.path.join(ROOT, "build", "lm_harness")
-    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-w", "-gencode", "arch=compute_100a,code=sm_100a", "-ccbin", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++",
+    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-w", "-gencode", "arch=compute_90a,code=sm_90a", "-ccbin", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++",
                            "-Xcompiler", "-ffp-contract=off", "-o", exe, os.path.join(ROOT, "tests", "lm_harness.cu"),
                            "-L" + os.path.join(ROOT, "oracle"), "-loracle", "-Xlinker", "-rpath=" + os.path.join(ROOT, "oracle")])
     return exe
