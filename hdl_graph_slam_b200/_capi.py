@@ -115,6 +115,7 @@ SYMBOLS = [
     ("b2r_gicp_error_at", C.c_int, [_VP, _F64P, _F64P]),
     ("b2r_ndt_get_voxels", C.c_int, [_VP, _SZ, C.POINTER(_SZ), C.POINTER(C.c_int64), _I32P, _F64P, _F64P, _I32P, _I32P]),
     ("b2r_ndt_derivatives_at", C.c_int, [_VP, _F64P, _F64P, _F64P, _F64P, C.POINTER(C.c_uint64)]),
+    ("b2r_ndt_hessian_at", C.c_int, [_VP, _F64P, _F64P]),
     ("b2r_voxelgrid", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_float, _VP, C.POINTER(_SZ), _I32P, _I32P]),
     ("b2r_voxelgrid_device", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_float, C.POINTER(_VP), C.POINTER(_SZ)]),
     ("b2r_distance_filter", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_double, C.c_double, _VP, C.POINTER(_SZ)]),

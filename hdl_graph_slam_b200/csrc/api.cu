@@ -1134,6 +1134,18 @@ extern "C" int b2r_ndt_derivatives_at(b2r_handle* h, const double p[6], double* 
   return ndt_derivatives_at(h->cfg, SRC(h), TGT(h), h->ndt_work, h->st, p, score, g, H, n_pairs);
 }
 
+extern "C" int b2r_ndt_hessian_at(b2r_handle* h, const double p[6], double* H) {
+  if (!h || !p || !H) return fail(B2R_EINVAL, "NULL argument");
+  if (h->cfg.method != B2R_METHOD_NDT) return fail(B2R_ESTATE, "NDT engine required");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (SRC(h).n == 0 || TGT(h).n == 0) return fail(B2R_ESTATE, "source/target not set");
+  int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
+  if (rc) return rc;
+  rc = ensure_grid(h, SRC(h));
+  if (rc) return rc;
+  return ndt_hessian_at(h->cfg, SRC(h), TGT(h), h->ndt_work, h->st, p, H);
+}
+
 extern "C" int b2r_voxelgrid(b2r_handle* h, const void* in, size_t n, size_t stride_bytes, float leaf, void* out, size_t* n_out,
                              int32_t* out_keys, int32_t* out_counts) {
   if (!h || !n_out || (n && (!in || !out))) return fail(B2R_EINVAL, "NULL argument");

@@ -50,6 +50,28 @@ B2R_HD float fsub(float a, float b) {
   volatile float r = a - b; return r;
 #endif
 }
+// the same for float64 (the NDT voxel finalisation follows the oracle's unfused operation order to the last bit)
+B2R_HD double dmul(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  volatile double r = a * b; return r;
+#endif
+}
+B2R_HD double dadd(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dadd_rn(a, b);
+#else
+  volatile double r = a + b; return r;
+#endif
+}
+B2R_HD double dsub(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dsub_rn(a, b);
+#else
+  volatile double r = a - b; return r;
+#endif
+}
 B2R_HD float dist2_f32(float qx, float qy, float qz, float px, float py, float pz) {
   float dx = fsub(qx, px), dy = fsub(qy, py), dz = fsub(qz, pz);
   return fadd(fadd(fmul(dx, dx), fmul(dy, dy)), fmul(dz, dz));

@@ -11,13 +11,17 @@ struct Sym3 {
 };
 
 // Cyclic Jacobi eigen-decomposition of a symmetric 3x3 (A row-major full).  w ascending, V columns = eigenvectors.
+// The NDT voxel finalisation decides validity on the sign of the smallest eigenvalue, which for an exactly planar or linear
+// voxel is rounding noise around 0; so this solver reproduces the oracle's orc::sym_eigen<3> bit for bit: the same sweep cap
+// (64), the same unfused operation order (dmul / dadd / dsub: no FMA contraction on the device) and the same selection sort
+// (it places tied eigenvalues' columns differently from a sorting network).
 B2R_HD void sym_eigen3(const double* Ain, double* w, double* V) {
   double A[9];
 #pragma unroll
   for (int i = 0; i < 9; i++) A[i] = Ain[i];
   V[0] = 1; V[1] = 0; V[2] = 0; V[3] = 0; V[4] = 1; V[5] = 0; V[6] = 0; V[7] = 0; V[8] = 1;
-  for (int sweep = 0; sweep < 32; sweep++) {
-    double off = A[1] * A[1] + A[2] * A[2] + A[5] * A[5];
+  for (int sweep = 0; sweep < 64; sweep++) {
+    const double off = dadd(dadd(dmul(A[1], A[1]), dmul(A[2], A[2])), dmul(A[5], A[5]));
     if (off == 0.0) break;
 #pragma unroll
     for (int pq = 0; pq < 3; pq++) {
@@ -26,39 +30,42 @@ B2R_HD void sym_eigen3(const double* Ain, double* w, double* V) {
       double apq = A[p * 3 + q];
       if (apq == 0.0) continue;
       double app = A[p * 3 + p], aqq = A[q * 3 + q];
-      double theta = (aqq - app) / (2.0 * apq);
-      double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-      double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+      double theta = dsub(aqq, app) / dmul(2.0, apq);
+      double t = (theta >= 0 ? 1.0 : -1.0) / dadd(fabs(theta), sqrt(dadd(dmul(theta, theta), 1.0)));
+      double c = 1.0 / sqrt(dadd(dmul(t, t), 1.0)), s = dmul(t, c);
 #pragma unroll
       for (int k = 0; k < 3; k++) {
         double akp = A[k * 3 + p], akq = A[k * 3 + q];
-        A[k * 3 + p] = c * akp - s * akq;
-        A[k * 3 + q] = s * akp + c * akq;
+        A[k * 3 + p] = dsub(dmul(c, akp), dmul(s, akq));
+        A[k * 3 + q] = dadd(dmul(s, akp), dmul(c, akq));
       }
 #pragma unroll
       for (int k = 0; k < 3; k++) {
         double apk = A[p * 3 + k], aqk = A[q * 3 + k];
-        A[p * 3 + k] = c * apk - s * aqk;
-        A[q * 3 + k] = s * apk + c * aqk;
+        A[p * 3 + k] = dsub(dmul(c, apk), dmul(s, aqk));
+        A[q * 3 + k] = dadd(dmul(s, apk), dmul(c, aqk));
       }
 #pragma unroll
       for (int k = 0; k < 3; k++) {
         double vkp = V[k * 3 + p], vkq = V[k * 3 + q];
-        V[k * 3 + p] = c * vkp - s * vkq;
-        V[k * 3 + q] = s * vkp + c * vkq;
+        V[k * 3 + p] = dsub(dmul(c, vkp), dmul(s, vkq));
+        V[k * 3 + q] = dadd(dmul(s, vkp), dmul(c, vkq));
       }
     }
   }
   w[0] = A[0]; w[1] = A[4]; w[2] = A[8];
-  // sort ascending (3-element network), permuting columns
+  // selection sort ascending (first minimum wins), permuting columns; written with constant indices so w / V stay in registers
 #define B2R_SWAPCOL(a, b)                                  \
-  if (w[b] < w[a]) {                                       \
+  {                                                        \
     double tw = w[a]; w[a] = w[b]; w[b] = tw;              \
     for (int k = 0; k < 3; k++) { double tv = V[k * 3 + a]; V[k * 3 + a] = V[k * 3 + b]; V[k * 3 + b] = tv; } \
   }
-  B2R_SWAPCOL(0, 1)
-  B2R_SWAPCOL(1, 2)
-  B2R_SWAPCOL(0, 1)
+  if (w[1] < w[0]) {
+    if (w[2] < w[1]) B2R_SWAPCOL(0, 2) else B2R_SWAPCOL(0, 1)
+  } else if (w[2] < w[0]) {
+    B2R_SWAPCOL(0, 2)
+  }
+  if (w[2] < w[1]) B2R_SWAPCOL(1, 2)
 #undef B2R_SWAPCOL
 }
 
@@ -152,6 +159,75 @@ B2R_HD void mul3(const double* a, const double* b, double* o) {
   for (int i = 0; i < 3; i++)
 #pragma unroll
     for (int j = 0; j < 3; j++) o[i * 3 + j] = a[i * 3 + 0] * b[0 * 3 + j] + a[i * 3 + 1] * b[1 * 3 + j] + a[i * 3 + 2] * b[2 * 3 + j];
+}
+
+// inv3 / mul3 in the same formulas, unfused (the NDT voxel finalisation; inv3 / mul3 above stay as they are on the GICP path)
+B2R_HD double inv3_rn(const double* m, double* o) {
+  const double c00 = dsub(dmul(m[4], m[8]), dmul(m[5], m[7]));
+  const double c01 = dsub(dmul(m[5], m[6]), dmul(m[3], m[8]));
+  const double c02 = dsub(dmul(m[3], m[7]), dmul(m[4], m[6]));
+  const double det = dadd(dadd(dmul(m[0], c00), dmul(m[1], c01)), dmul(m[2], c02));
+  const double id = 1.0 / det;
+  o[0] = dmul(c00, id);
+  o[1] = dmul(dsub(dmul(m[2], m[7]), dmul(m[1], m[8])), id);
+  o[2] = dmul(dsub(dmul(m[1], m[5]), dmul(m[2], m[4])), id);
+  o[3] = dmul(c01, id);
+  o[4] = dmul(dsub(dmul(m[0], m[8]), dmul(m[2], m[6])), id);
+  o[5] = dmul(dsub(dmul(m[2], m[3]), dmul(m[0], m[5])), id);
+  o[6] = dmul(c02, id);
+  o[7] = dmul(dsub(dmul(m[1], m[6]), dmul(m[0], m[7])), id);
+  o[8] = dmul(dsub(dmul(m[0], m[4]), dmul(m[1], m[3])), id);
+  return det;
+}
+
+B2R_HD void mul3_rn(const double* a, const double* b, double* o) {
+#pragma unroll
+  for (int i = 0; i < 3; i++)
+#pragma unroll
+    for (int j = 0; j < 3; j++)
+      o[i * 3 + j] = dadd(dadd(dmul(a[i * 3 + 0], b[0 * 3 + j]), dmul(a[i * 3 + 1], b[1 * 3 + j])), dmul(a[i * 3 + 2], b[2 * 3 + j]));
+}
+
+// ndt_omp VoxelGridCovariance::applyFilter, the finalisation of one voxel from its float64 moments (cnt points, sums S, second
+// moments S2 row-major): mean, and for cnt >= 6 the covariance with PCL's (n-1)/n factor, its eigenvalues clamped to 1 % of the
+// largest, and the inverse.  Returns the voxel's point count, or -1 when the voxel is invalidated (a negative or zero
+// eigenvalue, or a non-finite inverse).  Every operation is unfused and in the oracle's order, so host and device agree bitwise.
+B2R_HD int ndt_voxel_gaussian(int cnt, const double* S, const double* S2, double* mean, double* icov) {
+  const double nn = (double)cnt;
+  mean[0] = S[0] / nn; mean[1] = S[1] / nn; mean[2] = S[2] / nn;
+#pragma unroll
+  for (int k = 0; k < 9; k++) icov[k] = 0.0;
+  if (cnt < 6) return cnt;
+  double cov[9];
+  const double f = dsub(nn, 1.0) / nn;
+#pragma unroll
+  for (int a = 0; a < 3; a++)
+#pragma unroll
+    for (int bb = 0; bb < 3; bb++) {
+      // cov = (S2 - 2*(sum*mean^T))/n + mean*mean^T ; cov *= (n-1)/n
+      const double t = dsub(S2[a * 3 + bb], dmul(2.0, dmul(S[a], mean[bb]))) / nn;
+      cov[a * 3 + bb] = dmul(dadd(t, dmul(mean[a], mean[bb])), f);
+    }
+  double w[3], V[9];
+  sym_eigen3(cov, w, V);
+  if (w[0] < 0 || w[1] < 0 || w[2] <= 0) return -1;
+  const double minv = dmul(0.01, w[2]);
+  if (w[0] < minv) {
+    w[0] = minv;
+    if (w[1] < minv) w[1] = minv;
+    double Vi[9], VD[9];
+    inv3_rn(V, Vi);
+#pragma unroll
+    for (int a = 0; a < 3; a++)
+#pragma unroll
+      for (int bb = 0; bb < 3; bb++) VD[a * 3 + bb] = dmul(V[a * 3 + bb], w[bb]);
+    mul3_rn(VD, Vi, cov);
+  }
+  inv3_rn(cov, icov);
+  bool bad = false;
+#pragma unroll
+  for (int a = 0; a < 9; a++) bad |= !(fabs(icov[a]) < INFINITY);  // +-inf or NaN
+  return bad ? -1 : cnt;
 }
 
 // ---- 6x6 host/device helpers used by the LM / Newton drivers -----------------------------------------------------

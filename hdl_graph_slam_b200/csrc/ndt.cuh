@@ -172,57 +172,17 @@ __global__ void k_vox_finalize(const unsigned int* __restrict__ keys_sorted, con
   for (int j = s; j < n && keys_sorted[j] == key; j++) {
     const float4 p = sorted[j];
     const double x = (double)p.x, y = (double)p.y, z = (double)p.z;
-    sx += x; sy += y; sz += z;
-    // products of two float32 values are exact in float64, so contraction cannot change these sums
-    cxx += x * x; cxy += x * y; cxz += x * z; cyy += y * y; cyz += y * z; czz += z * z;
+    sx = dadd(sx, x); sy = dadd(sy, y); sz = dadd(sz, z);
+    // products of two float32 values are exact in float64 (a fused add would round the same); unfused like the rest of the kernel
+    cxx = dadd(cxx, dmul(x, x)); cxy = dadd(cxy, dmul(x, y)); cxz = dadd(cxz, dmul(x, z));
+    cyy = dadd(cyy, dmul(y, y)); cyz = dadd(cyz, dmul(y, z)); czz = dadd(czz, dmul(z, z));
     cnt++;
   }
   NdtVoxel R;
-  const double nn = (double)cnt;
-  R.mean[0] = sx / nn; R.mean[1] = sy / nn; R.mean[2] = sz / nn;
-  R.npts = cnt;
+  const double S[3] = {sx, sy, sz};
+  const double S2[9] = {cxx, cxy, cxz, cxy, cyy, cyz, cxz, cyz, czz};
+  R.npts = ndt_voxel_gaussian(cnt, S, S2, R.mean, R.icov);  // linalg.cuh: unfused, bitwise the oracle's finalisation
   R.pad[0] = R.pad[1] = R.pad[2] = 0;
-  for (int k = 0; k < 9; k++) R.icov[k] = 0.0;
-  if (cnt >= 6) {
-    const double S[3] = {sx, sy, sz};
-    const double S2[9] = {cxx, cxy, cxz, cxy, cyy, cyz, cxz, cyz, czz};
-    double cov[9];
-    const double f = __ddiv_rn(__dsub_rn(nn, 1.0), nn);
-#pragma unroll
-    for (int a = 0; a < 3; a++)
-#pragma unroll
-      for (int bb = 0; bb < 3; bb++) {
-        // cov = (S2 - 2*(sum*mean^T))/n + mean*mean^T ; cov *= (n-1)/n       (non-contracted, as the oracle)
-        double t = __dmul_rn(2.0, __dmul_rn(S[a], R.mean[bb]));
-        t = __ddiv_rn(__dsub_rn(S2[a * 3 + bb], t), nn);
-        t = __dadd_rn(t, __dmul_rn(R.mean[a], R.mean[bb]));
-        cov[a * 3 + bb] = __dmul_rn(t, f);
-      }
-    double w[3], V[9];
-    sym_eigen3(cov, w, V);
-    if (w[0] < 0 || w[1] < 0 || w[2] <= 0) {
-      R.npts = -1;
-    } else {
-      const double minv = 0.01 * w[2];
-      if (w[0] < minv) {
-        w[0] = minv;
-        if (w[1] < minv) w[1] = minv;
-        double Vi[9], VD[9];
-        inv3(V, Vi);
-#pragma unroll
-        for (int a = 0; a < 3; a++)
-#pragma unroll
-          for (int bb = 0; bb < 3; bb++) VD[a * 3 + bb] = V[a * 3 + bb] * w[bb];
-        mul3(VD, Vi, cov);
-      }
-      inv3(cov, R.icov);
-      double mxv = -INFINITY, mnv = INFINITY;
-      bool nan_in = false;
-#pragma unroll
-      for (int a = 0; a < 9; a++) { mxv = fmax(mxv, R.icov[a]); mnv = fmin(mnv, R.icov[a]); nan_in |= (R.icov[a] != R.icov[a]); }
-      if (mxv == INFINITY || mnv == -INFINITY || nan_in) R.npts = -1;
-    }
-  }
   vox[s] = R;
   NdtCell C;
   C.mean[0] = R.mean[0]; C.mean[1] = R.mean[1]; C.mean[2] = R.mean[2];
@@ -1033,6 +993,22 @@ inline int ndt_derivatives_at(const b2r_config& cfg, Cloud& src, Cloud& tgt, Ndt
   std::memcpy(g, P.g, sizeof(P.g));
   std::memcpy(H, P.H, sizeof(P.H));
   if (n_pairs) *n_pairs = P.pairs;
+  return B2R_OK;
+}
+
+// the float64 Hessian pass (k_ndt_hessian) alone at pose p: what ndt_align runs after an active More-Thuente loop
+inline int ndt_hessian_at(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& W, cudaStream_t st, const double* p, double* H) {
+  int rc = ndt_sync_geom(*tgt.ndt, W, st);
+  if (rc) return rc;
+  NdtScalars K;
+  ndt_gauss(cfg, K);
+  ndt_angle_derivs(p, K);
+  float Tf[16];
+  ndt_pose_to_matrix(p, Tf);
+  NdtPass P;
+  rc = ndt_run_pass(cfg, src, tgt, W, st, K, Tf, true, true, &P);
+  if (rc) return rc;
+  std::memcpy(H, P.H, sizeof(P.H));
   return B2R_OK;
 }
 

@@ -226,6 +226,14 @@ class Registration:
         check(self._lib.b2r_ndt_derivatives_at(self._h, p.ctypes.data_as(dp), C.byref(score), g.ctypes.data_as(dp), H.ctypes.data_as(dp), C.byref(npairs)))
         return score.value, g, H, npairs.value
 
+    def ndtHessianAt(self, p):
+        """the float64 Hessian pass alone (computeHessian, run after an active More-Thuente line search) at p: H (6, 6)"""
+        p = np.ascontiguousarray(p, np.float64)
+        H = np.empty((6, 6), np.float64)
+        dp = C.POINTER(C.c_double)
+        check(self._lib.b2r_ndt_hessian_at(self._h, p.ctypes.data_as(dp), H.ctypes.data_as(dp)))
+        return H
+
     # --- companion / prefilter chain
     def _filter(self, fn, cloud, *args):
         a, n, s = _cloud(cloud)

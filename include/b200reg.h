@@ -159,6 +159,8 @@ int b2r_ndt_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int64_t
                        int32_t min_b[3], int32_t div_b[3]);
 /* one computeDerivatives pass at p = (tx,ty,tz,rx,ry,rz): score, g[6], H[36] row-major, number of (point,cell) pairs */
 int b2r_ndt_derivatives_at(b2r_handle* h, const double p[6], double* score, double* g, double* H, uint64_t* n_pairs);
+/* one float64 computeHessian pass at p (the pass the align runs after an active More-Thuente line search): H[36] row-major */
+int b2r_ndt_hessian_at(b2r_handle* h, const double p[6], double* H);
 
 /* ---- companion: voxel-grid downsample ---------------------------------------------------------------------------
  * replaces pcl::VoxelGrid<PointXYZI>::filter with setLeafSize(leaf,leaf,leaf) (apps/prefiltering_nodelet.cpp:54-58,138-149;

@@ -105,6 +105,36 @@ struct orc_ndt_map {
   bool empty = true;
 };
 
+extern "C" int orc_ndt_voxel_gaussian(int n, const double* S, const double* S2, double* mean, double* cov, double* icov) {
+  const double nn = (double)n;
+  for (int d = 0; d < 3; d++) mean[d] = S[d] / nn;
+  for (int a = 0; a < 9; a++) { cov[a] = 0.0; icov[a] = 0.0; }
+  if (n < 6) return n;
+  // cov = (S2 - 2*(sum*mean^T))/n + mean*mean^T ; cov *= (n-1)/n
+  for (int a = 0; a < 3; a++)
+    for (int b = 0; b < 3; b++) cov[a * 3 + b] = (S2[a * 3 + b] - 2 * (S[a] * mean[b])) / nn + mean[a] * mean[b];
+  double f = (nn - 1.0) / nn;
+  for (int a = 0; a < 9; a++) cov[a] *= f;
+  double w[3], V[9];
+  sym_eigen<3>(cov, w, V);
+  if (w[0] < 0 || w[1] < 0 || w[2] <= 0) return -1;
+  double minv = 0.01 * w[2];
+  if (w[0] < minv) {
+    w[0] = minv;
+    if (w[1] < minv) w[1] = minv;
+    double Vi[9], VD[9];
+    inv3(V, Vi);
+    for (int a = 0; a < 3; a++)
+      for (int b = 0; b < 3; b++) VD[a * 3 + b] = V[a * 3 + b] * w[b];
+    mul3(VD, Vi, cov);
+  }
+  inv3(cov, icov);
+  double mxv = -INFINITY, mnv = INFINITY;
+  for (int a = 0; a < 9; a++) { mxv = std::max(mxv, icov[a]); mnv = std::min(mnv, icov[a]); }
+  if (mxv == INFINITY || mnv == -INFINITY || mxv != mxv || mnv != mnv) return -1;
+  return n;
+}
+
 extern "C" orc_ndt_map* orc_ndt_build(const float* tgt, size_t m, size_t stride, float resolution) {
   orc_ndt_map* M = new orc_ndt_map();
   M->leaf = resolution;
@@ -150,36 +180,7 @@ extern "C" orc_ndt_map* orc_ndt_build(const float* tgt, size_t m, size_t stride,
     std::memset(&L, 0, sizeof(L));
     L.key = kv.first;
     const Acc& A = kv.second;
-    L.nr_points = A.n;
-    double nn = (double)A.n;
-    for (int d = 0; d < 3; d++) L.mean[d] = A.s[d] / nn;
-    if (A.n >= 6) {
-      // cov = (S2 - 2*(sum*mean^T))/n + mean*mean^T ; cov *= (n-1)/n
-      for (int a = 0; a < 3; a++)
-        for (int b = 0; b < 3; b++) L.cov[a * 3 + b] = (A.c[a * 3 + b] - 2 * (A.s[a] * L.mean[b])) / nn + L.mean[a] * L.mean[b];
-      double f = (nn - 1.0) / nn;
-      for (int a = 0; a < 9; a++) L.cov[a] *= f;
-      double w[3], V[9];
-      sym_eigen<3>(L.cov, w, V);
-      if (w[0] < 0 || w[1] < 0 || w[2] <= 0) {
-        L.nr_points = -1;
-      } else {
-        double minv = 0.01 * w[2];
-        if (w[0] < minv) {
-          w[0] = minv;
-          if (w[1] < minv) w[1] = minv;
-          double Vi[9], VD[9];
-          inv3(V, Vi);
-          for (int a = 0; a < 3; a++)
-            for (int b = 0; b < 3; b++) VD[a * 3 + b] = V[a * 3 + b] * w[b];
-          mul3(VD, Vi, L.cov);
-        }
-        inv3(L.cov, L.icov);
-        double mxv = -INFINITY, mnv = INFINITY;
-        for (int a = 0; a < 9; a++) { mxv = std::max(mxv, L.icov[a]); mnv = std::min(mnv, L.icov[a]); }
-        if (mxv == INFINITY || mnv == -INFINITY || mxv != mxv || mnv != mnv) L.nr_points = -1;
-      }
-    }
+    L.nr_points = orc_ndt_voxel_gaussian(A.n, A.s, A.c, L.mean, L.cov, L.icov);
     M->leaves.push_back(L);
   }
   std::sort(M->leaves.begin(), M->leaves.end(), [](const Leaf& a, const Leaf& b) { return a.key < b.key; });
@@ -343,6 +344,18 @@ static inline double ndt_point_cell(const NdtConsts& K, const float J[3][6], con
 
 static const int kOff7[7][3] = {{0, 0, 0}, {1, 0, 0}, {-1, 0, 0}, {0, 1, 0}, {0, -1, 0}, {0, 0, 1}, {0, 0, -1}};
 
+// getNeighborhoodAtPoint's base cell, floor(xt / leaf) per axis.  ndt_omp casts without a guard, which is undefined for a
+// non-finite point or a cell beyond int range; the oracle (like the engine) drops such a point: it contributes no pair.
+static inline bool base_cell(const orc_ndt_map* M, const float* xt, int* ijk) {
+  for (int d = 0; d < 3; d++) {
+    if (!std::isfinite(xt[d])) return false;
+    const float f = std::floor(xt[d] / M->leaf);
+    if (!(std::fabs(f) < 1.0e9f)) return false;
+    ijk[d] = (int)f;
+  }
+  return true;
+}
+
 // Row-major float 4x4 from p = (t, euler xyz): Translation * AngleAxis(x) * AngleAxis(y) * AngleAxis(z) in float32
 static void pose_to_matrix_f32(const double* p, float* T) {
   float ang[3] = {(float)p[3], (float)p[4], (float)p[5]};
@@ -406,9 +419,8 @@ static double derivatives(const orc_ndt_map* M, const float* src, size_t n, size
     uint8_t mask = 0;
     bool have_pd = false;
     float J[3][6], PH[3][3][3];
-    if (!M->empty) {
-      int ijk[3];
-      for (int d = 0; d < 3; d++) ijk[d] = (int)std::floor(xt[d] / M->leaf);
+    int ijk[3];
+    if (!M->empty && base_cell(M, xt, ijk)) {
       for (int c = 0; c < ncell; c++) {
         int cc[3] = {ijk[0] + kOff7[c][0], ijk[1] + kOff7[c][1], ijk[2] + kOff7[c][2]};
         bool inb = true;
@@ -483,7 +495,7 @@ static void hessian_only(const orc_ndt_map* M, const float* src, size_t n, size_
     const double* tab[3][3] = {{a, b, cV}, {b, dV, eV}, {cV, eV, fV}};
     double* H = &he[(size_t)i * 36];
     int ijk[3];
-    for (int d = 0; d < 3; d++) ijk[d] = (int)std::floor(xt[d] / M->leaf);
+    if (!base_cell(M, xt, ijk)) continue;
     for (int c = 0; c < ncell; c++) {
       int cc[3] = {ijk[0] + kOff7[c][0], ijk[1] + kOff7[c][1], ijk[2] + kOff7[c][2]};
       bool inb = true;
@@ -533,6 +545,16 @@ extern "C" double orc_ndt_derivatives(const orc_ndt_map* M, const float* src, si
   float Tf[16];
   pose_to_matrix_f32(p, Tf);
   return derivatives(M, src, n, stride, Tf, cfg, K, g, H, true, n_pairs, per_point_cells);
+}
+
+extern "C" void orc_ndt_hessian_at(const orc_ndt_map* M, const float* src, size_t n, size_t stride, const orc_ndt_config* cfg,
+                                   const double* p, double* H) {
+  NdtConsts K;
+  gauss_consts(cfg, K);
+  angle_derivs(p, K);
+  float Tf[16];
+  pose_to_matrix_f32(p, Tf);
+  hessian_only(M, src, n, stride, Tf, cfg, K, H);
 }
 
 // ---- More-Thuente helpers (PCL ndt.hpp; SURVEY A.2)
@@ -695,7 +717,7 @@ extern "C" void orc_ndt_align(const orc_ndt_map* M, const float* src, size_t n, 
         else interval_converged = updateIntervalMT(a_l, f_l, g_l, a_u, f_u, g_u, a_t, phi_t, d_phi_t);
         step_iterations++;
       }
-      if (step_iterations) { hessian_only(M, src, n, stride, Tfinal, cfg, K, H); passes++; }
+      if (step_iterations) { hessian_only(M, src, n, stride, Tfinal, cfg, K, H); passes++; res->hessian_passes++; }
     }
     double delta_p_norm = a_t;
     for (int i = 0; i < 6; i++) { dp[i] *= delta_p_norm; p[i] += dp[i]; }

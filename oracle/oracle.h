@@ -106,6 +106,9 @@ void orc_deskew(const float* pts, size_t n, size_t stride, double scan_period, c
 
 /* ---- NDT (pclomp::NormalDistributionsTransform + VoxelGridCovariance) ---- */
 typedef struct orc_ndt_map orc_ndt_map;
+/* VoxelGridCovariance::applyFilter's finalisation of one voxel from its float64 moments (n points, sums S[3], second moments
+ * S2[9] row-major): mean[3], cov[9] (after the eigenvalue clamp), icov[9].  Returns n, or -1 for an invalidated voxel. */
+int orc_ndt_voxel_gaussian(int n, const double* S, const double* S2, double* mean, double* cov, double* icov);
 orc_ndt_map* orc_ndt_build(const float* tgt, size_t m, size_t stride, float resolution);
 void orc_ndt_free(orc_ndt_map*);
 /* voxel table dump: returns number of leaves (all occupied leaves, ascending key). Arrays may be NULL to query size.
@@ -132,13 +135,18 @@ typedef struct {
 double orc_ndt_derivatives(const orc_ndt_map*, const float* src, size_t n, size_t stride, const orc_ndt_config* cfg,
                            const double* p, double* g, double* H, uint64_t* n_pairs, uint8_t* per_point_cells);
 
+/* ndt_omp computeHessian (float64, the pass run after an active More-Thuente loop) at p. H[36] row-major. */
+void orc_ndt_hessian_at(const orc_ndt_map*, const float* src, size_t n, size_t stride, const orc_ndt_config* cfg,
+                        const double* p, double* H);
+
 typedef struct {
   float T[16];
   int converged;
   int iterations;
   double trans_probability;
   double p[6];
-  uint64_t derivative_passes;
+  uint64_t derivative_passes;     /* every pass over the source, the Hessian passes included */
+  uint64_t hessian_passes;        /* float64 computeHessian passes (one after every More-Thuente loop that iterated) */
 } orc_ndt_result;
 
 void orc_ndt_align(const orc_ndt_map*, const float* src, size_t n, size_t stride, const orc_ndt_config* cfg,

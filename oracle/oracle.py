@@ -37,7 +37,7 @@ class NdtConfig(C.Structure):
 
 class NdtResult(C.Structure):
     _fields_ = [("T", C.c_float * 16), ("converged", C.c_int), ("iterations", C.c_int), ("trans_probability", C.c_double), ("p", C.c_double * 6),
-                ("derivative_passes", C.c_uint64)]
+                ("derivative_passes", C.c_uint64), ("hessian_passes", C.c_uint64)]
 
 
 def lib():
@@ -323,6 +323,16 @@ class NdtMap:
                                           C.byref(npairs), cells.ctypes.data_as(vp))
         return dict(score=score, g=g, H=H, n_pairs=npairs.value, cells=cells[:n])
 
+    def hessian_at(self, src, p, **kw):
+        """the float64 computeHessian pass alone at p: H (6, 6)"""
+        sa, sp, n, ss = _f32(src)
+        cfg = self._cfg(**kw)
+        p = np.ascontiguousarray(p, np.float64)
+        H = np.empty((6, 6))
+        vp = C.c_void_p
+        lib().orc_ndt_hessian_at(self._m, sp, C.c_size_t(n), C.c_size_t(ss), C.byref(cfg), p.ctypes.data_as(vp), H.ctypes.data_as(vp))
+        return H
+
     def align(self, src, guess=None, trace=False, **kw):
         sa, sp, n, ss = _f32(src)
         cfg = self._cfg(**kw)
@@ -332,7 +342,8 @@ class NdtMap:
         lib().orc_ndt_align(self._m, sp, C.c_size_t(n), C.c_size_t(ss), C.byref(cfg), g.ctypes.data_as(C.c_void_p), C.byref(res),
                             tp.ctypes.data_as(C.c_void_p) if trace else None)
         out = dict(T=np.array(res.T, np.float32).reshape(4, 4), converged=bool(res.converged), iterations=res.iterations,
-                   trans_probability=res.trans_probability, p=np.array(res.p), derivative_passes=res.derivative_passes)
+                   trans_probability=res.trans_probability, p=np.array(res.p), derivative_passes=res.derivative_passes,
+                   hessian_passes=res.hessian_passes)
         if trace:
             out["trace_p"] = tp
         return out

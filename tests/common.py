@@ -29,6 +29,48 @@ def perturb(seed, dt=0.3, dr_deg=2.0):
     return T
 
 
+VOXEL_KINDS = ("generic", "plane_z", "plane_diag", "line_x", "line_diag", "identical", "clamp_one_below", "clamp_one_above",
+               "clamp_two", "clamp_none")
+
+
+def voxel_points(kind, n, cell, res, rng, offset=(0.0, 0.0, 0.0)):
+    """n float32 points (x y z 1) inside the NDT cell `cell` (integer ijk) of size `res`, shaped so the voxel's covariance is
+    degenerate or sits at the eigenvalue clamp.  Coordinates are multiples of res/64 away from the cell faces, so they are exact
+    in float32 (also after `offset`, a multiple of res/64) and exact planes / lines stay exact:
+      plane_z (z = const), plane_diag (x - y = const), line_x (y, z const), line_diag (x = y = z up to the cell origin),
+      identical (n copies of one point), clamp_*: 3 orthogonal point pairs whose eigenvalue ratios are 1 % -+ 1e-4 of the largest
+      (one_below: the smallest is clamped, one_above: not, two: both smaller ones clamped, none: all above 1 %)."""
+    o = (np.asarray(cell, np.float64) + 0.5) * res + np.asarray(offset, np.float64)  # cell centre
+    q = res / 64.0
+    u = lambda m: rng.integers(-20, 21, m) * q  # noqa: E731  grid offsets within +-0.31 res of the centre
+    p = np.zeros((n, 3))
+    if kind == "generic":
+        p = np.c_[u(n), u(n), u(n)]
+    elif kind == "plane_z":
+        p = np.c_[u(n), u(n), np.full(n, 3 * q)]
+    elif kind == "plane_diag":
+        a = u(n)
+        p = np.c_[a, a - 2 * q, u(n)]
+    elif kind == "line_x":
+        p = np.c_[u(n), np.full(n, -q), np.full(n, 5 * q)]
+    elif kind == "line_diag":
+        a = u(n)
+        p = np.c_[a, a, a]
+    elif kind == "identical":
+        p = np.tile([[q, -2 * q, 3 * q]], (n, 1))
+    else:
+        r2 = {"clamp_one_below": (0.25, 0.0099), "clamp_one_above": (0.25, 0.0101), "clamp_two": (0.0099, 0.0098),
+              "clamp_none": (0.25, 0.02)}[kind]
+        a = 0.3 * res
+        ax = [a, a * np.sqrt(r2[0]), a * np.sqrt(r2[1])]
+        base = [np.eye(3)[d] * s * ax[d] for d in range(3) for s in (1.0, -1.0)]
+        p = np.array([base[i % 6] for i in range(n)])
+        if n % 6:  # extra points at the centre keep the mean and the axes
+            p[6:] = 0.0
+    pts = (o + p).astype(np.float32)
+    return np.c_[pts, np.ones(n, np.float32)]
+
+
 def relrel(a, b):
     a = np.asarray(a, np.float64)
     b = np.asarray(b, np.float64)

@@ -2,6 +2,7 @@
 create a handle (no CPU fallback); the product never links or loads the oracle."""
 import os
 import re
+import shutil
 import subprocess
 import pytest
 
@@ -66,6 +67,34 @@ def test_product_does_not_touch_the_oracle():
             if f.endswith((".py", ".cu", ".cuh", ".c", ".h")):
                 txt = open(os.path.join(dirpath, f), errors="replace").read()
                 assert "liboracle" not in txt and "from oracle" not in txt and "import oracle" not in txt, f
+
+
+def test_voxel_finalize_is_not_contracted(tmp_path):
+    """k_vox_finalize decides a voxel's validity on the sign of its smallest eigenvalue, which for a planar or linear voxel is
+    rounding noise: its float64 arithmetic must be the oracle's unfused sequence.  In the PTX of the engine (compiled with the
+    library's own flags) every float64 multiply / add / subtract of the kernel carries an explicit .rn (which ptxas never fuses)
+    and there is no fma.  The SASS of the built library can still hold DFMA: correctly rounded float64 division and square root
+    are DFMA sequences, and those round exactly like the oracle's / and sqrt."""
+    from hdl_graph_slam_b200 import build
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    ptx = tmp_path / "api.ptx"
+    flags = [f for f in build.NVCC_FLAGS if f not in ("-shared", "-Xcompiler", "-fPIC", "-lineinfo")]
+    flags = [f.replace("code=sm_90a", "code=compute_90a") for f in flags]
+    subprocess.check_call([nvcc] + flags + ["-ptx", "-o", str(ptx), os.path.join(ROOT, "hdl_graph_slam_b200", "csrc", "api.cu")])
+    s = ptx.read_text()
+    i = s.index(".entry _ZN3b2r14k_vox_finalize")
+    body = s[i:s.index("\n}\n", i)]
+    ops = re.findall(r"\b(fma|mad|mul|add|sub)((?:\.\w+)*)\.f64\b", body)
+    assert len(ops) > 100  # the eigen-solve is in the kernel
+    assert not [o for o in ops if o[0] in ("fma", "mad")], "contracted float64 in k_vox_finalize"
+    assert not [o for o in ops if ".rn" not in o[1]], "float64 arithmetic without .rn (ptxas may fuse it) in k_vox_finalize"
+    # the built library holds the kernel as sm_90a SASS
+    build.build_engine()
+    so = os.path.join(ROOT, "hdl_graph_slam_b200", "_lib", "libb200reg.so")
+    cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    sass = subprocess.run([cuobjdump, "-sass", so], capture_output=True, text=True, check=True).stdout
+    fins = [f for f in sass.split("Function : ") if f.startswith("_ZN3b2r14k_vox_finalize")]
+    assert len(fins) == 1 and "DMUL" in fins[0]
 
 
 def test_pcd_header_parser_runs_without_gpu(tmp_path):

@@ -172,3 +172,48 @@ reg.close()
         assert r.returncode == 0, r.stdout + r.stderr
         outs.append(json.loads(r.stdout.strip().splitlines()[-1]))
     assert outs[0] == outs[1]
+
+
+def _gicp_degenerate_clouds():
+    """exact degenerate neighbourhoods (coordinates on a 1/8 grid, exact in float32): name -> (cloud, kind, direction)"""
+    g = np.arange(-3, 3, dtype=np.float64) / 8.0
+    t = np.arange(30, dtype=np.float64) / 8.0 - 2.0
+    u, v = [a.reshape(-1) for a in np.meshgrid(g, g, indexing="ij")]
+    out = {
+        "identical": (np.tile([[1.25, -0.5, 2.0]], (24, 1)), "point", None),
+        "line_x": (np.c_[t, np.full(30, 0.5), np.full(30, -1.0)], "line", (1, 0, 0)),
+        "line_y": (np.c_[np.full(30, 0.5), t, np.full(30, -1.0)], "line", (0, 1, 0)),
+        "line_z": (np.c_[np.full(30, 0.5), np.full(30, -1.0), t], "line", (0, 0, 1)),
+        "line_diag": (np.c_[t, t, t], "line", (1, 1, 1)),
+        "plane_z": (np.c_[u, v, np.full(u.size, 0.75)], "plane", (0, 0, 1)),
+        "plane_x": (np.c_[np.full(u.size, -0.25), u, v], "plane", (1, 0, 0)),
+        "plane_diag": (np.c_[u, u - 0.5, v], "plane", (1, -1, 0)),  # x - y = 0.5
+    }
+    return {k: (np.c_[c, np.ones(c.shape[0])].astype(np.float32), kind, d) for k, (c, kind, d) in out.items()}
+
+
+@pytest.mark.parametrize("case", list(_gicp_degenerate_clouds()))
+def test_degenerate_neighbourhood_covariances(reg, oracle, case):
+    """fast_gicp's PLANE regularisation on neighbourhoods whose covariance is degenerate.  A plane has a unique normal: engine ==
+    oracle to 1e-8 == I - 0.999 n n^T of the plane's normal, eigenvalues (numpy eigh) {1e-3, 1, 1}.  A zero covariance (all k
+    neighbours one point) has every direction as eigenvector: both follow JacobiSVD (U = I, smallest last) -> diag(1, 1, 1e-3).  A
+    line leaves the normal free in the plane orthogonal to it: only the properties are pinned (symmetric, eigenvalues {1e-3, 1, 1},
+    the 1e-3 direction orthogonal to the line)."""
+    cloud, kind, d = _gicp_degenerate_clouds()[case]
+    reg.setInputTarget(cloud)
+    got = reg.getCovariances(1, cloud.shape[0])
+    want = oracle.gicp_covariances(cloud, 20)
+    for C in (got, want):
+        assert np.max(np.abs(C - np.transpose(C, (0, 2, 1)))) < 1e-15
+        w, V = np.linalg.eigh(C)
+        assert np.max(np.abs(w - [1e-3, 1.0, 1.0])) < 1e-12
+        if kind == "point":
+            assert np.max(np.abs(C - np.diag([1.0, 1.0, 1e-3]))) < 1e-12
+        elif kind == "line":
+            dn = np.asarray(d, np.float64) / np.linalg.norm(d)
+            assert np.max(np.abs(V[:, :, 0] @ dn)) < 1e-9
+        else:
+            n = np.asarray(d, np.float64) / np.linalg.norm(d)
+            assert np.max(np.abs(C - (np.eye(3) - 0.999 * np.outer(n, n)))) < 1e-8
+    if kind != "line":
+        assert np.max(np.abs(got - want)) < 1e-8

@@ -35,6 +35,23 @@ def test_min_eigenvector_solver_matches_jacobi(tmp_path):
     assert out.returncode == 0, out.stdout + out.stderr
 
 
+def test_voxel_finalize_equals_oracle_bitwise(oracle, tmp_path):
+    """The NDT voxel finalisation (ndt_voxel_gaussian: covariance, Jacobi eigen-solve, 1 % clamp, inverse — what k_vox_finalize runs)
+    and its eigen-solver sym_eigen3 alone, compiled as host code, against the oracle's orc_ndt_voxel_gaussian / orc::sym_eigen<3> on
+    1e5 voxels of 5-15 points on exact planes and lines, all-identical points, generic and nearly planar voxels, at the origin and
+    shifted by (2e4, -3e4, 50): npts, mean, icov, eigenvalues and eigenvectors bit-identical."""
+    exe = tmp_path / "vox_eig_harness"
+    subprocess.check_call(["nvcc", "-O2", "-std=c++17", "-w", "-Wno-deprecated-gpu-targets", "-ccbin", "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++",
+                           "-Xcompiler", "-ffp-contract=off", "-o", str(exe), os.path.join(ROOT, "tests", "vox_eig_harness.cu"),
+                           "-L" + os.path.join(ROOT, "oracle"), "-loracle", "-Xlinker", "-rpath=" + os.path.join(ROOT, "oracle")])
+    out = subprocess.run([str(exe), "100000"], capture_output=True, text=True)
+    assert out.returncode == 0, out.stdout + out.stderr
+    assert "eig_mismatch=0" in out.stdout and "gauss_mismatch=0" in out.stdout
+    # the cases reach every branch: invalidated voxels, one and two clamped eigenvalues
+    stats = dict(kv.split("=") for kv in out.stdout.split() if "=" in kv)
+    assert int(stats["invalid"]) > 1000 and int(stats["clamped_one"]) > 1000 and int(stats["clamped_two"]) > 1000
+
+
 @pytest.fixture(scope="module")
 def warp_harness(oracle):
     os.makedirs(os.path.join(ROOT, "build"), exist_ok=True)

@@ -189,3 +189,85 @@ def test_ndt_score_and_gradient_independent(synth, oracle):
         rel_pos = np.max(np.abs(g - o["g"])) / np.max(np.abs(g))
         rel_neg = np.max(np.abs(g + o["g"])) / np.max(np.abs(g))
         assert min(rel_pos, rel_neg) < 2e-3, (rel_pos, rel_neg)
+
+
+def _rot_derivs(a):
+    """R(a) about one axis and its first and second derivatives, for the x, y, z factors of R = Rx Ry Rz"""
+    c, s = np.cos(a), np.sin(a)
+    R = np.array([[c, -s], [s, c]])
+    dR = np.array([[-s, -c], [c, -s]])
+    return R, dR, -R
+
+
+def _euler_factor(axis, a, order):
+    M = np.zeros((3, 3))
+    keep = [i for i in range(3) if i != axis]
+    blk = _rot_derivs(a)[order]
+    if axis == 1:  # Ry = [[c, 0, s], [0, 1, 0], [-s, 0, c]]: the 2x2 block acts on (z, x)
+        blk = blk.T
+    M[np.ix_(keep, keep)] = blk
+    if order == 0:
+        M[axis, axis] = 1.0
+    return M
+
+
+def indep_ndt_hessian(ind, src, p, cells_mask):
+    """ndt_omp computeHessian restated from the definition: the Hessian in p of sum over (point, cell) of -d1 exp(-d2/2 q^T C q),
+    q = R(p) x + t - mean, with dq/dp and d2q/dp2 from the derivatives of R = Rx Ry Rz (numpy float64; the (point, cell) pairs are
+    the ones the oracle visited)"""
+    x = src[:, :3].astype(np.float64)
+    R, t = euler_xyz(p)
+    F = [[_euler_factor(ax, p[3 + ax], o) for o in range(3)] for ax in range(3)]
+    def dR(orders):  # noqa: E306
+        return F[0][orders[0]] @ F[1][orders[1]] @ F[2][orders[2]]
+    d1R = [dR([1 if k == a else 0 for k in range(3)]) for a in range(3)]
+    d2R = [[dR([(a == k) + (b == k) for k in range(3)]) for b in range(3)] for a in range(3)]
+    xt = x @ R.T + t
+    base = np.floor(xt / ind.res).astype(np.int64)  # only used with the oracle's accepted offsets below
+    H = np.zeros((6, 6))
+    offs = ((0, 0, 0), (1, 0, 0), (-1, 0, 0), (0, 1, 0), (0, -1, 0), (0, 0, 1), (0, 0, -1))
+    for i in range(x.shape[0]):
+        if not cells_mask[i]:
+            continue
+        J = np.zeros((3, 6))
+        J[:, :3] = np.eye(3)
+        for a in range(3):
+            J[:, 3 + a] = d1R[a] @ x[i]
+        Hx = [[d2R[a][b] @ x[i] for b in range(3)] for a in range(3)]
+        for c, off in enumerate(offs):
+            if not (cells_mask[i] >> c) & 1:
+                continue
+            mean, C = ind.cells[tuple(base[i] + np.array(off))]
+            q = xt[i] - mean
+            e = np.exp(-0.5 * ind.d2 * q @ C @ q)
+            qCJ = q @ C @ J
+            sec = np.zeros((6, 6))
+            for a in range(3):
+                for b in range(3):
+                    sec[3 + a, 3 + b] = q @ C @ Hx[a][b]
+            H += ind.d1 * ind.d2 * e * (-ind.d2 * np.outer(qCJ, qCJ) + J.T @ C @ J + sec)
+    return H
+
+
+def test_ndt_hessian_pass_independent(synth, oracle):
+    """the oracle's float64 Hessian pass (what k_ndt_hessian must reproduce) against the Hessian of the NDT score derived from its
+    definition with numpy, on the same (point, cell) pairs"""
+    tgt = synth.scan("vlp16_16k", frame=0, stride=8)
+    src = synth.scan("vlp16_16k", frame=1, stride=8)[::8]
+    m = oracle.NdtMap(tgt, 1.0)
+    ind = IndepNdt(tgt, 1.0)
+    for p in (np.array([0.1, -0.05, 0.02, 0.0, 0.0, 0.0]), np.array([0.2, -0.1, 0.05, 0.01, -0.02, 0.03])):
+        # the oracle picks cells by the float32 transform: keep the points that are not within 1e-4 of a cell face
+        R, t = euler_xyz(p)
+        xt = src[:, :3].astype(np.float64) @ R.T + t
+        same = np.ones(src.shape[0], bool)
+        for d in range(3):
+            lo = np.floor(xt[:, d])
+            same &= (np.abs(xt[:, d] - lo) > 1e-4) & (np.abs(xt[:, d] - lo - 1) > 1e-4)
+        sub = src[same]
+        o = m.hessian_at(sub, p)
+        cells = m.derivatives(sub, p)["cells"]
+        assert int(sum(bin(int(c)).count("1") for c in cells)) > 1000
+        h = indep_ndt_hessian(ind, sub, p, cells)
+        # the oracle transforms the point in float32 (~1e-6 m at these ranges): agreement to ~2e-5, a wrong term is off by O(1)
+        assert relrel(o, h) < 1e-4, relrel(o, h)

@@ -1,7 +1,7 @@
 """GPU parity of the NDT path (ndt_omp semantics, SURVEY.md A.2/A.3) against the CPU oracle, through the C ABI.
 
-Tolerances: voxel keys / point counts / validity set and the number of (point, cell) pairs bit-exact; voxel mean and inverse
-covariance rel <= 1e-9; score, gradient, Hessian of one derivative pass rel <= 1e-9 (the per-pair float32 math follows the
+Tolerances: voxel keys / point counts / validity set, voxel means and inverse covariances, and the number of (point, cell) pairs
+bit-exact; score, gradient, Hessian of one derivative pass rel <= 1e-9 (the per-pair float32 math follows the
 oracle's operation order exactly, only the float64 summation tree differs); final pose <= 1e-4 m / 1e-4 rad and the same
 iteration count."""
 import numpy as np
@@ -49,9 +49,7 @@ def test_voxel_map(pair, oracle, res):
     assert np.max(np.abs(got["mean"] - want["mean"])) == 0.0
     valid = want["npts"] >= 6
     assert valid.sum() > 100
-    num = np.abs(got["icov"][valid] - want["icov"][valid]).reshape(valid.sum(), -1).max(axis=1)
-    den = np.abs(want["icov"][valid]).reshape(valid.sum(), -1).max(axis=1)
-    assert np.max(num / den) < 1e-9
+    assert np.array_equal(got["icov"], want["icov"])  # the finalisation is the oracle's unfused float64 sequence
     r.close()
 
 
