@@ -446,8 +446,8 @@ static int build_bvh(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
   }
   // clouds beyond 131 072 points: bounding box, keys, toolkit radix sort, leaves
   B2R_CUDA(B.keys_a.reserve(n)); B2R_CUDA(B.keys_b.reserve(n)); B2R_CUDA(B.vals_a.reserve(n)); B2R_CUDA(B.vals_b.reserve(n));
-  size_t tmp_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, B.keys_a.p, B.keys_b.p, B.vals_a.p, B.vals_b.p, N, 0, 30, st);
+  size_t tmp_bytes = 0;  // queried for the bit range the sort below runs over
+  B2R_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, B.keys_a.p, B.keys_b.p, B.vals_a.p, B.vals_b.p, N, 0, 32, st));
   B2R_CUDA(B.sort_tmp.reserve(tmp_bytes + 256));
   TEL_BEGIN(&h->tel, st);
   const unsigned nb = (unsigned)((n + 255) / 256);
@@ -456,9 +456,9 @@ static int build_bvh(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
   k_fill_i32<<<nb, 256, 0, st>>>(c.pos_of.p, N, -1);
   k_morton_keys<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, N, B.mm, B.keys_a.p, B.vals_a.p);
   size_t tb = B.sort_tmp.cap;
-  // stable LSD sort: ties keep ascending index.  Keys are 30-bit Hilbert indices, or 0xffffffff for dropped points: the two top
-  // bits are constant among valid keys, so sorting bits [0,30) orders them; dropped points are recognised by their key afterwards
-  cub::DeviceRadixSort::SortPairs(B.sort_tmp.p, tb, B.keys_a.p, B.keys_b.p, B.vals_a.p, B.vals_b.p, N, 0, 32, st);
+  // stable LSD sort over all 32 bits: ties keep ascending index.  Keys are 30-bit Hilbert indices, or 0xffffffff for dropped
+  // points, which therefore sort behind every valid key and are recognised by their key afterwards
+  B2R_CUDA(cub::DeviceRadixSort::SortPairs(B.sort_tmp.p, tb, B.keys_a.p, B.keys_b.p, B.vals_a.p, B.vals_b.p, N, 0, 32, st));
   k_bvh_leaves<<<c.nsup, 1024, 0, st>>>(c.raw_view, c.stride_f, N, B.keys_b.p, B.vals_b.p, c.sorted.p, c.pos_of.p, c.leaf_lo.p, c.leaf_hi.p,
                                         c.sup_lo.p, c.sup_hi.p);
   TEL_END(&h->tel, KC_GRID, 10, st);
@@ -1041,8 +1041,14 @@ extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (!h->corr_valid) return fail(B2R_ESTATE, "no linearisation has run since the clouds were set");
   if (n != SRC(h).n) return fail(B2R_EINVAL, "n does not match the source cloud");
+  // a non-finite source point is not in the source's search structure (pos_of = -1): no search writes its entry, and like a PCL
+  // query that finds nothing it has no correspondence
+  std::vector<int> pos(n);
   B2R_CUDA(cudaMemcpyAsync(out, h->corr[h->cur].p, n * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaMemcpyAsync(pos.data(), SRC(h).pos_of.p, n * sizeof(int), cudaMemcpyDeviceToHost, h->st));
   B2R_CUDA(cudaStreamSynchronize(h->st));
+  for (size_t i = 0; i < n; i++)
+    if (pos[i] < 0) out[i] = -1;
   return B2R_OK;
 }
 
@@ -1573,8 +1579,8 @@ extern "C" int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot
   int* flags = h->tmp_i.p;
   int* slots = h->tmp_i.p + total + 8;
   size_t tmp_sort = 0, tmp_scan = 0;
-  cub::DeviceRadixSort::SortKeys(nullptr, tmp_sort, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st);
-  cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, flags, slots, (int)total, st);
+  B2R_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_sort, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st));
+  B2R_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, flags, slots, (int)total, st));
   B2R_CUDA(h->bc[0].sort_tmp.reserve(std::max(tmp_sort, tmp_scan) + 256));
   if (!h->map_geom) {
     B2R_CUDA(cudaMalloc(&h->map_geom, sizeof(MapGeom) + 64));
@@ -1592,15 +1598,18 @@ extern "C" int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot
     }
     k_map_keys<<<nb, 256, 0, st>>>(cloud.p, sf, T, h->map_geom, h->map_keys[0].p);
     size_t tb = h->bc[0].sort_tmp.cap;
-    cub::DeviceRadixSort::SortKeys(h->bc[0].sort_tmp.p, tb, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st);
+    B2R_CUDA(cub::DeviceRadixSort::SortKeys(h->bc[0].sort_tmp.p, tb, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st));
     k_map_heads<<<nb, 256, 0, st>>>(h->map_keys[1].p, T, flags);
     tb = h->bc[0].sort_tmp.cap;
-    cub::DeviceScan::ExclusiveSum(h->bc[0].sort_tmp.p, tb, flags, slots, (int)total, st);
+    B2R_CUDA(cub::DeviceScan::ExclusiveSum(h->bc[0].sort_tmp.p, tb, flags, slots, (int)total, st));
     k_map_centers<<<nb, 256, 0, st>>>(h->map_keys[1].p, flags, slots, T, h->map_geom, sf, src.p, n_dev);
     TEL_END(&h->tel, KC_MISC, 106, st); }
   B2R_CUDA(cudaGetLastError());
   B2R_CUDA(cudaMemcpyAsync(h->map_h, n_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(h->map_h + 1, &h->map_geom->overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2R_CUDA(cudaStreamSynchronize(st));
+  // the octree keys hold 21 bits per axis: a deeper box leaves every point uninserted, which must not pass for an empty map
+  if (h->map_h[1]) return fail(B2R_EUNSUPPORTED, "map extent needs more than 21 octree levels at this resolution");
   const size_t m = (size_t)h->map_h[0];
   if (out_capacity < m) return fail(B2R_EINVAL, "output capacity too small");
   if (m) {

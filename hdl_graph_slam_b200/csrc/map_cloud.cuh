@@ -115,10 +115,10 @@ __global__ void k_map_keys(const float* __restrict__ cloud, int stride_f, long l
     const float x = p[0], y = p[1], z = p[2];
     unsigned long long key = 0xffffffffffffffffull;  // non-finite points are not inserted (OctreePointCloud::addPointsFromInputCloud)
     if (finite3(x, y, z) && G.defined && !G.overflow) {
-      // genOctreeKeyforPoint: key = static_cast<unsigned int>((point - min) / resolution), float64
-      const unsigned long long kx = (unsigned long long)(((double)x - G.mn[0]) / G.r);
-      const unsigned long long ky = (unsigned long long)(((double)y - G.mn[1]) / G.r);
-      const unsigned long long kz = (unsigned long long)(((double)z - G.mn[2]) / G.r);
+      // genOctreeKeyforPoint: key = static_cast<unsigned int>((point - min) / resolution), float64 (the subtraction explicitly rounded)
+      const unsigned long long kx = (unsigned long long)(dsub((double)x, G.mn[0]) / G.r);
+      const unsigned long long ky = (unsigned long long)(dsub((double)y, G.mn[1]) / G.r);
+      const unsigned long long kz = (unsigned long long)(dsub((double)z, G.mn[2]) / G.r);
       key = (kz << 42) | (ky << 21) | kx;
     }
     keys[g] = key;
@@ -142,10 +142,12 @@ __global__ void k_map_centers(const unsigned long long* __restrict__ keys, const
     const unsigned long long k = keys[g];
     const unsigned long long kx = k & 0x1fffffull, ky = (k >> 21) & 0x1fffffull, kz = k >> 42;
     float* o = out + (size_t)slots[g] * stride_f;
-    // genLeafNodeCenterFromOctreeKey: (key + 0.5f) * resolution + min, float64, narrowed to float
-    o[0] = (float)(((double)kx + 0.5) * G.r + G.mn[0]);
-    o[1] = (float)(((double)ky + 0.5) * G.r + G.mn[1]);
-    o[2] = (float)(((double)kz + 0.5) * G.r + G.mn[2]);
+    // genLeafNodeCenterFromOctreeKey: (key + 0.5f) * resolution + min, float64, narrowed to float.  Multiply and add are rounded
+    // separately (dmul / dadd): a contracted DFMA rounds once and can move the centre by one float64 ulp, which the narrowing to
+    // float may keep
+    o[0] = (float)dadd(dmul(dadd((double)kx, 0.5), G.r), G.mn[0]);
+    o[1] = (float)dadd(dmul(dadd((double)ky, 0.5), G.r), G.mn[1]);
+    o[2] = (float)dadd(dmul(dadd((double)kz, 0.5), G.r), G.mn[2]);
     if (stride_f >= 4) o[3] = 1.0f;
     for (int q = 4; q < stride_f; q++) o[q] = 0.f;
   }

@@ -667,7 +667,7 @@ inline int ndt_ensure_map(const b2r_config& cfg, Cloud& c, NdtWork& W, cudaStrea
   B2R_CUDA(M.table.reserve(tsize));
   B2R_CUDA(B->keys_a.reserve(c.n + 1)); B2R_CUDA(B->vals_a.reserve(c.n + 1)); B2R_CUDA(B->vals_b.reserve(c.n + 1));
   size_t tmp_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, B->keys_a.p, M.keys.p, B->vals_a.p, B->vals_b.p, n, 0, 32, st);
+  B2R_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, B->keys_a.p, M.keys.p, B->vals_a.p, B->vals_b.p, n, 0, 32, st));
   B2R_CUDA(B->sort_tmp.reserve(tmp_bytes + 256));
   TEL_BEGIN(W.tel, st);
   k_grid_reset<<<1, 32, 0, st>>>(B->mm);
@@ -680,7 +680,7 @@ inline int ndt_ensure_map(const b2r_config& cfg, Cloud& c, NdtWork& W, cudaStrea
     k_vox_keys<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, n, M.geom, B->keys_a.p, B->vals_a.p);
     size_t tb = B->sort_tmp.cap;
     // stable LSD radix sort by voxel key: inside a voxel the points stay in ascending index, the order the moments are summed in
-    cub::DeviceRadixSort::SortPairs(B->sort_tmp.p, tb, B->keys_a.p, M.keys.p, B->vals_a.p, B->vals_b.p, n, 0, 32, st);
+    B2R_CUDA(cub::DeviceRadixSort::SortPairs(B->sort_tmp.p, tb, B->keys_a.p, M.keys.p, B->vals_a.p, B->vals_b.p, n, 0, 32, st));
     k_vox_gather<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, n, M.keys.p, B->vals_b.p, M.sorted.p);
     k_vox_finalize<<<(n + 127) / 128, 128, 0, st>>>(M.keys.p, M.sorted.p, M.vox.p, M.cells.p, M.table.p, M.mask, n);
   }

@@ -357,8 +357,8 @@ inline int voxelgrid_device(VoxelWork& W, cudaStream_t st, const float* d_in, si
   B2R_CUDA(W.keys_a.reserve(n)); B2R_CUDA(W.keys_b.reserve(n)); B2R_CUDA(W.vals_a.reserve(n)); B2R_CUDA(W.vals_b.reserve(n));
   B2R_CUDA(W.flags.reserve(n)); B2R_CUDA(W.slots.reserve(n));
   size_t tmp_sort = 0, tmp_scan = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, W.keys_a.p, W.keys_b.p, W.vals_a.p, W.vals_b.p, N, 0, 32, st);
-  cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, W.flags.p, W.slots.p, N, st);
+  B2R_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, W.keys_a.p, W.keys_b.p, W.vals_a.p, W.vals_b.p, N, 0, 32, st));
+  B2R_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, W.flags.p, W.slots.p, N, st));
   B2R_CUDA(W.tmp.reserve(std::max(tmp_sort, tmp_scan) + 256));
   const unsigned nb = (unsigned)((n + 255) / 256);
   TEL_BEGIN(W.tel, st);
@@ -368,10 +368,10 @@ inline int voxelgrid_device(VoxelWork& W, cudaStream_t st, const float* d_in, si
   B2R_CUDA(cudaMemcpyAsync(W.h_geom, W.geom, sizeof(VgGeom), cudaMemcpyDeviceToHost, st));
   k_vg_keys<<<nb, 256, 0, st>>>(d_in, sf, N, W.geom, W.keys_a.p, W.vals_a.p);
   size_t tb = W.tmp.cap;
-  cub::DeviceRadixSort::SortPairs(W.tmp.p, tb, W.keys_a.p, W.keys_b.p, W.vals_a.p, W.vals_b.p, N, 0, 32, st);
+  B2R_CUDA(cub::DeviceRadixSort::SortPairs(W.tmp.p, tb, W.keys_a.p, W.keys_b.p, W.vals_a.p, W.vals_b.p, N, 0, 32, st));
   k_vg_heads<<<nb, 256, 0, st>>>(W.keys_b.p, N, W.flags.p);
   tb = W.tmp.cap;
-  cub::DeviceScan::ExclusiveSum(W.tmp.p, tb, W.flags.p, W.slots.p, N, st);
+  B2R_CUDA(cub::DeviceScan::ExclusiveSum(W.tmp.p, tb, W.flags.p, W.slots.p, N, st));
   k_vg_centroid<<<nb, 256, 0, st>>>(d_in, sf, N, W.keys_b.p, W.vals_b.p, W.flags.p, W.slots.p, W.out.p, sf, W.okeys.p, W.ocounts.p,
                                     (int*)(W.mm + 6));
   TEL_END(W.tel, KC_VOXELGRID, 14, st);

@@ -39,12 +39,14 @@ def pose_matrix(k, step=1.0):
 
 
 def scan(sensor="vlp16", frame=0, step=1.0, sigma=0.02, stride=8, xyyaw=None, roll=0.0, pitch=0.0, seed=None, out=None):
-    """One synthetic scan in the sensor frame: float32 (n, stride) array (stride 8 == pcl::PointXYZI record)."""
+    """One synthetic scan in the sensor frame: float32 (n, stride) array (stride 8 == pcl::PointXYZI record).  `sensor` is a name of
+    SENSORS or a (rings, azimuth steps) pair with 2 to 64 rings; other shapes raise ValueError."""
     rings, n_az = SENSORS[sensor] if isinstance(sensor, str) else sensor
     x, y, th = pose(frame, step) if xyyaw is None else xyyaw
     n = rings * n_az
     if out is None:
         out = np.zeros((n, stride), np.float32)
     sd = (0xB2000000 + frame) if seed is None else seed
-    _load().b2s_scan(rings, n_az, x, y, th, roll, pitch, sd, sigma, out.ctypes.data_as(C.c_void_p), stride)
+    if _load().b2s_scan(rings, n_az, x, y, th, roll, pitch, sd, sigma, out.ctypes.data_as(C.c_void_p), stride) != n:
+        raise ValueError(f"scan shape ({rings}, {n_az}): the generator takes 2 to 64 rings and at least one azimuth step")
     return out

@@ -109,11 +109,14 @@ void b2s_pose(int k, double step, double* x, double* y, double* yaw) {
   *yaw = th + 0.05 * sin(5.0 * th);
 }
 
-/* rings: 16 (VLP-16), 32 (HDL-32e), 64 (KITTI HDL-64E shape). returns number of points = rings*n_az. */
+/* rings: 16 (VLP-16), 32 (HDL-32e), 64 (KITTI HDL-64E shape); any other count from 2 to 64 spreads the beams evenly.
+ * returns number of points = rings*n_az, or 0 (nothing written) for a ring count outside [2, 64] (elev[] holds 64 beams) or
+ * n_az < 1. */
 size_t b2s_scan(int rings, int n_az, double px, double py, double yaw, double roll, double pitch, uint64_t seed, double sigma,
                 float* out, size_t stride) {
-  build_scene();
   double elev[64];
+  if (rings < 2 || rings > 64 || n_az < 1) return 0;
+  build_scene();
   if (rings == 16) for (int r = 0; r < 16; r++) elev[r] = (-15.0 + 2.0 * r) * M_PI / 180.0;
   else if (rings == 32) for (int r = 0; r < 32; r++) elev[r] = (10.67 - (41.34 / 31.0) * r) * M_PI / 180.0;
   else for (int r = 0; r < rings; r++) elev[r] = (2.0 - (26.8 / (rings - 1)) * r) * M_PI / 180.0;

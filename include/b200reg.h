@@ -227,7 +227,9 @@ int b2r_prefilter(b2r_handle* h, const void* points, size_t n, size_t stride_byt
  * resolution <= 0 returns that cloud (intensity kept), otherwise the centres of the occupied voxels of a
  * pcl::octree::OctreePointCloud(resolution) — the same SET of centres as PCL's lattice (anchored at the first finite point),
  * emitted in ascending key order instead of octree traversal order; x,y,z,1 with intensity 0.
- * Returns 1 with *n_out = 0 when there is no keyframe ("warning: keyframes empty!!").  out: capacity out_capacity records. */
+ * Returns 1 with *n_out = 0 when there is no keyframe ("warning: keyframes empty!!").  out: capacity out_capacity records.
+ * Fails with B2R_EUNSUPPORTED when resolution > 0 and the octree needs more than 21 levels to hold every point (the voxel keys
+ * hold 21 bits per axis: e.g. resolution 0.001 with points 3 km apart); PCL would grow a deeper octree. */
 typedef struct b2r_keyframe_snapshot {
   const void* points;  /* KeyFrameSnapshot::cloud: n records of stride_bytes */
   size_t n;

@@ -39,7 +39,10 @@ extern "C" int orc_voxelgrid(const float* in, size_t n, size_t stride, float lea
   if (n == 0 || !(mn[0] <= mx[0])) return 0;
   const float inv = 1.0f / leaf;
   int64_t dx = (int64_t)((mx[0] - mn[0]) * inv) + 1, dy = (int64_t)((mx[1] - mn[1]) * inv) + 1, dz = (int64_t)((mx[2] - mn[2]) * inv) + 1;
-  if (dx * dy * dz > (int64_t)INT_MAX) {  // "Leaf size is too small for the input dataset" -> output = input
+  // PCL forms dx * dy * dz in int64, which overflows (undefined) once the extents pass ~2^21 leaves per axis and can then let a
+  // far too fine grid through; the volume is checked factor by factor instead (as the engine does), without overflow
+  const bool too_small = dx > INT_MAX || dy > INT_MAX || dz > INT_MAX || dx * dy > INT_MAX || dx * dy * dz > INT_MAX;
+  if (too_small) {  // "Leaf size is too small for the input dataset" -> output = input
     for (size_t i = 0; i < n; i++) {
       const float* p = in + i * stride;
       out_xyzi[i * 4 + 0] = p[0]; out_xyzi[i * 4 + 1] = p[1]; out_xyzi[i * 4 + 2] = p[2]; out_xyzi[i * 4 + 3] = has_i ? p[4] : 0.f;

@@ -69,22 +69,33 @@ def test_product_does_not_touch_the_oracle():
                 assert "liboracle" not in txt and "from oracle" not in txt and "import oracle" not in txt, f
 
 
-def test_voxel_finalize_is_not_contracted(tmp_path):
-    """k_vox_finalize decides a voxel's validity on the sign of its smallest eigenvalue, which for a planar or linear voxel is
-    rounding noise: its float64 arithmetic must be the oracle's unfused sequence.  In the PTX of the engine (compiled with the
-    library's own flags) every float64 multiply / add / subtract of the kernel carries an explicit .rn (which ptxas never fuses)
-    and there is no fma.  The SASS of the built library can still hold DFMA: correctly rounded float64 division and square root
-    are DFMA sequences, and those round exactly like the oracle's / and sqrt."""
+def _f64_ops_of_kernel(ptx_text, mangled_prefix):
+    """(op, modifiers) of every float64 multiply / add / subtract / fma in the PTX body of one kernel"""
+    i = ptx_text.index(".entry " + mangled_prefix)
+    body = ptx_text[i:ptx_text.index("\n}\n", i)]
+    return re.findall(r"\b(fma|mad|mul|add|sub)((?:\.\w+)*)\.f64\b", body)
+
+
+@pytest.fixture(scope="module")
+def engine_ptx(tmp_path_factory):
+    """the PTX of the engine, compiled with the library's own flags"""
     from hdl_graph_slam_b200 import build
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
-    ptx = tmp_path / "api.ptx"
+    ptx = tmp_path_factory.mktemp("ptx") / "api.ptx"
     flags = [f for f in build.NVCC_FLAGS if f not in ("-shared", "-Xcompiler", "-fPIC", "-lineinfo")]
     flags = [f.replace("code=sm_90a", "code=compute_90a") for f in flags]
     subprocess.check_call([nvcc] + flags + ["-ptx", "-o", str(ptx), os.path.join(ROOT, "hdl_graph_slam_b200", "csrc", "api.cu")])
-    s = ptx.read_text()
-    i = s.index(".entry _ZN3b2r14k_vox_finalize")
-    body = s[i:s.index("\n}\n", i)]
-    ops = re.findall(r"\b(fma|mad|mul|add|sub)((?:\.\w+)*)\.f64\b", body)
+    return ptx.read_text()
+
+
+def test_voxel_finalize_is_not_contracted(engine_ptx):
+    """k_vox_finalize decides a voxel's validity on the sign of its smallest eigenvalue, which for a planar or linear voxel is
+    rounding noise: its float64 arithmetic must be the oracle's unfused sequence.  In the PTX of the engine every float64
+    multiply / add / subtract of the kernel carries an explicit .rn (which ptxas never fuses) and there is no fma.  The SASS of
+    the built library can still hold DFMA: correctly rounded float64 division and square root are DFMA sequences, and those
+    round exactly like the oracle's / and sqrt."""
+    from hdl_graph_slam_b200 import build
+    ops = _f64_ops_of_kernel(engine_ptx, "_ZN3b2r14k_vox_finalize")
     assert len(ops) > 100  # the eigen-solve is in the kernel
     assert not [o for o in ops if o[0] in ("fma", "mad")], "contracted float64 in k_vox_finalize"
     assert not [o for o in ops if ".rn" not in o[1]], "float64 arithmetic without .rn (ptxas may fuse it) in k_vox_finalize"
@@ -95,6 +106,17 @@ def test_voxel_finalize_is_not_contracted(tmp_path):
     sass = subprocess.run([cuobjdump, "-sass", so], capture_output=True, text=True, check=True).stdout
     fins = [f for f in sass.split("Function : ") if f.startswith("_ZN3b2r14k_vox_finalize")]
     assert len(fins) == 1 and "DMUL" in fins[0]
+
+
+@pytest.mark.parametrize("kernel,min_ops", [("_ZN3b2r13k_map_centers", 9), ("_ZN3b2r10k_map_keys", 3)])
+def test_map_cloud_voxel_arithmetic_is_not_contracted(engine_ptx, kernel, min_ops):
+    """The map cloud's voxel keys (point - min) / resolution and centres ((key + 0.5) * resolution) + min are float64 expressions
+    the oracle rounds after every operation; a multiply-add contracted into one fma rounds once and can move a centre.  The
+    kernels' PTX holds no fma and only explicitly rounded (.rn) float64 multiply / add / subtract."""
+    ops = _f64_ops_of_kernel(engine_ptx, kernel)
+    assert len(ops) >= min_ops  # three axes: add, mul, add each (centres) / sub each (keys)
+    assert not [o for o in ops if o[0] in ("fma", "mad")], f"contracted float64 in {kernel}"
+    assert not [o for o in ops if ".rn" not in o[1]], f"float64 arithmetic without .rn (ptxas may fuse it) in {kernel}"
 
 
 def test_pcd_header_parser_runs_without_gpu(tmp_path):

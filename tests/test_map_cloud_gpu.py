@@ -1,6 +1,6 @@
 """GPU: MapCloudGenerator::generate ("next" row f-3; src/hdl_graph_slam/map_cloud_generator.cpp:13-51) on the device against a numpy
 restatement that follows PCL's sequential octree growth: the concatenated transformed cloud bit-exact, the occupied voxel centres
-equal as a SET (float rounding of the centre aside) — PCL's traversal order is not reproduced (documented in b200reg.h)."""
+equal bit for bit as a SET — PCL's traversal order is not reproduced (documented in b200reg.h)."""
 import numpy as np
 import pytest
 import hdl_graph_slam_b200 as pkg
@@ -33,6 +33,6 @@ def test_voxel_centres_equal_octree_occupied_centres(synth, oracle, res):
     assert got.shape[0] == want.shape[0] and 0 < got.shape[0] < sum(c.shape[0] for c, _ in kfs)
     g = got[:, :3]
     g = g[np.lexsort((g[:, 0], g[:, 1], g[:, 2]))]
-    assert np.max(np.abs(g.astype(np.float64) - want.astype(np.float64))) < 1e-4 * max(res, 0.1)
+    assert np.array_equal(g, want)  # (key + 0.5) * res + min rounded after the multiply and after the add, as the oracle does
     assert np.all(got[:, 3] == 1.0) and np.all(got[:, 4] == 0.0)
     reg.close()

@@ -166,3 +166,12 @@ def test_ndt_align_on_synthetic_pair(oracle, synth):
     # identical clouds, identity guess: stays at identity
     rid = m.align(tgt, np.eye(4, dtype=np.float32))
     assert rid["converged"] and trans_err(rid["T"], np.eye(4)) < 1e-3
+
+
+def test_voxelgrid_leaf_too_small_when_the_grid_volume_overflows_int64(oracle):
+    """pcl::VoxelGrid's "leaf size is too small" guard on a grid of ~3e6 leaves per axis: the volume (~2.8e19) does not fit in
+    int64, so a product formed in one go would wrap and let the grid through; the guard must still fire and pass the input on"""
+    c = np.array([[-60.0, -20.0, -2.0, 1.0, 5.0, 0, 0, 0], [3000.0, 3000.0, 3000.0, 1.0, 7.0, 0, 0, 0]], np.float32)
+    out, keys, counts, rc = oracle.voxelgrid(c, 0.001)
+    assert rc == 1 and np.array_equal(out[:, :3], c[:, :3]) and np.array_equal(out[:, 3], c[:, 4])
+    assert np.all(keys == -1) and np.all(counts == 1)
