@@ -24,6 +24,7 @@
 #include "fitness.cuh"
 #include "ndt.cuh"
 #include "voxelgrid.cuh"
+#include "approx_voxelgrid.cuh"
 #include "prefilter.cuh"
 #include "map_cloud.cuh"
 #include "ingest.cuh"
@@ -1180,6 +1181,41 @@ extern "C" int b2r_voxelgrid_device(b2r_handle* h, const void* d_in, size_t n, s
   return B2R_OK;
 }
 
+static int avg_check(b2r_handle* h, size_t n, size_t stride_bytes, float leaf, const size_t* n_out) {
+  if (!h || !n_out) return fail(B2R_EINVAL, "NULL argument");
+  if (stride_bytes < 12 || (stride_bytes & 3)) return fail(B2R_EINVAL, "bad stride");
+  if (!(leaf > 0.f) || !std::isfinite(leaf)) return fail(B2R_EINVAL, "leaf must be finite and positive");
+  if (n > (size_t)0x3fffffff) return fail(B2R_EINVAL, "too many points");
+  return B2R_OK;
+}
+
+// pcl::ApproximateVoxelGrid<PointXYZI> with setLeafSize(leaf,leaf,leaf) (apps/prefiltering_nodelet.cpp:61-63,138-149)
+extern "C" int b2r_approximate_voxelgrid(b2r_handle* h, const void* in, size_t n, size_t stride_bytes, float leaf, void* out, size_t* n_out,
+                                         int32_t* out_counts) {
+  int rc = avg_check(h, n, stride_bytes, leaf, n_out);
+  if (rc) return rc;
+  if (n && (!in || !out)) return fail(B2R_EINVAL, "NULL argument");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  return approx_voxelgrid_filter(h->vg_work, h->st, in, n, stride_bytes, leaf, out, n_out, out_counts);
+}
+
+extern "C" int b2r_approximate_voxelgrid_device(b2r_handle* h, const void* d_in, size_t n, size_t stride_bytes, float leaf, const void** d_out,
+                                                size_t* n_out) {
+  int rc = avg_check(h, n, stride_bytes, leaf, n_out);
+  if (rc) return rc;
+  if (!d_out || (n && !d_in)) return fail(B2R_EINVAL, "NULL argument");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  *d_out = nullptr; *n_out = 0;
+  if (n == 0) return B2R_OK;
+  size_t m = 0;
+  rc = approx_voxelgrid_device(h->vg_work, h->st, (const float*)d_in, n, stride_bytes, leaf, &m);
+  if (rc) return rc;
+  h->tel.d2h += 4;
+  *d_out = h->vg_work.out.p;
+  *n_out = m;
+  return B2R_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ prefilter chain (next rows)
 // Every stage is device -> device: records in an engine buffer, keep flags and the order-preserving compaction on the GPU; only
 // the 4-byte count of a stage comes back (host-mapped word) because the next stage's launch geometry needs it.
@@ -1358,6 +1394,8 @@ extern "C" int b2r_prefilter(b2r_handle* h, const void* points, size_t n, size_t
   if (!h || !p || !n_out || (n && !points)) return fail(B2R_EINVAL, "NULL argument");
   if (stride_bytes < 12 || (stride_bytes & 3)) return fail(B2R_EINVAL, "bad stride");
   if (n > (size_t)0x3fffffff) return fail(B2R_EINVAL, "too many points");
+  if (p->downsample_method == B2R_DOWNSAMPLE_APPROX_VOXELGRID && !(p->downsample_resolution > 0.f && std::isfinite(p->downsample_resolution)))
+    return fail(B2R_EINVAL, "downsample_resolution must be finite and positive");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   *n_out = 0;
   if (d_out) *d_out = nullptr;
@@ -1397,6 +1435,11 @@ extern "C" int b2r_prefilter(b2r_handle* h, const void* points, size_t n, size_t
     rc = voxelgrid_device(h->vg_work, h->st, cur, m, stride_bytes, p->downsample_resolution, &mv, &overflow);
     if (rc) return rc;
     if (!overflow) { cur = h->vg_work.out.p; m = mv; }  // (the voxel grid writes its own buffer: the ping-pong pair stays free)
+  } else if (p->downsample_method == B2R_DOWNSAMPLE_APPROX_VOXELGRID && m) {  // :61-63, applied at :132
+    size_t mv = 0;
+    rc = approx_voxelgrid_device(h->vg_work, h->st, cur, m, stride_bytes, p->downsample_resolution, &mv);
+    if (rc) return rc;
+    cur = h->vg_work.out.p; m = mv;
   }
   if (p->outlier_removal_method == B2R_OUTLIER_STATISTICAL && m) {  // :133
     rc = pf_statistical(h, cur, m, sf, p->statistical_mean_k, p->statistical_stddev, h->pf_buf[nxt].p, &m);

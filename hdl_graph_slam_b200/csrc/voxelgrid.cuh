@@ -34,6 +34,7 @@ struct VgGeom {
 struct VoxelWork {
   DevBuf<float> in, out;
   DevBuf<int> keys_a, keys_b, vals_a, vals_b, flags, slots, okeys, ocounts;
+  DevBuf<int> buckets;  // approx_voxelgrid.cuh: per hash slot, occupied flag, then the output slot of its last run
   DevBuf<char> tmp;
   int* mm = nullptr;
   VgGeom* geom = nullptr;
@@ -44,7 +45,7 @@ struct VoxelWork {
   bool wide_clusters = false;  // 16-CTA clusters may be launched on this device (set by the handle: cluster16_allowed())
   void release() {
     in.release(); out.release(); keys_a.release(); keys_b.release(); vals_a.release(); vals_b.release(); flags.release(); slots.release();
-    okeys.release(); ocounts.release(); tmp.release();
+    okeys.release(); ocounts.release(); buckets.release(); tmp.release();
     if (mm) cudaFree(mm);
     if (geom) cudaFree(geom);
     if (h_geom) cudaFreeHost(h_geom);
@@ -324,11 +325,8 @@ static cudaError_t launch_voxelgrid_cluster(int shape_index, const VgArgs& A, cu
   }
 }
 
-// device-resident voxel grid: d_in (device records) -> W.out / W.okeys / W.ocounts (device); *m = voxel count, *overflow = PCL's
-// "leaf size too small" condition (output then undefined: the caller passes the input through)
-inline int voxelgrid_device(VoxelWork& W, cudaStream_t st, const float* d_in, size_t n, size_t stride_bytes, float leaf, size_t* m, int* overflow) {
-  const int sf = (int)(stride_bytes / 4);
-  const int N = (int)n;
+// the small device / pinned words of the voxel-grid chains, allocated on first use
+inline int vg_alloc_words(VoxelWork& W) {
   if (!W.mm) {
     B2R_CUDA(cudaMalloc(&W.mm, 8 * sizeof(int)));
     B2R_CUDA(cudaMalloc(&W.geom, sizeof(VgGeom)));
@@ -336,6 +334,16 @@ inline int voxelgrid_device(VoxelWork& W, cudaStream_t st, const float* d_in, si
     B2R_CUDA(cudaHostAlloc(&W.h_total, 4 * sizeof(int), cudaHostAllocMapped));
     B2R_CUDA(cudaHostGetDevicePointer((void**)&W.h_total_dev, W.h_total, 0));
   }
+  return B2R_OK;
+}
+
+// device-resident voxel grid: d_in (device records) -> W.out / W.okeys / W.ocounts (device); *m = voxel count, *overflow = PCL's
+// "leaf size too small" condition (output then undefined: the caller passes the input through)
+inline int voxelgrid_device(VoxelWork& W, cudaStream_t st, const float* d_in, size_t n, size_t stride_bytes, float leaf, size_t* m, int* overflow) {
+  const int sf = (int)(stride_bytes / 4);
+  const int N = (int)n;
+  int rc = vg_alloc_words(W);
+  if (rc) return rc;
   B2R_CUDA(W.out.reserve(n * sf + 8));
   B2R_CUDA(W.okeys.reserve(n + 1)); B2R_CUDA(W.ocounts.reserve(n + 1));
   const BuildShape shape = build_shape_for(n, W.wide_clusters);

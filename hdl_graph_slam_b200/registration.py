@@ -9,6 +9,7 @@ Names follow the reference so that tests read like its call sites:
   ScanMatchingOdometry.matching <- apps/scan_matching_odometry_nodelet.cpp:165-262
   LoopDetector.matching         <- include/hdl_graph_slam/loop_detector.hpp:117-171
   VoxelGrid.filter              <- pcl::VoxelGrid as set up at apps/prefiltering_nodelet.cpp:54-58
+  approximateVoxelGridFilter    <- pcl::ApproximateVoxelGrid as set up at apps/prefiltering_nodelet.cpp:61-63
 
 Clouds are float32 numpy arrays of shape (n, 4) [x,y,z,1] or (n, 8) [pcl::PointXYZI record]; 4x4 poses are ordinary
 row-major numpy matrices (the wrapper converts to the ABI's column-major layout).  All arithmetic happens in the CUDA
@@ -338,6 +339,26 @@ class Registration:
         if with_keys:
             return out[:m], keys[:m], counts[:m], rc
         return out[:m]
+
+    def approximateVoxelGridFilter(self, cloud, leaf, with_counts=False):
+        """pcl::ApproximateVoxelGrid::filter (b2r_approximate_voxelgrid): the outputs in PCL's order; with_counts also returns the
+        number of points behind each output"""
+        a, n, s = _cloud(cloud)
+        out = np.zeros_like(a)
+        n_out = C.c_size_t()
+        counts = np.empty(max(n, 1), np.int32)
+        check(self._lib.b2r_approximate_voxelgrid(self._h, a.ctypes.data_as(C.c_void_p), n, s, leaf, out.ctypes.data_as(C.c_void_p), C.byref(n_out),
+                                                  counts.ctypes.data_as(C.POINTER(C.c_int32))))
+        m = n_out.value
+        if with_counts:
+            return out[:m], counts[:m]
+        return out[:m]
+
+    def approximateVoxelGridFilterDevice(self, d_ptr, n, stride_bytes, leaf):
+        """device pointer in -> (device pointer out, output count): the result stays in HBM (b2r_approximate_voxelgrid_device)"""
+        out, m = C.c_void_p(), C.c_size_t()
+        check(self._lib.b2r_approximate_voxelgrid_device(self._h, C.c_void_p(d_ptr), n, stride_bytes, leaf, C.byref(out), C.byref(m)))
+        return out.value, m.value
 
 
 def select_registration_method(params=None, device_id=0):

@@ -176,6 +176,19 @@ int b2r_voxelgrid(b2r_handle* h, const void* in, size_t n, size_t stride_bytes, 
  * registration without leaving HBM.  Returns 1 with *d_out = d_in when the leaf is too small (pass-through). */
 int b2r_voxelgrid_device(b2r_handle* h, const void* d_in, size_t n, size_t stride_bytes, float leaf, const void** d_out, size_t* n_out);
 
+/* ---- companion: approximate voxel-grid downsample ------------------------------------------------------------------
+ * replaces pcl::ApproximateVoxelGrid<PointXYZI>::filter with setLeafSize(leaf,leaf,leaf) and its 512-slot hash table
+ * (apps/prefiltering_nodelet.cpp:61-63,138-149; downsample_method "APPROX_VOXELGRID").  Records as for b2r_voxelgrid; the outputs
+ * come in PCL's order (flushes on hash collisions in input order, then the remaining slots 0..511), and one cell may appear more
+ * than once.  out must hold n records; *n_out receives the output count; out_counts (capacity n, may be NULL) the points per output.
+ * Non-finite points are not skipped (PCL has no check).  B2R_EINVAL for a leaf that is not finite and positive or a bad stride. */
+int b2r_approximate_voxelgrid(b2r_handle* h, const void* in, size_t n, size_t stride_bytes, float leaf, void* out, size_t* n_out,
+                              int32_t* out_counts);
+/* the same filter with input and output resident in device memory: *d_out receives an engine-owned device buffer of *n_out records
+ * (valid until the next voxel-grid or prefilter call on this handle) for b2r_set_source_device and the other device entry points. */
+int b2r_approximate_voxelgrid_device(b2r_handle* h, const void* d_in, size_t n, size_t stride_bytes, float leaf, const void** d_out,
+                                     size_t* n_out);
+
 /* ---- "next" rows (SURVEY.md 8f-2): the rest of the prefilter chain.  Records are copied whole; kept points stay in input order.
  * PrefilteringNodelet::distance_filter (apps/prefiltering_nodelet.cpp:164-180): keep near < ||p|| < far (float32 norm). */
 int b2r_distance_filter(b2r_handle* h, const void* in, size_t n, size_t stride_bytes, double near_thresh, double far_thresh, void* out, size_t* n_out);
@@ -197,6 +210,7 @@ int b2r_deskew(b2r_handle* h, const void* in, size_t n, size_t stride_bytes, dou
  * not NULL (capacity n records). */
 #define B2R_DOWNSAMPLE_NONE 0
 #define B2R_DOWNSAMPLE_VOXELGRID 1
+#define B2R_DOWNSAMPLE_APPROX_VOXELGRID 2  /* :59-63; any other value passes the cloud through, as the reference does (:64-70) */
 #define B2R_OUTLIER_NONE 0
 #define B2R_OUTLIER_STATISTICAL 1
 #define B2R_OUTLIER_RADIUS 2
@@ -209,7 +223,7 @@ typedef struct b2r_prefilter_params {
   int32_t use_distance_filter;    /* "use_distance_filter" (true)                           :96                          */
   double distance_near_thresh;    /* 1.0                                                    :97                          */
   double distance_far_thresh;     /* 100.0                                                  :98                          */
-  int32_t downsample_method;      /* "downsample_method" VOXELGRID                          :51                          */
+  int32_t downsample_method;      /* "downsample_method" VOXELGRID (or NONE, APPROX_VOXELGRID) :51                        */
   float downsample_resolution;    /* 0.1                                                    :52                          */
   int32_t outlier_removal_method; /* "outlier_removal_method" STATISTICAL                   :71                          */
   int32_t statistical_mean_k;     /* 20                                                     :73                          */
