@@ -66,7 +66,7 @@ class OdometryParams(C.Structure):
     _fields_ = [
         ("keyframe_delta_trans", C.c_double), ("keyframe_delta_angle", C.c_double), ("keyframe_delta_time", C.c_double),
         ("transform_thresholding", C.c_int32), ("max_acceptable_trans", C.c_double), ("max_acceptable_angle", C.c_double),
-        ("publish_status", C.c_int32),
+        ("publish_status", C.c_int32), ("downsample_method", C.c_int32), ("downsample_resolution", C.c_float),
     ]
 
 

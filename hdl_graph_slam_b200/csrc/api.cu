@@ -16,6 +16,7 @@
 #include <string>
 #include <vector>
 #include <algorithm>
+#include <functional>
 #include <cub/device/device_radix_sort.cuh>
 #include "engine.cuh"
 #include "gicp.cuh"
@@ -780,7 +781,10 @@ static bool report_consistent(const volatile unsigned long long* flag, unsigned 
 
 // Run the handle's single pair from `mode` at pose x (row-major 3x4 in x[0..11]) until its report lands in mapped memory.
 // Rounds are enqueued ahead of the device (no host wait per iteration); a finished pair's remaining rounds exit at once.
-static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, const LmCfg& cfg, int first_batch, bool cov_beside_first_search = false) {
+// `between` (may be null) runs on the host once the first rounds are enqueued and before the wait for the report: host work that
+// blocks on another stream (the odometry's next-frame downsample) then overlaps the align instead of delaying its enqueue.
+static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, const LmCfg& cfg, int first_batch, bool cov_beside_first_search = false,
+                           const std::function<int()>* between = nullptr) {
   Cloud& s = SRC(h);
   Cloud& t = TGT(h);
   PairDev P;
@@ -834,6 +838,7 @@ static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, co
   };
   int rc = enqueue(first_batch);
   if (rc) return rc;
+  const int rc_between = between ? (*between)() : B2R_OK;  // its error is returned once this align has finished
   const volatile unsigned long long* flag = h->h_pflag;
   const volatile unsigned long long* prog = h->h_pflag + 1;
   const volatile unsigned long long* w = reinterpret_cast<const volatile unsigned long long*>(h->h_rep);
@@ -860,7 +865,7 @@ static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, co
   }
   h->last_rounds = h->h_rep->rounds;
   h->tel.d2h += sizeof(PairReport);
-  return B2R_OK;
+  return rc_between;
 }
 
 static void store_result(b2r_handle* h, const float* T_row, bool converged, int iterations, b2r_result* out) {
@@ -875,7 +880,7 @@ static void store_result(b2r_handle* h, const float* T_row, bool converged, int 
   }
 }
 
-static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out) {
+static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out, const std::function<int()>* between = nullptr) {
   Cloud& s = SRC(h);
   Cloud& t = TGT(h);
   double x0[16];
@@ -885,7 +890,7 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out) {
   for (int i = 0; i < 16; i++) Tg[i] = (float)x0[i];
   if (s.n == 0 || t.n == 0) {  // pcl::Registration::initCompute fails silently: converged_ = false
     store_result(h, Tg, false, 0, out);
-    return B2R_OK;
+    return between ? (*between)() : B2R_OK;
   }
   static const bool overlap = !getenv("B2R_NO_COV_OVERLAP");
   const bool cov_beside = overlap && !s.cov_ready;  // see run_single_pair
@@ -904,7 +909,7 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out) {
   // enqueue as many rounds as the previous align needed (consecutive frames need the same number almost always): a finished
   // pair's surplus rounds exit at once, a shortfall is topped up while the device works
   const int predicted = h->last_rounds > 0 ? h->last_rounds : 5;
-  rc = run_single_pair(h, x0, PM_FIRST, 0, cfg, predicted < 2 ? 2 : predicted, cov_beside);
+  rc = run_single_pair(h, x0, PM_FIRST, 0, cfg, predicted < 2 ? 2 : predicted, cov_beside, between);
   if (rc) return rc;
   const PairReport& rep = *h->h_rep;
   h->cur = rep.cur;
@@ -916,11 +921,12 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out) {
   return B2R_OK;
 }
 
-extern "C" int b2r_align(b2r_handle* h, const float guess[16], b2r_result* out) {
+// b2r_align; `between` as in run_single_pair (GICP only: the NDT Newton loop is host-driven and has no single enqueue point)
+static int align_impl(b2r_handle* h, const float guess[16], b2r_result* out, const std::function<int()>* between) {
   if (!h || !guess) return fail(B2R_EINVAL, "NULL argument");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   int rc;
-  if (h->cfg.method == B2R_METHOD_GICP) rc = gicp_align(h, guess, out);
+  if (h->cfg.method == B2R_METHOD_GICP) rc = gicp_align(h, guess, out, between);
   else {
     float Tfinal[16];
     bool conv = false;
@@ -935,6 +941,8 @@ extern "C" int b2r_align(b2r_handle* h, const float guess[16], b2r_result* out) 
   }
   return rc;
 }
+
+extern "C" int b2r_align(b2r_handle* h, const float guess[16], b2r_result* out) { return align_impl(h, guess, out, nullptr); }
 
 // ------------------------------------------------------------------------------------------------ outputs
 extern "C" int b2r_get_aligned(b2r_handle* h, void* out_points, size_t n, size_t stride_bytes) {
@@ -1677,7 +1685,37 @@ struct b2r_odometry {
   const void* next_ptr = nullptr;
   size_t next_n = 0, next_stride = 0;
   bool next_device = false, next_pending = false;
+  // downsample() (:147-157) with downsample_method VOXELGRID / APPROX_VOXELGRID: the mirror's own voxel-grid work spaces, never the
+  // handle's vg_work, whose output may be the very cloud passed in (b2r_prefilter's or b2r_voxelgrid_device's d_out).
+  // Which filtered clouds must coexist: a GICP handle registers a device cloud by pointer (upload: raw_view) and reads it while
+  // the cloud's BVH and covariances are built, and in b2r_get_aligned while it is the source.  Those builds have finished when
+  // the align that first uses the cloud returns (its report is written after the accumulate kernel that reads the covariances).
+  // A promoted target's raw_view is never read again: b2r_promote_source_to_target finds its BVH and covariances built, and the
+  // align, the fitness and the nearest-neighbour searches read the target's sorted copy only.  An NDT handle copies a device
+  // cloud on the main stream.  So two slots are enough: the current frame's cloud (slot `cur`) and the prefetched next one
+  // (slot cur ^ 1).  An unprefetched frame is filtered into `cur` on the main stream, behind every kernel that read the previous
+  // frame there, and never into cur ^ 1, which the prefetch stream may still be reading (an announced cloud that was not adopted).
+  // The prefetch writes cur ^ 1 on the prefetch stream after `ev_free`, recorded on the main stream once the current cloud has
+  // been set: whatever the main stream had enqueued on the slot's previous cloud (e.g. the first keyframe's covariances) is done.
+  // Each slot's `in` holds a host cloud's upload, its `out` the filtered records.
+  VoxelWork vw[2];
+  int cur = 0;
+  cudaEvent_t ev_free = nullptr;
+  int device_id = 0;
+  // the prefetched frame: identity of the announced RAW cloud, and its filtered copy as handed to b2r_prefetch_source_device
+  bool pf_valid = false;
+  int pf_slot = 0;
+  const void* pf_ptr = nullptr;
+  size_t pf_n = 0, pf_stride = 0;
+  bool pf_device = false;
+  unsigned long long pf_stamp = 0;
+  const float* pf_out = nullptr;
+  size_t pf_m = 0;
 };
+
+static bool odometry_downsamples(const b2r_odometry_params& p) {
+  return p.downsample_method == B2R_DOWNSAMPLE_VOXELGRID || p.downsample_method == B2R_DOWNSAMPLE_APPROX_VOXELGRID;  // else PassThrough
+}
 
 static void mat4_identity(float* m) { for (int i = 0; i < 16; i++) m[i] = (i % 5 == 0) ? 1.f : 0.f; }
 static void mat4_mul(const float* a, const float* b, float* o) {
@@ -1724,19 +1762,97 @@ static void row_to_col(const float* r, float* c) {
 
 extern "C" int b2r_odometry_create(b2r_handle* reg, const b2r_odometry_params* p, b2r_odometry** out) {
   if (!reg || !out) return fail(B2R_EINVAL, "NULL argument");
+  *out = nullptr;
+  // the filters' own argument checks (b2r_voxelgrid, b2r_approximate_voxelgrid), made once here instead of on every frame
+  if (p && p->downsample_method == B2R_DOWNSAMPLE_VOXELGRID && !(p->downsample_resolution > 0.f))
+    return fail(B2R_EINVAL, "downsample_resolution must be positive");
+  if (p && p->downsample_method == B2R_DOWNSAMPLE_APPROX_VOXELGRID && !(p->downsample_resolution > 0.f && std::isfinite(p->downsample_resolution)))
+    return fail(B2R_EINVAL, "downsample_resolution must be finite and positive");
   b2r_odometry* o = new b2r_odometry();
   o->reg = reg;
   if (p) o->p = *p;
-  else {
+  else {  // and downsample_method NONE
     o->p.keyframe_delta_trans = 0.25; o->p.keyframe_delta_angle = 0.15; o->p.keyframe_delta_time = 1.0;
     o->p.transform_thresholding = 0; o->p.max_acceptable_trans = 1.0; o->p.max_acceptable_angle = 1.0; o->p.publish_status = 0;
+  }
+  o->device_id = reg->cfg.device_id;
+  if (odometry_downsamples(o->p)) {
+    if (cudaSetDevice(o->device_id) != cudaSuccess || cudaEventCreateWithFlags(&o->ev_free, cudaEventDisableTiming) != cudaSuccess) {
+      delete o;
+      return fail(B2R_ECUDA, "cudaEventCreate failed");
+    }
+    for (VoxelWork& W : o->vw) { W.tel = &reg->tel; W.wide_clusters = cluster16_allowed(); }
   }
   mat4_identity(o->prev_trans);
   mat4_identity(o->keyframe_pose);
   *out = o;
   return B2R_OK;
 }
-extern "C" void b2r_odometry_destroy(b2r_odometry* o) { delete o; }
+extern "C" void b2r_odometry_destroy(b2r_odometry* o) {
+  if (!o) return;
+  if (o->ev_free) {
+    cudaSetDevice(o->device_id);
+    o->vw[0].release(); o->vw[1].release();  // (cudaFree waits for kernels still reading them, e.g. an unadopted prefetch)
+    cudaEventDestroy(o->ev_free);
+  }
+  delete o;
+}
+
+static int odometry_check_cloud(const void* cloud, size_t n, size_t stride_bytes) {
+  if (stride_bytes < 12 || (stride_bytes & 3)) return fail(B2R_EINVAL, "stride_bytes must be a multiple of 4 and >= 12");
+  if (n > 0 && !cloud) return fail(B2R_EINVAL, "points is NULL");
+  if (n > (size_t)0x3fffffff) return fail(B2R_EINVAL, "too many points");
+  return B2R_OK;
+}
+
+// downsample(cloud) (:147-157) into slot `slot` on stream `st`: *d_reg / *m_reg = the device cloud to register.  Both filters read
+// their output count back to the host, so the stream has drained when this returns: a host cloud's buffer (pinned or pageable) is
+// then free again, as b2r_set_source promises.
+static int odometry_downsample(b2r_odometry* o, int slot, cudaStream_t st, const void* cloud, size_t n, size_t stride, bool device,
+                               const float** d_reg, size_t* m_reg) {
+  b2r_handle* h = o->reg;
+  VoxelWork& W = o->vw[slot];
+  const float* d_in = (const float*)cloud;
+  if (!device) {
+    B2R_CUDA(W.in.reserve(n * (stride / 4) + 4));
+    if (n) B2R_CUDA(cudaMemcpyAsync(W.in.p, cloud, n * stride, cudaMemcpyHostToDevice, st));
+    h->tel.h2d += n * stride;
+    d_in = W.in.p;
+  }
+  *d_reg = d_in;
+  *m_reg = n;
+  if (n == 0) return B2R_OK;
+  size_t m = 0;
+  if (o->p.downsample_method == B2R_DOWNSAMPLE_VOXELGRID) {
+    int overflow = 0;
+    int rc = voxelgrid_device(W, st, d_in, n, stride, o->p.downsample_resolution, &m, &overflow);
+    if (rc) return rc;
+    h->tel.d2h += 8;
+    if (overflow) return B2R_OK;  // PCL: "Leaf size is too small": the cloud passes through (as b2r_voxelgrid_device)
+  } else {
+    int rc = approx_voxelgrid_device(W, st, d_in, n, stride, o->p.downsample_resolution, &m);
+    if (rc) return rc;
+    h->tel.d2h += 4;
+  }
+  *d_reg = W.out.p;
+  *m_reg = m;
+  return B2R_OK;
+}
+
+// this frame's filtered cloud: the prefetched one if `cloud` is the announced raw cloud (same pointer, size and stride, and for a
+// host cloud the same content stamp), else filtered afresh on the main stream
+static int odometry_take(b2r_odometry* o, const void* cloud, size_t n, size_t stride, bool device, const float** d_reg, size_t* m_reg) {
+  const bool hit = o->pf_valid && o->pf_ptr == cloud && o->pf_n == n && o->pf_stride == stride && o->pf_device == device &&
+                   (device || content_stamp(cloud, n, stride) == o->pf_stamp);
+  o->pf_valid = false;
+  if (hit) {
+    o->cur = o->pf_slot;
+    *d_reg = o->pf_out;
+    *m_reg = o->pf_m;
+    return B2R_OK;
+  }
+  return odometry_downsample(o, o->cur, o->reg->st, cloud, n, stride, device, d_reg, m_reg);
+}
 
 static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* cloud, size_t n, size_t stride_bytes, const float* msf_delta,
                                   b2r_odometry_status* out, bool device);
@@ -1748,8 +1864,47 @@ extern "C" int b2r_odometry_prefetch(b2r_odometry* o, const void* cloud, size_t 
 static int odometry_issue_prefetch(b2r_odometry* o) {
   if (!o->next_pending) return B2R_OK;
   o->next_pending = false;
-  return o->next_device ? b2r_prefetch_source_device(o->reg, o->next_ptr, o->next_n, o->next_stride)
-                        : b2r_prefetch_source(o->reg, o->next_ptr, o->next_n, o->next_stride);
+  if (!odometry_downsamples(o->p))
+    return o->next_device ? b2r_prefetch_source_device(o->reg, o->next_ptr, o->next_n, o->next_stride)
+                          : b2r_prefetch_source(o->reg, o->next_ptr, o->next_n, o->next_stride);
+  // downsample the announced cloud on the prefetch stream, then let b2r_prefetch_source_device build its BVH and covariances
+  // there: the next matching() hands the filtered buffer to b2r_set_source_device, whose adoption test recognises it
+  b2r_handle* h = o->reg;
+  int rc = odometry_check_cloud(o->next_ptr, o->next_n, o->next_stride);
+  if (rc) return rc;
+  const int slot = o->cur ^ 1;
+  B2R_CUDA(cudaStreamWaitEvent(h->st2, o->ev_free, 0));
+  const unsigned long long stamp = o->next_device ? 0 : content_stamp(o->next_ptr, o->next_n, o->next_stride);
+  const float* d = nullptr;
+  size_t m = 0;
+  rc = odometry_downsample(o, slot, h->st2, o->next_ptr, o->next_n, o->next_stride, o->next_device, &d, &m);
+  if (rc) return rc;
+  rc = b2r_prefetch_source_device(h, d, m, o->next_stride);
+  if (rc) return rc;
+  o->pf_valid = true; o->pf_slot = slot;
+  o->pf_ptr = o->next_ptr; o->pf_n = o->next_n; o->pf_stride = o->next_stride; o->pf_device = o->next_device; o->pf_stamp = stamp;
+  o->pf_out = d; o->pf_m = m;
+  return B2R_OK;
+}
+
+// setInputTarget / setInputSource(downsample(cloud)) (:171-172, :176-177); *n_reg = the number of points registered
+static int odometry_set_cloud(b2r_odometry* o, bool is_target, const void* cloud, size_t n, size_t stride_bytes, bool device, size_t* n_reg) {
+  b2r_handle* reg = o->reg;
+  *n_reg = n;
+  if (!odometry_downsamples(o->p)) {  // PassThrough: the cloud as given
+    if (is_target) return device ? b2r_set_target_device(reg, cloud, n, stride_bytes) : b2r_set_target(reg, cloud, n, stride_bytes);
+    return device ? b2r_set_source_device(reg, cloud, n, stride_bytes) : b2r_set_source(reg, cloud, n, stride_bytes);
+  }
+  int rc = odometry_check_cloud(cloud, n, stride_bytes);
+  if (rc) return rc;
+  B2R_CUDA(cudaSetDevice(reg->cfg.device_id));
+  const float* d = nullptr;
+  rc = odometry_take(o, cloud, n, stride_bytes, device, &d, n_reg);
+  if (rc) return rc;
+  rc = is_target ? b2r_set_target_device(reg, d, *n_reg, stride_bytes) : b2r_set_source_device(reg, d, *n_reg, stride_bytes);
+  if (rc) return rc;
+  B2R_CUDA(cudaEventRecord(o->ev_free, reg->st));
+  return B2R_OK;
 }
 
 extern "C" int b2r_odometry_matching(b2r_odometry* o, double stamp, const void* cloud, size_t n, size_t stride_bytes,
@@ -1774,7 +1929,8 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
     mat4_identity(o->prev_trans);
     mat4_identity(o->keyframe_pose);
     o->keyframe_stamp = stamp;
-    int rc = device ? b2r_set_target_device(reg, cloud, n, stride_bytes) : b2r_set_target(reg, cloud, n, stride_bytes);
+    size_t n_reg = 0;
+    int rc = odometry_set_cloud(o, true, cloud, n, stride_bytes, device, &n_reg);  // keyframe = downsample(cloud)
     if (rc) return rc;
     rc = odometry_issue_prefetch(o);
     if (rc) return rc;
@@ -1784,10 +1940,18 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
     out->keyframe_updated = 1;
     return B2R_OK;
   }
-  int rc = device ? b2r_set_source_device(reg, cloud, n, stride_bytes) : b2r_set_source(reg, cloud, n, stride_bytes);  // :177
+  size_t n_reg = 0;  // aligned->size() of :321
+  int rc = odometry_set_cloud(o, false, cloud, n, stride_bytes, device, &n_reg);  // :176-177
   if (rc) return rc;
-  rc = odometry_issue_prefetch(o);  // the NEXT frame's upload / BVH / covariances overlap this frame's align on a second stream
-  if (rc) return rc;
+  // the NEXT frame's upload / BVH / covariances overlap this frame's align on a second stream.  Its downsample waits on the host
+  // for the filter's output count; on a GICP handle it is therefore issued from inside the align, once the align's first rounds
+  // are on the main stream, so that the wait does not hold them back
+  const bool prefetch_in_align = odometry_downsamples(o->p) && reg->cfg.method == B2R_METHOD_GICP;
+  if (!prefetch_in_align) {
+    rc = odometry_issue_prefetch(o);
+    if (rc) return rc;
+  }
+  const std::function<int()> issue_prefetch = [o]() { return odometry_issue_prefetch(o); };
   float guess_row[16], delta_row[16];
   if (msf_delta) { for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) delta_row[r * 4 + c] = msf_delta[c * 4 + r]; }
   else mat4_identity(delta_row);
@@ -1795,7 +1959,7 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
   float guess_col[16];
   row_to_col(guess_row, guess_col);
   b2r_result res;
-  rc = b2r_align(reg, guess_col, &res);
+  rc = align_impl(reg, guess_col, &res, prefetch_in_align ? &issue_prefetch : nullptr);
   if (rc) return rc;
   out->converged = res.converged;
   out->iterations = res.iterations;
@@ -1806,7 +1970,7 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
     rc = b2r_fitness(reg, nullptr, DBL_MAX, 0.5f * 0.5f, &score, &used, &inl);
     if (rc) return rc;
     out->matching_error = score;
-    out->inlier_fraction = n ? (float)inl / (float)n : 0.f;
+    out->inlier_fraction = n_reg ? (float)inl / (float)n_reg : 0.f;
   }
   float odom_row[16];
   if (!res.converged) {  // :214-218

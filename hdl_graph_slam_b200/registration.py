@@ -377,14 +377,19 @@ def select_registration_method(params=None, device_id=0):
 
 
 class ScanMatchingOdometry:
-    """Mirror of ScanMatchingOdometryNodelet's matching() state machine (keyframe, prev_trans, thresholds)."""
+    """Mirror of ScanMatchingOdometryNodelet's matching() state machine (keyframe, prev_trans, thresholds).
+
+    downsample_method / downsample_resolution are the odometry nodelet's own downsample (:83-103): B2R_DOWNSAMPLE_VOXELGRID or
+    B2R_DOWNSAMPLE_APPROX_VOXELGRID filter every cloud on the device before it is registered; B2R_DOWNSAMPLE_NONE (the default here,
+    and what every shipped launch file sets) and unknown values register the cloud as given."""
 
     def __init__(self, registration, keyframe_delta_trans=0.25, keyframe_delta_angle=0.15, keyframe_delta_time=1.0,
-                 transform_thresholding=False, max_acceptable_trans=1.0, max_acceptable_angle=1.0, publish_status=False):
+                 transform_thresholding=False, max_acceptable_trans=1.0, max_acceptable_angle=1.0, publish_status=False,
+                 downsample_method=_capi.B2R_DOWNSAMPLE_NONE, downsample_resolution=0.1):
         self._lib = _capi.load()
         self.registration = registration
         p = OdometryParams(keyframe_delta_trans, keyframe_delta_angle, keyframe_delta_time, int(transform_thresholding),
-                           max_acceptable_trans, max_acceptable_angle, int(publish_status))
+                           max_acceptable_trans, max_acceptable_angle, int(publish_status), int(downsample_method), float(downsample_resolution))
         self._o = C.c_void_p()
         check(self._lib.b2r_odometry_create(registration._h, C.byref(p), C.byref(self._o)))
         self._keep = []

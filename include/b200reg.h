@@ -281,6 +281,9 @@ typedef struct b2r_odometry_params {
   double max_acceptable_trans;  /* :80 */
   double max_acceptable_angle;  /* :81 */
   int32_t publish_status;       /* 1: also compute fitness + inlier fraction each frame (status topic subscribed, :298-335) */
+  int32_t downsample_method;    /* "downsample_method" :83-103: B2R_DOWNSAMPLE_* (0 = NONE, the cloud as given; unknown values pass
+                                   through).  Every shipped launch file sets NONE (the prefilter has already downsampled). */
+  float downsample_resolution;  /* "downsample_resolution" :84 (0.1): leaf of VOXELGRID / APPROX_VOXELGRID */
 } b2r_odometry_params;
 typedef struct b2r_odometry_status {
   float odom[16];           /* keyframe_pose * trans, column-major (return value of matching(), :165-262) */
@@ -293,10 +296,15 @@ typedef struct b2r_odometry_status {
   float inlier_fraction;    /* (status only) */
   int32_t reserved;
 } b2r_odometry_status;
+/* p == NULL: the code defaults above, downsample NONE.  B2R_EINVAL when downsample_method is VOXELGRID and downsample_resolution is
+ * not positive, or APPROX_VOXELGRID and it is not finite and positive (the checks of b2r_voxelgrid / b2r_approximate_voxelgrid). */
 int b2r_odometry_create(b2r_handle* registration, const b2r_odometry_params* p, b2r_odometry** out);
 void b2r_odometry_destroy(b2r_odometry* o);
 /* ScanMatchingOdometryNodelet::matching(stamp, cloud) (apps/scan_matching_odometry_nodelet.cpp:165-262);
- * msf_delta may be NULL (identity). */
+ * msf_delta may be NULL (identity).  With downsample_method VOXELGRID / APPROX_VOXELGRID the cloud is filtered first, on the device
+ * and in buffers the odometry owns (never the handle's voxel-grid buffer, so b2r_prefilter's d_out may be passed on the same handle),
+ * exactly as b2r_voxelgrid_device / b2r_approximate_voxelgrid_device would (including the "leaf too small" pass-through); the
+ * filtered cloud is what is registered, becomes the keyframe, and is the denominator of inlier_fraction. */
 int b2r_odometry_matching(b2r_odometry* o, double stamp, const void* cloud, size_t n, size_t stride_bytes, const float* msf_delta,
                           b2r_odometry_status* out);
 
@@ -305,7 +313,9 @@ int b2r_odometry_matching_device(b2r_odometry* o, double stamp, const void* d_cl
                                  b2r_odometry_status* out);
 
 /* announce the cloud of the NEXT matching() call: the following matching() prefetches it (b2r_prefetch_source) right after it
- * has set its own source, so the next frame's preprocessing overlaps this frame's align.  device != 0: device pointer */
+ * has set its own source, so the next frame's preprocessing overlaps this frame's align.  device != 0: device pointer.
+ * With a downsample, the prefetch also filters the announced cloud on the prefetch stream; the next matching() uses that result only
+ * if it is given the same raw cloud (pointer, n, stride and, for a host cloud, the same content), and filters afresh otherwise. */
 int b2r_odometry_prefetch(b2r_odometry* o, const void* cloud, size_t n, size_t stride_bytes, int device);
 
 /* LoopDetector::matching (include/hdl_graph_slam/loop_detector.hpp:117-171): align every candidate against the new
