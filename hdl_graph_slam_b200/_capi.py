@@ -147,6 +147,7 @@ SYMBOLS = [
     ("b2r_batch_synchronize", C.c_int, [_VP]),
     ("b2r_batch_align", C.c_int, [_VP, C.POINTER(Pair), _SZ, C.c_int, C.c_double, C.POINTER(Result)]),
     ("b2r_batch_calc_fitness_score", C.c_int, [_VP, C.POINTER(Pair), _SZ, C.c_double, _F64P]),
+    ("b2r_batch_map_cloud_generate", C.c_int, [_VP, _I32P, _F32P, _SZ, C.c_double, _SZ, _VP, _SZ, C.POINTER(_VP), C.POINTER(_SZ)]),
     ("b2r_information_params_default", C.c_int, [C.POINTER(InformationParams)]),
     ("b2r_information_from_fitness", C.c_int, [C.POINTER(InformationParams), C.c_double, _F64P]),
     ("b2r_batch_last_rounds", C.c_int, [_VP, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),

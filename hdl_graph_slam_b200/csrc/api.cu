@@ -1573,6 +1573,57 @@ extern "C" int b2r_ingest_pcd(b2r_handle* h, const char* path, const void** d_po
 }
 
 // ------------------------------------------------------------------------------------------------ map cloud ("next" row f-3)
+static unsigned map_blocks(const b2r_handle* h, size_t total) { return (unsigned)std::min<size_t>((total + 255) / 256, (size_t)h->n_sm * 16); }
+
+// The octree stage of MapCloudGenerator::generate, shared by both map entry points: the concatenated transformed cloud (`total`
+// records of cloud_sf floats on the device, non-finite points are not inserted) -> *m occupied-voxel centres at `out` (device,
+// records of out_sf floats).  Synchronises the engine stream.
+static int map_voxel_centres(b2r_handle* h, const float* cloud, int cloud_sf, size_t total, double resolution, float* out, int out_sf, size_t* m) {
+  cudaStream_t st = h->st;
+  const long long T = (long long)total;
+  const unsigned nb = map_blocks(h, total);
+  // voxel keys -> sort -> unique -> centres
+  B2R_CUDA(h->map_keys[0].reserve(total + 8));
+  B2R_CUDA(h->map_keys[1].reserve(total + 8));
+  B2R_CUDA(h->tmp_i.reserve(2 * total + 16));
+  int* flags = h->tmp_i.p;
+  int* slots = h->tmp_i.p + total + 8;
+  size_t tmp_sort = 0, tmp_scan = 0;
+  B2R_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_sort, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st));
+  B2R_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, flags, slots, (int)total, st));
+  B2R_CUDA(h->bc[0].sort_tmp.reserve(std::max(tmp_sort, tmp_scan) + 256));
+  if (!h->map_geom) {
+    B2R_CUDA(cudaMalloc(&h->map_geom, sizeof(MapGeom) + 64));
+    B2R_CUDA(cudaMallocHost(&h->map_h, 64));
+  }
+  unsigned long long* first_idx = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(h->map_geom) + sizeof(MapGeom));
+  int* n_dev = reinterpret_cast<int*>(first_idx + 1);
+  { TEL_BEGIN(&h->tel, st);
+    // replay of the octree's bounding-box growth: each round finds the first point outside the box and grows the box for it; the
+    // box settles after ~log2(extent / resolution) rounds, further rounds exit at once (G.done)
+    k_oct_init<<<1, 1, 0, st>>>(h->map_geom, resolution, first_idx);
+    for (int round = 0; round < 48; round++) {
+      k_oct_first_violator<<<nb, 256, 0, st>>>(cloud, cloud_sf, T, h->map_geom, first_idx);
+      k_oct_grow<<<1, 1, 0, st>>>(cloud, cloud_sf, h->map_geom, first_idx);
+    }
+    k_map_keys<<<nb, 256, 0, st>>>(cloud, cloud_sf, T, h->map_geom, h->map_keys[0].p);
+    size_t tb = h->bc[0].sort_tmp.cap;
+    B2R_CUDA(cub::DeviceRadixSort::SortKeys(h->bc[0].sort_tmp.p, tb, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st));
+    k_map_heads<<<nb, 256, 0, st>>>(h->map_keys[1].p, T, flags);
+    tb = h->bc[0].sort_tmp.cap;
+    B2R_CUDA(cub::DeviceScan::ExclusiveSum(h->bc[0].sort_tmp.p, tb, flags, slots, (int)total, st));
+    k_map_centers<<<nb, 256, 0, st>>>(h->map_keys[1].p, flags, slots, T, h->map_geom, out_sf, out, n_dev);
+    TEL_END(&h->tel, KC_MISC, 106, st); }
+  B2R_CUDA(cudaGetLastError());
+  B2R_CUDA(cudaMemcpyAsync(h->map_h, n_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(h->map_h + 1, &h->map_geom->overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaStreamSynchronize(st));
+  // the octree keys hold 21 bits per axis: a deeper box leaves every point uninserted, which must not pass for an empty map
+  if (h->map_h[1]) return fail(B2R_EUNSUPPORTED, "map extent needs more than 21 octree levels at this resolution");
+  *m = (size_t)h->map_h[0];
+  return B2R_OK;
+}
+
 extern "C" int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot* keyframes, size_t n_keyframes, size_t stride_bytes, double resolution,
                                       void* out, size_t out_capacity, size_t* n_out) {
   if (!h || !n_out) return fail(B2R_EINVAL, "NULL argument");
@@ -1610,10 +1661,8 @@ extern "C" int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot
   B2R_CUDA(h->map_kf.reserve(kf2.size() * sizeof(MapKf) + 64));
   B2R_CUDA(cudaMemcpyAsync(h->map_kf.p, kf2.data(), kf2.size() * sizeof(MapKf), cudaMemcpyHostToDevice, st));
   B2R_CUDA(cudaStreamSynchronize(st));  // kf2 is pageable host memory on the stack of this call
-  const long long T = (long long)total;
-  unsigned nb = (unsigned)std::min<size_t>((total + 255) / 256, (size_t)h->n_sm * 16);
   { TEL_BEGIN(&h->tel, st);
-    k_map_transform<<<nb, 256, 0, st>>>(reinterpret_cast<const MapKf*>(h->map_kf.p), (int)kf2.size(), sf, T, cloud.p);
+    k_map_transform<<<map_blocks(h, total), 256, 0, st>>>(reinterpret_cast<const MapKf*>(h->map_kf.p), (int)kf2.size(), sf, (long long)total, cloud.p);
     TEL_END(&h->tel, KC_MISC, 1, st); }
   if (!(resolution > 0.0)) {  // "To get unfiltered point cloud with intensity" (:39-40)
     if (out_capacity < total) return fail(B2R_EINVAL, "output capacity too small");
@@ -1623,45 +1672,9 @@ extern "C" int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot
     *n_out = total;
     return B2R_OK;
   }
-  // voxel keys -> sort -> unique -> centres
-  B2R_CUDA(h->map_keys[0].reserve(total + 8));
-  B2R_CUDA(h->map_keys[1].reserve(total + 8));
-  B2R_CUDA(h->tmp_i.reserve(2 * total + 16));
-  int* flags = h->tmp_i.p;
-  int* slots = h->tmp_i.p + total + 8;
-  size_t tmp_sort = 0, tmp_scan = 0;
-  B2R_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_sort, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st));
-  B2R_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, flags, slots, (int)total, st));
-  B2R_CUDA(h->bc[0].sort_tmp.reserve(std::max(tmp_sort, tmp_scan) + 256));
-  if (!h->map_geom) {
-    B2R_CUDA(cudaMalloc(&h->map_geom, sizeof(MapGeom) + 64));
-    B2R_CUDA(cudaMallocHost(&h->map_h, 64));
-  }
-  unsigned long long* first_idx = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(h->map_geom) + sizeof(MapGeom));
-  int* n_dev = reinterpret_cast<int*>(first_idx + 1);
-  { TEL_BEGIN(&h->tel, st);
-    // replay of the octree's bounding-box growth: each round finds the first point outside the box and grows the box for it; the
-    // box settles after ~log2(extent / resolution) rounds, further rounds exit at once (G.done)
-    k_oct_init<<<1, 1, 0, st>>>(h->map_geom, resolution, first_idx);
-    for (int round = 0; round < 48; round++) {
-      k_oct_first_violator<<<nb, 256, 0, st>>>(cloud.p, sf, T, h->map_geom, first_idx);
-      k_oct_grow<<<1, 1, 0, st>>>(cloud.p, sf, h->map_geom, first_idx);
-    }
-    k_map_keys<<<nb, 256, 0, st>>>(cloud.p, sf, T, h->map_geom, h->map_keys[0].p);
-    size_t tb = h->bc[0].sort_tmp.cap;
-    B2R_CUDA(cub::DeviceRadixSort::SortKeys(h->bc[0].sort_tmp.p, tb, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st));
-    k_map_heads<<<nb, 256, 0, st>>>(h->map_keys[1].p, T, flags);
-    tb = h->bc[0].sort_tmp.cap;
-    B2R_CUDA(cub::DeviceScan::ExclusiveSum(h->bc[0].sort_tmp.p, tb, flags, slots, (int)total, st));
-    k_map_centers<<<nb, 256, 0, st>>>(h->map_keys[1].p, flags, slots, T, h->map_geom, sf, src.p, n_dev);
-    TEL_END(&h->tel, KC_MISC, 106, st); }
-  B2R_CUDA(cudaGetLastError());
-  B2R_CUDA(cudaMemcpyAsync(h->map_h, n_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
-  B2R_CUDA(cudaMemcpyAsync(h->map_h + 1, &h->map_geom->overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
-  B2R_CUDA(cudaStreamSynchronize(st));
-  // the octree keys hold 21 bits per axis: a deeper box leaves every point uninserted, which must not pass for an empty map
-  if (h->map_h[1]) return fail(B2R_EUNSUPPORTED, "map extent needs more than 21 octree levels at this resolution");
-  const size_t m = (size_t)h->map_h[0];
+  size_t m = 0;
+  int rc = map_voxel_centres(h, cloud.p, sf, total, resolution, src.p, sf, &m);
+  if (rc) return rc;
   if (out_capacity < m) return fail(B2R_EINVAL, "output capacity too small");
   if (m) {
     B2R_CUDA(cudaMemcpyAsync(out, src.p, m * stride_bytes, cudaMemcpyDeviceToHost, st));

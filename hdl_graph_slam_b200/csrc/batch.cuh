@@ -220,21 +220,21 @@ extern "C" int b2r_batch_cloud_count(const b2r_batch* b) {
   return (int)(b->clouds.size() - b->free_ids.size());
 }
 
-// Search structure (bvh_build.cuh) + FastGICP::calculate_covariances for every cloud a batch names that does not have them yet:
-// one cluster-build launch per cluster size and one k-NN launch for all of them (what setInputSource / setInputTarget make the
-// reference pay per call: kd-tree build + covariances, loop_detector.hpp:122,136)
-static int batch_build_structures(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool need_cov) {
+// Search structure (bvh_build.cuh) + FastGICP::calculate_covariances (need_cov) for every cloud of ids[0..n_ids) (known ids, in
+// any order, repeats allowed) that does not have them yet: one cluster-build launch per cluster size and one k-NN launch for all of
+// them (what setInputSource / setInputTarget make the reference pay per call: kd-tree build + covariances, loop_detector.hpp:122,136)
+static int batch_build_structures(b2r_batch* b, const int32_t* ids, size_t n_ids, bool need_cov) {
   b2r_handle* h = b->eng;
   cudaStream_t st = h->st;
   std::vector<Cloud*> todo;
   std::vector<char> queued(b->clouds.size(), 0);
-  for (size_t i = 0; i < n_pairs; i++)
-    for (int32_t id : {pairs[i].source, pairs[i].target}) {
-      Cloud* c = b->clouds[id];
-      if (queued[id] || c->n == 0 || (c->bvh_ready && (c->cov_ready || !need_cov))) continue;
-      queued[id] = 1;
-      todo.push_back(c);
-    }
+  for (size_t i = 0; i < n_ids; i++) {
+    const int32_t id = ids[i];
+    Cloud* c = b->clouds[id];
+    if (queued[id] || c->n == 0 || (c->bvh_ready && (c->cov_ready || !need_cov))) continue;
+    queued[id] = 1;
+    todo.push_back(c);
+  }
   if (todo.empty()) return B2R_OK;
   {  // ---- structures
     std::vector<Cloud*> by_cl[kBuildShapes];  // one launch per (cluster size, pairs per thread) shape
@@ -487,7 +487,9 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   const auto t_a = std::chrono::steady_clock::now();
   int rc = batch_sync_builds(b, false);  // the main stream waits for every outstanding upload / build
   if (rc) return rc;
-  rc = batch_build_structures(b, pairs, n_pairs, !fit_only);
+  std::vector<int32_t> named(2 * n_pairs);
+  for (size_t i = 0; i < n_pairs; i++) { named[2 * i] = pairs[i].source; named[2 * i + 1] = pairs[i].target; }
+  rc = batch_build_structures(b, named.data(), named.size(), !fit_only);
   if (rc) return rc;
   const auto t_b = std::chrono::steady_clock::now();
   const size_t chunk = std::min(b->max_chunk, std::max<size_t>(n_pairs, 1));
@@ -542,6 +544,102 @@ extern "C" int b2r_batch_calc_fitness_score(b2r_batch* b, const b2r_pair* pairs,
   B2R_CUDA(cudaStreamSynchronize(st));
   b->eng->tel.d2h += n_pairs * sizeof(PairReport);
   for (size_t i = 0; i < n_pairs; i++) scores[i] = b->h_reports[i].r.fitness;
+  return B2R_OK;
+}
+
+// MapCloudGenerator::generate (map_cloud_generator.cpp:13-51) over the keyframe clouds the batch already holds: keyframe k = cloud
+// ids[k] at poses[16k..16k+16).  resolution > 0 reads every cloud's search structure (built here if missing, as the next align
+// would), so no record is uploaded and device-added clouds work after their buffers are gone; resolution <= 0 needs the full records
+// and therefore the cache's own upload of each cloud.  The result is b2r_map_cloud_generate's on the same clouds and poses.
+extern "C" int b2r_batch_map_cloud_generate(b2r_batch* b, const int32_t* ids, const float* poses, size_t n_keyframes, double resolution,
+                                            size_t out_stride_bytes, void* out_host, size_t out_capacity, const void** d_out, size_t* n_out) {
+  if (!b || !n_out) return fail(B2R_EINVAL, "NULL argument");
+  *n_out = 0;
+  if (d_out) *d_out = nullptr;
+  if (n_keyframes == 0) return 1;  // "warning: keyframes empty!!" -> nullptr (map_cloud_generator.cpp:14-17)
+  if (!ids || !poses) return fail(B2R_EINVAL, "NULL argument");
+  if (out_stride_bytes < 12 || (out_stride_bytes & 3)) return fail(B2R_EINVAL, "bad stride");
+  const bool voxels = resolution > 0.0;
+  size_t total = 0;
+  for (size_t k = 0; k < n_keyframes; k++) {
+    const int32_t id = ids[k];
+    if (id < 0 || (size_t)id >= b->clouds.size() || !b->clouds[id]) return fail(B2R_EINVAL, "unknown cloud id " + std::to_string(id));
+    const Cloud& c = *b->clouds[id];
+    if (!voxels && (c.raw_view != c.raw.p || !c.raw.p))  // a device-added cloud's records are the caller's, valid only until its build
+      return fail(B2R_EINVAL, "cloud id " + std::to_string(id) + " was added from device memory: resolution <= 0 needs records the batch holds");
+    if (!voxels && (size_t)c.stride_f * 4 != out_stride_bytes)
+      return fail(B2R_EINVAL, "cloud id " + std::to_string(id) + " has " + std::to_string(c.stride_f * 4) + "-byte records, not out_stride_bytes");
+    total += c.n;
+  }
+  if (total >= (size_t)0x7fffffff) return fail(B2R_EINVAL, "map cloud too large (>= 2^31 points)");
+  if (total == 0) return B2R_OK;
+  if (out_host && !voxels && out_capacity < total) return fail(B2R_EINVAL, "output capacity too small");
+  b2r_handle* h = b->eng;
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  cudaStream_t st = h->st;
+  int rc = batch_sync_builds(b, false);  // the uploads of the named clouds
+  if (rc) return rc;
+  const int sf = (int)(out_stride_bytes / 4);
+  DevBuf<float>& out = h->pf_buf[0];
+  DevBuf<float>& cloud = h->pf_buf[1];
+  B2R_CUDA(out.reserve(total * sf + 8));
+  size_t m = 0;
+  if (!voxels) {  // "To get unfiltered point cloud with intensity" (:39-40): the transformed records, straight into the output
+    std::vector<MapKf> kf;
+    size_t first = 0;
+    for (size_t k = 0; k < n_keyframes; k++) {
+      const Cloud& c = *b->clouds[ids[k]];
+      if (c.n) {  // empty keyframes must not shadow their successors in the binary search
+        MapKf d;
+        d.pts = c.raw.p; d.first = (long long)first; d.n = (int)c.n; d.pad = 0;
+        for (int r = 0; r < 3; r++) for (int col = 0; col < 4; col++) d.T[r * 4 + col] = poses[16 * k + col * 4 + r];
+        kf.push_back(d);
+      }
+      first += c.n;
+    }
+    B2R_CUDA(h->map_kf.reserve(kf.size() * sizeof(MapKf) + 64));
+    B2R_CUDA(cudaMemcpyAsync(h->map_kf.p, kf.data(), kf.size() * sizeof(MapKf), cudaMemcpyHostToDevice, st));
+    { TEL_BEGIN(&h->tel, st);
+      k_map_transform<<<map_blocks(h, total), 256, 0, st>>>(reinterpret_cast<const MapKf*>(h->map_kf.p), (int)kf.size(), sf, (long long)total, out.p);
+      TEL_END(&h->tel, KC_MISC, 1, st); }
+    B2R_CUDA(cudaGetLastError());
+    B2R_CUDA(cudaStreamSynchronize(st));  // kf is pageable host memory of this call
+    m = total;
+  } else {
+    rc = batch_build_structures(b, ids, n_keyframes, false);
+    if (rc) return rc;
+    std::vector<MapCachedKf> kf;
+    size_t first = 0;
+    for (size_t k = 0; k < n_keyframes; k++) {
+      const Cloud& c = *b->clouds[ids[k]];
+      if (c.n) {
+        MapCachedKf d;
+        d.sorted = c.sorted.p; d.pos_of = c.pos_of.p; d.first = (long long)first;
+        for (int r = 0; r < 3; r++) for (int col = 0; col < 4; col++) d.T[r * 4 + col] = poses[16 * k + col * 4 + r];
+        kf.push_back(d);
+      }
+      first += c.n;
+    }
+    B2R_CUDA(cloud.reserve(total * 4 + 8));
+    B2R_CUDA(h->map_kf.reserve(kf.size() * sizeof(MapCachedKf) + 64));
+    B2R_CUDA(cudaMemcpyAsync(h->map_kf.p, kf.data(), kf.size() * sizeof(MapCachedKf), cudaMemcpyHostToDevice, st));
+    B2R_CUDA(cudaStreamSynchronize(st));  // kf is pageable host memory of this call
+    { TEL_BEGIN(&h->tel, st);
+      k_map_gather<<<map_blocks(h, total), 256, 0, st>>>(reinterpret_cast<const MapCachedKf*>(h->map_kf.p), (int)kf.size(), (long long)total,
+                                                         reinterpret_cast<float4*>(cloud.p));
+      TEL_END(&h->tel, KC_MISC, 1, st); }
+    B2R_CUDA(cudaGetLastError());
+    rc = map_voxel_centres(h, cloud.p, 4, total, resolution, out.p, sf, &m);
+    if (rc) return rc;
+    if (out_host && out_capacity < m) return fail(B2R_EINVAL, "output capacity too small");
+  }
+  if (out_host && m) {
+    B2R_CUDA(cudaMemcpyAsync(out_host, out.p, m * out_stride_bytes, cudaMemcpyDeviceToHost, st));
+    B2R_CUDA(cudaStreamSynchronize(st));
+    h->tel.d2h += m * out_stride_bytes;
+  }
+  if (d_out) *d_out = out.p;
+  *n_out = m;
   return B2R_OK;
 }
 

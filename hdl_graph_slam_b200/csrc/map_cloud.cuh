@@ -10,6 +10,8 @@
 // sort of the keys (cub::DeviceRadixSort — 10^7..10^8 keys, far beyond the cluster sort's reach), unique, centres
 // (key + 0.5) resolution + min.  The result is the same SET of centres as PCL's; PCL emits them in octree traversal order, here
 // they come out in ascending (z, y, x) key order — the consumers (rviz, save_map) do not depend on the order.
+// b2r_batch_map_cloud_generate builds the same concatenated cloud from a batch's cached keyframes (k_map_gather) instead of
+// uploading them; everything after the transform is shared.
 #pragma once
 #include <cub/device/device_radix_sort.cuh>
 #include "engine.cuh"
@@ -48,6 +50,37 @@ __global__ void k_map_transform(const MapKf* __restrict__ kfs, int n_kf, int str
     o[1] = xform_row(K.T[4], K.T[5], K.T[6], K.T[7], x, y, z);
     o[2] = xform_row(K.T[8], K.T[9], K.T[10], K.T[11], x, y, z);
     if (stride_f >= 4) o[3] = 1.0f;
+  }
+}
+
+// one keyframe of a b2r_batch's cache, read through its search structure (bvh_build.cuh): the raw records of a device-added
+// cloud belong to the caller and are gone once the structure is built, the BVH-sorted copy is the engine's own
+struct MapCachedKf {
+  const float4* sorted;   // (x, y, z, bits(original index)), ascending (Hilbert key, original index)
+  const int* pos_of;      // original index -> sorted position; -1 = a non-finite point, dropped from the structure
+  long long first;        // index of its first point in the concatenated cloud
+  float T[12];            // rows 0..2 of pose.cast<float>()
+};
+
+// dst[first + i] = pose * src[i] for point i of every keyframe, in the original point order (the box replay below depends on it),
+// packed as float4 (only x, y, z are read downstream).  A point the structure dropped comes out as NaN: pose * (a non-finite
+// point) is non-finite on every axis, so the octree skips either one alike.
+__global__ void k_map_gather(const MapCachedKf* __restrict__ kfs, int n_kf, long long total, float4* __restrict__ out) {
+  const float qnan = __int_as_float(0x7fc00000);
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (long long)gridDim.x * blockDim.x) {
+    int lo = 0, hi = n_kf - 1;  // keyframe of point g: last one with first <= g
+    while (lo < hi) { const int mid = (lo + hi + 1) >> 1; if (kfs[mid].first <= g) lo = mid; else hi = mid - 1; }
+    const MapCachedKf& K = kfs[lo];
+    const int s = K.pos_of[g - K.first];
+    float4 o = make_float4(qnan, qnan, qnan, qnan);
+    if (s >= 0) {
+      const float4 p = K.sorted[s];
+      o.x = xform_row(K.T[0], K.T[1], K.T[2], K.T[3], p.x, p.y, p.z);
+      o.y = xform_row(K.T[4], K.T[5], K.T[6], K.T[7], p.x, p.y, p.z);
+      o.z = xform_row(K.T[8], K.T[9], K.T[10], K.T[11], p.x, p.y, p.z);
+      o.w = 1.0f;
+    }
+    out[g] = o;
   }
 }
 

@@ -568,6 +568,7 @@ class RegistrationBatch:
         self.engine = Registration(_handle=eng)
         self.engine.close = lambda: None  # owned by the batch
         self._keep = {}
+        self._sizes = {}  # cloud id -> point count: the capacity of a host map cloud
 
     def close(self):
         if self._b:
@@ -586,17 +587,20 @@ class RegistrationBatch:
         cid = C.c_int32(-1)
         check(self._lib.b2r_batch_add_cloud(self._b, a.ctypes.data_as(C.c_void_p), n, s, C.byref(cid)))
         self._keep[cid.value] = a
+        self._sizes[cid.value] = n
         return cid.value
 
     def addCloudRaw(self, ptr, n, stride_bytes, device=False):
         cid = C.c_int32(-1)
         fn = self._lib.b2r_batch_add_cloud_device if device else self._lib.b2r_batch_add_cloud
         check(fn(self._b, C.c_void_p(ptr), n, stride_bytes, C.byref(cid)))
+        self._sizes[cid.value] = n
         return cid.value
 
     def removeCloud(self, cid):
         check(self._lib.b2r_batch_remove_cloud(self._b, cid))
         self._keep.pop(cid, None)
+        self._sizes.pop(cid, None)
 
     def cloudCount(self):
         return self._lib.b2r_batch_cloud_count(self._b)
@@ -630,6 +634,27 @@ class RegistrationBatch:
         out = np.empty(max(len(edges), 1), np.float64)
         check(self._lib.b2r_batch_calc_fitness_score(self._b, arr, len(edges), max_range, out.ctypes.data_as(C.POINTER(C.c_double))))
         return out[: len(edges)]
+
+    def mapCloudGenerate(self, ids, poses, resolution, stride_bytes=32, device=False):
+        """MapCloudGenerator::generate over cached clouds: keyframe k = cloud ids[k] at the 4x4 pose poses[k] -> map cloud of
+        stride_bytes records (b2r_batch_map_cloud_generate); device=True returns (engine-owned device pointer, record count)
+        instead.  None if ids is empty."""
+        ids = [int(i) for i in ids]
+        if len(poses) != len(ids):
+            raise ValueError("one pose per id")
+        idarr = (C.c_int32 * max(len(ids), 1))(*ids)
+        P = np.ascontiguousarray(np.concatenate([_colmajor(p) for p in poses]) if ids else np.zeros(16, np.float32))
+        Pp = P.ctypes.data_as(C.POINTER(C.c_float))
+        m = C.c_size_t()
+        if device:
+            dptr = C.c_void_p()
+            rc = check(self._lib.b2r_batch_map_cloud_generate(self._b, idarr, Pp, len(ids), float(resolution), stride_bytes, None, 0, C.byref(dptr), C.byref(m)))
+            return None if rc == 1 else (dptr.value, m.value)
+        cap = sum(self._sizes.get(i, 0) for i in ids)
+        out = np.zeros((max(cap, 1), stride_bytes // 4), np.float32)
+        rc = check(self._lib.b2r_batch_map_cloud_generate(self._b, idarr, Pp, len(ids), float(resolution), stride_bytes, out.ctypes.data_as(C.c_void_p),
+                                                          cap, None, C.byref(m)))
+        return None if rc == 1 else out[: m.value]
 
     def lastRounds(self):
         a, b = C.c_uint64(), C.c_uint64()

@@ -361,6 +361,17 @@ int b2r_batch_align(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, int wan
  * pairs[i].target = cloud1 (the tree), pairs[i].source = cloud2 (transformed), pairs[i].guess = relpose.cast<float>() column-major.
  * scores[i] = mean squared NN distance over the neighbours with d2 <= max_range, DBL_MAX when there is none. */
 int b2r_batch_calc_fitness_score(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, double max_range, double* scores);
+/* MapCloudGenerator::generate over clouds of the b2r_batch keyframe cache: keyframe k = cloud ids[k] at poses[16k..16k+16)
+ * (KeyFrameSnapshot::pose cast to float, column-major).  Same result as b2r_map_cloud_generate on the same clouds and poses,
+ * with no point uploaded.  out_host (capacity out_capacity records of out_stride_bytes, may be NULL) and/or *d_out (engine-owned,
+ * valid until the next map or prefilter call on the batch's engine handle, may be NULL; NULL when *n_out = 0).
+ * Ids may come in any order and repeat; an unknown or removed id is B2R_EINVAL.  Returns 1 with *n_out = 0 when n_keyframes = 0.
+ * resolution > 0 reads the clouds' search structures and builds the missing ones (the build the next b2r_batch_align would do; a
+ * device-added cloud must be valid until then, as for an align).  resolution <= 0 copies the records the batch uploaded itself:
+ * every cloud must come from b2r_batch_add_cloud with stride_bytes == out_stride_bytes, else B2R_EINVAL naming the id.
+ * B2R_EUNSUPPORTED beyond 21 octree levels, as b2r_map_cloud_generate; the batch stays usable. */
+int b2r_batch_map_cloud_generate(b2r_batch* b, const int32_t* ids, const float* poses, size_t n_keyframes, double resolution,
+                                 size_t out_stride_bytes, void* out_host, size_t out_capacity, const void** d_out, size_t* n_out);
 /* the rest of InformationMatrixCalculator::calc_information_matrix (information_matrix_calculator.cpp:25-47, weight() at
  * information_matrix_calculator.hpp:39-42): fitness score -> diagonal of the 6x6 information matrix (x,y,z, then rotation).
  * Defaults of the reference's rosparams: b2r_information_params_default. */
