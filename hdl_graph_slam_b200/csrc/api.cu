@@ -1274,7 +1274,9 @@ static int pf_knn_stat(b2r_handle* h, const float* d_in, size_t n, int sf, int k
   c.raw_view = d_in;
   int rc = ensure_grid(h, c);
   if (rc) return rc;
-  k_fill_i32<<<(unsigned)((n + 255) / 256), 256, 0, h->st>>>(reinterpret_cast<int*>(h->tmp_f.p), (int)n, 0x7fc00000);  // NaN = non-finite point
+  // the value a non-finite point keeps: NaN for the k-th distance, kStatNonFinite for the mean distance (whose NaN is a real value)
+  const int fill = mode == 0 ? 0x7fc00000 : (int)kStatNonFiniteBits;
+  k_fill_i32<<<(unsigned)((n + 255) / 256), 256, 0, h->st>>>(reinterpret_cast<int*>(h->tmp_f.p), (int)n, fill);
   const size_t smem = (size_t)k * kKnnThreads * sizeof(unsigned long long);
   if (smem > 48 * 1024 && !h->stat_smem_attr) {
     B2R_CUDA(cudaFuncSetAttribute(k_knn_stat, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * kKnnThreads * 8));
@@ -1300,7 +1302,7 @@ static int pf_radius(b2r_handle* h, const float* d_in, size_t n, int sf, double 
 static int pf_statistical(b2r_handle* h, const float* d_in, size_t n, int sf, int mean_k, double stddev_mul, float* d_out, size_t* m) {
   int rc = pf_knn_stat(h, d_in, n, sf, mean_k + 1, 1);
   if (rc) return rc;
-  k_sor_stats<<<1, 1024, 0, h->st>>>(h->tmp_f.p, (int)n, stddev_mul, h->pf_stats);
+  k_sor_stats<<<1, kSorThreads, 0, h->st>>>(h->tmp_f.p, (int)n, stddev_mul, h->pf_stats);
   k_sor_flags<<<(unsigned)((n + 255) / 256), 256, 0, h->st>>>(h->tmp_f.p, (int)n, h->pf_stats, h->pf_flags.p);
   return pf_compact(h, d_in, n, sf, d_out, m);
 }

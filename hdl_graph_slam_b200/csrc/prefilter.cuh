@@ -6,7 +6,7 @@
 //   STATISTICAL keep p  iff  mean distance to its mean_k nearest neighbours (itself excluded) <= mean + mul * stddev over the cloud
 //   k_deskew           <- PrefilteringNodelet::deskewing                 /root/reference/apps/prefiltering_nodelet.cpp:182-243
 // Decisions and compaction stay on the device: the per-point statistic, the cloud-wide mean / stddev of the statistical filter
-// (fixed-order float64 reduction), the keep flags, and an order-preserving stream compaction (count / scan / scatter) — so the
+// (PCL's index-order float64 sums), the keep flags, and an order-preserving stream compaction (count / scan / scatter) — so the
 // chain deskew -> distance filter -> voxel grid -> outlier removal hands a device-resident cloud to the registration.
 #pragma once
 #include "common.cuh"
@@ -30,6 +30,11 @@ __global__ void k_distance_flags(const float* __restrict__ raw, int stride_f, in
 
 // mode 0: out[orig idx] = squared distance of the k-th nearest neighbour (self included), +inf if fewer than k points
 // mode 1: out[orig idx] = (float)( sum_{j=1..k-1} sqrtf(d2_j) / (k-1) )   (PCL StatisticalOutlierRemoval, k = mean_k + 1)
+//         mean_k = 0 gives 0/0 = NaN, as in PCL: a NaN mean distance is a valid point's statistic, so a non-finite point (not in
+//         the BVH, never written here) is marked by the caller's fill with a negative value no mean distance can take.
+// Non-finite points keep the caller's fill: NaN in mode 0, kStatNonFinite in mode 1.
+constexpr float kStatNonFinite = -1.0f;
+constexpr unsigned kStatNonFiniteBits = 0xbf800000u;  // __float_as_uint(kStatNonFinite), usable by the host's fill
 __global__ void __launch_bounds__(kKnnThreads, 4) k_knn_stat(Bvh b, int k, int mode, float* __restrict__ out) {
   extern __shared__ unsigned long long knn_keys[];
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -106,26 +111,45 @@ __global__ void k_radius_flags(const float* __restrict__ kth_d2, int n, double r
 
 // STATISTICAL (pcl::StatisticalOutlierRemoval::applyFilterIndices): sum and sum of squares of the per-point mean distances over
 // the VALID points (a non-finite point has distance 0 and is kept); squares are formed in float32 as PCL's `distance * distance`.
-// One block, fixed order: thread t adds elements t, t + 1024, ... sequentially, then a fixed tree => reproducible.
+// The two float64 sums are PCL's: one running sum each, in index order.  A float64 sum of values spanning many binades depends on
+// its order, and a mean distance that lands between two orders' thresholds is kept by one and removed by the other.
+// Fast path: every term is a non-negative multiple of 2^e (e = the smallest ulp exponent among the nonzero float32 terms), so
+// while a sum stays below 2^(e+53) every partial sum, in any order, is exact.  The block first sums in parallel (thread t adds
+// t, t + 1024, ..., then two butterflies); if a computed sum is below that bound, no partial sum can have rounded (the first
+// rounded one would be >= the bound, and adding non-negative terms never brings a rounded sum back below it), so it IS the
+// sequential sum.  NaN / inf sums are the same in every order too.  Otherwise the block stages tiles of the distances in shared
+// memory and thread 0 adds them up in index order (~16.5 ns per point on an H100: the _wide clouds of tools/sor_time.py).
+constexpr int kSorThreads = 1024, kSorTile = 8192;
 struct SorStats { double sum, sq_sum, thresh; unsigned long long valid; };
-__global__ void __launch_bounds__(1024) k_sor_stats(const float* __restrict__ dist, int n, double stddev_mul, SorStats* out) {
+__device__ __forceinline__ int sor_ulp_exp(float v) { return max((__float_as_int(v) >> 23) & 0xff, 1) - 150; }  // v >= 0
+__device__ __forceinline__ bool sor_order_free(double s, int e) { return !(s <= DBL_MAX) || e == INT_MAX || s < ldexp(1.0, e + 53); }
+__global__ void __launch_bounds__(kSorThreads) k_sor_stats(const float* __restrict__ dist, int n, double stddev_mul, SorStats* out) {
+  __shared__ float tile[kSorTile];
   __shared__ double s_sum[32], s_sq[32];
   __shared__ unsigned long long s_cnt[32];
+  __shared__ int s_e[32], s_esq[32];
+  __shared__ int sequential;
   double sum = 0.0, sq = 0.0;
   unsigned long long cnt = 0;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) {
+  int e = INT_MAX, esq = INT_MAX;
+  for (int i = threadIdx.x; i < n; i += kSorThreads) {
     const float d = dist[i];
-    if (d != d) continue;  // NaN marks a non-finite point: distance 0, not counted as valid
+    if (d < 0.f) continue;  // kStatNonFinite
+    const float dd = fmul(d, d);
     sum += (double)d;
-    sq += (double)fmul(d, d);
+    sq += (double)dd;
     cnt++;
+    if (d > 0.f) e = min(e, sor_ulp_exp(d));
+    if (dd > 0.f) esq = min(esq, sor_ulp_exp(dd));
   }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) {
     sum += __shfl_xor_sync(0xffffffffu, sum, o); sq += __shfl_xor_sync(0xffffffffu, sq, o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
   }
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (lane == 0) { s_sum[warp] = sum; s_sq[warp] = sq; s_cnt[warp] = cnt; }
+  e = __reduce_min_sync(0xffffffffu, e);
+  esq = __reduce_min_sync(0xffffffffu, esq);
+  if (lane == 0) { s_sum[warp] = sum; s_sq[warp] = sq; s_cnt[warp] = cnt; s_e[warp] = e; s_esq[warp] = esq; }
   __syncthreads();
   if (warp == 0) {
     sum = s_sum[lane]; sq = s_sq[lane]; cnt = s_cnt[lane];
@@ -133,21 +157,46 @@ __global__ void __launch_bounds__(1024) k_sor_stats(const float* __restrict__ di
     for (int o = 16; o > 0; o >>= 1) {
       sum += __shfl_xor_sync(0xffffffffu, sum, o); sq += __shfl_xor_sync(0xffffffffu, sq, o); cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
     }
-    if (lane == 0) {
-      const double nv = (double)cnt;
-      const double mean = sum / nv;
-      const double variance = (sq - sum * sum / nv) / (nv - 1.0);
-      out->sum = sum; out->sq_sum = sq; out->valid = cnt;
-      out->thresh = mean + stddev_mul * sqrt(variance);
+    e = __reduce_min_sync(0xffffffffu, s_e[lane]);
+    esq = __reduce_min_sync(0xffffffffu, s_esq[lane]);
+    if (lane == 0) sequential = !(sor_order_free(sum, e) && sor_order_free(sq, esq));
+  }
+  __syncthreads();
+  if (sequential) {
+    sum = 0.0; sq = 0.0; cnt = 0;
+    for (int base = 0; base < n; base += kSorTile) {
+      const int m = min(kSorTile, n - base);
+      for (int j = threadIdx.x; j < m; j += kSorThreads) tile[j] = dist[base + j];
+      __syncthreads();
+      if (threadIdx.x == 0) {
+#pragma unroll 8
+        for (int j = 0; j < m; j++) {
+          const float d = tile[j];
+          // a non-finite point (d == kStatNonFinite) is skipped: adding +0.0 leaves a sum of non-negative terms unchanged
+          const bool valid = !(d < 0.f);
+          sum += valid ? (double)d : 0.0;
+          sq += valid ? (double)fmul(d, d) : 0.0;
+          cnt += valid ? 1u : 0u;
+        }
+      }
+      __syncthreads();
     }
+  }
+  if (threadIdx.x == 0) {  // thread 0 holds the block's sums on either path
+    const double nv = (double)cnt;
+    const double mean = sum / nv;
+    const double variance = (sq - sum * sum / nv) / (nv - 1.0);
+    out->sum = sum; out->sq_sum = sq; out->valid = cnt;
+    out->thresh = __dadd_rn(mean, __dmul_rn(stddev_mul, sqrt(variance)));  // two roundings, as PCL: no fused multiply-add
   }
 }
 __global__ void k_sor_flags(const float* __restrict__ dist, int n, const SorStats* __restrict__ st, unsigned char* flags) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float d = dist[i];
-  // non-finite point: distance 0.0 <= threshold -> kept, as PCL does; no valid point at all: everything is removed (threshold is NaN)
-  const double dd = (d != d) ? 0.0 : (double)d;
+  // non-finite point: distance 0.0 <= threshold -> kept, as PCL does; mean_k = 0 (every mean distance NaN, so the threshold is NaN):
+  // !(d > NaN) keeps every point, as PCL does; no valid point at all: everything is removed
+  const double dd = (d < 0.f) ? 0.0 : (double)d;
   flags[i] = (st->valid > 0 && !(dd > st->thresh)) ? 1 : 0;
 }
 
