@@ -2040,25 +2040,9 @@ extern "C" int b2r_loop_matching(b2r_handle* h, const void* new_keyframe, size_t
   *best = -1;
   if (n_candidates == 0) return B2R_OK;  // loop_detector.hpp:118-120
   if (!candidates || !n_candidates_pts || !guesses) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_GICP) {  // NDT handle: the reference's sequential loop, one align + getFitnessScore per candidate
-    int rc = b2r_set_target(h, new_keyframe, n_new, stride_bytes);  // :122
-    if (rc) return rc;
-    std::vector<b2r_result> rs(n_candidates);
-    for (size_t i = 0; i < n_candidates; i++) {  // :135-154
-      rc = b2r_set_source(h, candidates[i], n_candidates_pts[i], stride_bytes);
-      if (rc) return rc;
-      rc = b2r_align(h, guesses + i * 16, &rs[i]);
-      if (rc) return rc;
-      double score;
-      rc = b2r_fitness(h, nullptr, fitness_score_max_range, 0.25f, &score, nullptr, nullptr);
-      if (rc) return rc;
-      rs[i].fitness = score;
-      if (results) results[i] = rs[i];
-    }
-    return b2r_loop_argmin(rs.data(), n_candidates, fitness_score_thresh, best);
-  }
-  // GICP: the candidate loop is ONE batched registration — all candidates of the new keyframe share the target (:122) and only
-  // couple through the argmin (:147), so every LM iteration of every candidate is one pair of launches (pair_engine.cuh)
+  // the candidate loop is ONE batched registration — all candidates of the new keyframe share the target (:122) and only couple
+  // through the argmin (:147): on a GICP handle every LM iteration of every candidate is one pair of launches (pair_engine.cuh), on
+  // an NDT handle every derivative pass of every candidate is one batched pass (batch_run_ndt_chunk)
   if (!h->loop_batch) {
     int rc = b2r_batch_create(&h->cfg, &h->loop_batch);
     if (rc) return rc;

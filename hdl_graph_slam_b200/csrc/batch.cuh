@@ -7,6 +7,9 @@
 //   b2r_batch_align      <- the candidate loop of LoopDetector::matching (loop_detector.hpp:135-154): align + getFitnessScore
 //   b2r_batch_loop_detect<- LoopDetector::matching for MANY new keyframes, groups sharded over the ranks of an NCCL communicator,
 //                           ONE ncclAllGather of 80-byte b2r_result records, per-group argmin with the reference's tie rule (:147,160)
+// A GICP batch runs the device-resident LM engine (pair_engine.cuh).  An NDT batch (the factory's default NDT_OMP, which the
+// loop detector builds its registration with) runs every pair's host Newton / More-Thuente driver (NdtPairState, ndt.cuh) in
+// rounds: one batched derivative pass per pass kind covers every pair in flight, the host waits once per round.
 #pragma once
 #include <nccl.h>
 #include <chrono>
@@ -60,6 +63,16 @@ struct b2r_batch {
   size_t h_knn_cap = 0;
   b2r_result* h_gather = nullptr;
   size_t h_gather_cap = 0;
+  // NDT batch (batch_run_ndt_chunk)
+  DevBuf<char> ndt_ws;              // per pair in flight: chunk rows, group rows, counters, ticket counter; fitness partials
+  DevBuf<NdtArgs> d_ndt_args;       // the round's pass records, grouped by pass kind
+  NdtArgs* h_ndt_args = nullptr;    // pinned staging
+  size_t h_ndt_cap = 0;
+  double* h_ndt_msg = nullptr;      // host-mapped: one result message per record of the round, then the round's flag
+  double* h_ndt_msg_dev = nullptr;
+  size_t ndt_msg_cap = 0;
+  unsigned int* d_ndt_round = nullptr;  // messages of the current round (the last one publishes the flag and re-arms it)
+  unsigned long long ndt_seq = 0;
   // telemetry of the last b2r_batch_align
   unsigned long long last_rounds = 0, last_pair_rounds = 0;
 };
@@ -104,6 +117,10 @@ extern "C" void b2r_batch_destroy(b2r_batch* b) {
   if (b->h_knn) cudaFreeHost(b->h_knn);
   if (b->h_build) cudaFreeHost(b->h_build);
   b->d_knn.release(); b->d_build.release();
+  b->ndt_ws.release(); b->d_ndt_args.release();
+  if (b->h_ndt_args) cudaFreeHost(b->h_ndt_args);
+  if (b->h_ndt_msg) cudaFreeHost(b->h_ndt_msg);
+  if (b->d_ndt_round) cudaFree(b->d_ndt_round);
   if (b->eng) b2r_destroy(b->eng);
   delete b;
 }
@@ -111,7 +128,7 @@ extern "C" void b2r_batch_destroy(b2r_batch* b) {
 extern "C" int b2r_batch_create(const b2r_config* cfg, b2r_batch** out) {
   if (!cfg || !out) return fail(B2R_EINVAL, "NULL argument");
   *out = nullptr;
-  if (cfg->method != B2R_METHOD_GICP) return fail(B2R_EUNSUPPORTED, "the batched path re-creates the GICP engine only (the reference's loop closure runs FAST_GICP: hdl_graph_slam.launch:127)");
+  if (cfg->method != B2R_METHOD_GICP && cfg->method != B2R_METHOD_NDT) return fail(B2R_EINVAL, "unknown method");
   b2r_batch* b = new b2r_batch();
   int rc = b2r_create(cfg, &b->eng);
   if (rc) { delete b; return rc; }
@@ -125,6 +142,8 @@ extern "C" int b2r_batch_create(const b2r_config* cfg, b2r_batch** out) {
     return bail(fail(B2R_ECUDA, "host allocation failed"));
   for (int i = 0; i < 8; i++) b->h_word[i] = 0;
   if (cudaEventCreateWithFlags(&b->fork_ev, cudaEventDisableTiming) != cudaSuccess) return bail(fail(B2R_ECUDA, "event creation failed"));
+  if (cudaMalloc(&b->d_ndt_round, sizeof(unsigned int)) != cudaSuccess || cudaMemset(b->d_ndt_round, 0, sizeof(unsigned int)) != cudaSuccess)
+    return bail(fail(B2R_ECUDA, "device allocation failed"));
   for (int l = 0; l < b2r_batch::kLanes; l++) {
     b2r_batch::Lane& L = b->lane[l];
     L.h_word = b->h_word + l; L.h_word_dev = b->h_word_dev + l;
@@ -464,6 +483,197 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
   return B2R_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ NDT batch
+// Voxel maps of the clouds a call names: every align target, and every cloud added from device memory (its records are the
+// caller's only until this call returns, so the map is built now even if the cloud is a target only later).
+static int batch_ndt_maps(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool fit_only) {
+  b2r_handle* h = b->eng;
+  for (size_t i = 0; i < n_pairs; i++) {
+    for (int side = 0; side < 2; side++) {
+      Cloud& c = *b->clouds[side ? pairs[i].target : pairs[i].source];
+      const bool device_added = c.raw_view != c.raw.p;
+      if (c.n == 0 || c.ndt_ready || !(device_added || (side == 1 && !fit_only))) continue;
+      int rc = ndt_ensure_map(h->cfg, c, h->ndt_work, h->st);
+      if (rc) return rc;
+    }
+  }
+  return B2R_OK;
+}
+
+constexpr int kNdtMsg = 48;  // doubles per result message: kNdtAcc sums (or 36 Hessian entries), pair count, checksum
+
+// per pair in flight: [chunks + 1][kNdtAcc] chunk rows (also the Hessian pass's [blocks][36]), [groups][kNdtAcc] group rows,
+// group counters, then counter / pair count / ticket counter — all zero at the start of a chunk of pairs
+struct NdtPairWs { size_t partials, grows, gcount, small, bytes; };
+static NdtPairWs ndt_pair_ws(const Cloud& s) {
+  const size_t nb = (size_t)s.nsup * 1024 / kNdtThreads, ng = (nb + 31) / 32;
+  NdtPairWs w;
+  w.partials = 0;
+  w.grows = align_up((nb + 1) * kNdtAcc * sizeof(double), 256);
+  w.gcount = w.grows + align_up(ng * kNdtAcc * sizeof(double), 256);
+  w.small = w.gcount + align_up(ng * sizeof(unsigned int), 256);
+  w.bytes = w.small + 256;  // [0,16) counter, [16,24) pair count, [24,32) ticket counter
+  return w;
+}
+
+// pairs[0..m) of an NDT batch -> rep[0..m) (host).  Every pair runs ndt_align's driver (NdtPairState); a round gathers the pass
+// each active pair asks for into at most three launches (derivatives with Hessian, without, float64 Hessian only), waits once for
+// the round's flag and hands every pair its result.  A pair reduces through its own rows and counters, exactly as alone.
+static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, double fit_max_range, PairReport* rep) {
+  b2r_handle* h = b->eng;
+  cudaStream_t st = h->st;
+  const b2r_config& cfg = h->cfg;
+  std::vector<NdtPairState> S(m);
+  std::vector<size_t> active, off(m, 0), fit_off(m, 0);
+  size_t ws = 0;
+  for (size_t i = 0; i < m; i++) {
+    Cloud& s = *b->clouds[pairs[i].source];
+    Cloud& t = *b->clouds[pairs[i].target];
+    if (s.n == 0 || t.n == 0) continue;  // ndt_align: initCompute fails silently (identity, not converged, no iteration)
+    fit_off[i] = ws;
+    ws += align_up((size_t)s.nsup * 1024 / kLinThreads * 3 * sizeof(double), 256) + 256;  // k_fitness partials, then its counter
+    int rc = ndt_sync_geom(*t.ndt, h->ndt_work, st);
+    if (rc) return rc;
+    if (t.ndt->h_geom.empty) continue;  // no finite target point: as above
+    S[i].start(cfg, pairs[i].guess);
+    active.push_back(i);
+    off[i] = ws;
+    ws += ndt_pair_ws(s).bytes;
+  }
+  const size_t fit_out = ws;  // 3 doubles per pair: the fitness sums
+  ws += align_up(m * 3 * sizeof(double), 256);
+  B2R_CUDA(b->ndt_ws.reserve(ws + 256));
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->ndt_ws.p), 256));
+  B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
+  B2R_CUDA(b->d_ndt_args.reserve(m));
+  if (b->h_ndt_cap < m) {
+    if (b->h_ndt_args) cudaFreeHost(b->h_ndt_args);
+    b->h_ndt_args = nullptr; b->h_ndt_cap = 0;
+    B2R_CUDA(cudaMallocHost(&b->h_ndt_args, m * sizeof(NdtArgs)));
+    b->h_ndt_cap = m;
+  }
+  if (b->ndt_msg_cap < m) {
+    if (b->h_ndt_msg) cudaFreeHost(b->h_ndt_msg);
+    b->h_ndt_msg = nullptr; b->ndt_msg_cap = 0;
+    B2R_CUDA(cudaHostAlloc(&b->h_ndt_msg, (m * kNdtMsg + 8) * sizeof(double), cudaHostAllocMapped));
+    B2R_CUDA(cudaHostGetDevicePointer((void**)&b->h_ndt_msg_dev, b->h_ndt_msg, 0));
+    std::memset(b->h_ndt_msg, 0, (m * kNdtMsg + 8) * sizeof(double));
+    b->ndt_msg_cap = m;
+  }
+  unsigned long long* flag = reinterpret_cast<unsigned long long*>(b->h_ndt_msg + b->ndt_msg_cap * kNdtMsg);
+  unsigned long long* flag_dev = reinterpret_cast<unsigned long long*>(b->h_ndt_msg_dev + b->ndt_msg_cap * kNdtMsg);
+  std::vector<unsigned long long> qnext(m, 0);
+  std::vector<size_t> order;
+  std::vector<int> kind_of;
+  while (!active.empty()) {
+    order.clear(); kind_of.clear();
+    size_t cnt[3] = {0, 0, 0};
+    unsigned max_nb[3] = {0, 0, 0};
+    for (int k = 0; k < 3; k++)
+      for (size_t i : active)
+        if (S[i].next() == k) {
+          order.push_back(i); kind_of.push_back(k); cnt[k]++;
+          max_nb[k] = std::max(max_nb[k], (unsigned)((size_t)b->clouds[pairs[i].source]->nsup * 1024 / kNdtThreads));
+        }
+    // blocks per pair of a derivative launch: about four waves of the device, and no more than the largest pair has chunks; a
+    // pair's blocks draw its chunks from its own ticket counter, so any count gives the same sums
+    unsigned G[3] = {0, 0, 0};
+    for (int k = 0; k < 2; k++)
+      if (cnt[k]) G[k] = std::max(1u, std::min(max_nb[k], (unsigned)((4ull * ndt_resident_blocks(k == 0) + cnt[k] - 1) / cnt[k])));
+    G[2] = max_nb[2];
+    const unsigned long long seq = ++b->ndt_seq;
+    for (size_t r = 0; r < order.size(); r++) {
+      const size_t i = order[r];
+      const int k = kind_of[r];
+      Cloud& s = *b->clouds[pairs[i].source];
+      Cloud& t = *b->clouds[pairs[i].target];
+      NdtArgs& A = b->h_ndt_args[r];
+      ndt_fill_args(cfg, s, t, S[i].K, S[i].Tfinal, k != NDT_PASS_DERIV, A);
+      const NdtPairWs w = ndt_pair_ws(s);
+      char* p = base + off[i];
+      A.partials = reinterpret_cast<double*>(p + w.partials);
+      A.grows = reinterpret_cast<double*>(p + w.grows);
+      A.gcount = reinterpret_cast<unsigned int*>(p + w.gcount);
+      A.counter = reinterpret_cast<unsigned int*>(p + w.small);
+      A.pairs = reinterpret_cast<unsigned long long*>(p + w.small + 16);
+      A.queue = reinterpret_cast<unsigned long long*>(p + w.small + 24);
+      A.qbase = qnext[i];
+      if (k != NDT_PASS_HESS) qnext[i] += (unsigned long long)(s.nsup * 1024 / kNdtThreads) + G[k];  // chunks + one closing draw per block
+      A.out = b->h_ndt_msg_dev + r * kNdtMsg;
+      A.flag = flag_dev;
+      A.seq = seq;
+      A.round = b->d_ndt_round;
+      A.round_n = (unsigned)order.size();
+    }
+    B2R_CUDA(cudaMemcpyAsync(b->d_ndt_args.p, b->h_ndt_args, order.size() * sizeof(NdtArgs), cudaMemcpyHostToDevice, st));
+    h->tel.h2d += order.size() * sizeof(NdtArgs);
+    size_t r0 = 0;
+    for (int k = 0; k < 3; k++) {
+      if (!cnt[k]) continue;
+      const dim3 grid(G[k], (unsigned)cnt[k]);
+      TEL_BEGIN(&h->tel, st);
+      if (k == NDT_PASS_DERIV_HESS) k_ndt_derivatives_batch<true><<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
+      else if (k == NDT_PASS_DERIV) k_ndt_derivatives_batch<false><<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
+      else k_ndt_hessian_batch<<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
+      TEL_END(&h->tel, k == NDT_PASS_HESS ? KC_NDT_HESS : KC_NDT_DERIV, 1, st);
+      B2R_CUDA(cudaGetLastError());
+      r0 += cnt[k];
+    }
+    h->tel.d2h += order.size() * kNdtMsg * sizeof(double);
+    b->last_rounds++;
+    for (size_t r = 0; r < order.size(); r++) {  // the first wait covers the round; the rest only check each message
+      const int k = kind_of[r];
+      const double* msg = b->h_ndt_msg + r * kNdtMsg;
+      int rc = (k == NDT_PASS_HESS) ? wait_host_result(flag, seq, msg, 36, false, st) : wait_host_result(flag, seq, msg, kNdtAcc, true, st);
+      if (rc) return rc;
+      NdtPass P;
+      ndt_read_pass(msg, k != NDT_PASS_DERIV, k == NDT_PASS_HESS, &P);
+      S[order[r]].consume(P);
+    }
+    size_t keep = 0;
+    for (size_t i : active)
+      if (S[i].next() != NDT_PASS_DONE) active[keep++] = i;
+    active.resize(keep);
+  }
+  // getFitnessScore at each final pose: the kernel and reduction of b2r_fitness, one launch per pair, one wait for all
+  std::vector<double> fit(m * 3, 0.0);
+  if (want_fitness) {
+    double* d_fit = reinterpret_cast<double*>(base + fit_out);
+    for (size_t i = 0; i < m; i++) {
+      Cloud& s = *b->clouds[pairs[i].source];
+      Cloud& t = *b->clouds[pairs[i].target];
+      if (s.n == 0 || t.n == 0) continue;
+      const size_t nb = (size_t)s.nsup * 1024 / kLinThreads;
+      FitArgs A;
+      A.src = s.bvh(); A.tgt = t.bvh();
+      for (int k = 0; k < 12; k++) A.Tf[k] = S[i].Tfinal[k];
+      A.max_range = fit_max_range; A.inlier_thresh_sq = 0.25f;
+      A.partials = reinterpret_cast<double*>(base + fit_off[i]);
+      A.counter = reinterpret_cast<unsigned int*>(base + fit_off[i] + align_up(nb * 3 * sizeof(double), 256));
+      A.out = d_fit + 3 * i;
+      TEL_BEGIN(&h->tel, st);
+      k_fitness<<<(unsigned)nb, kLinThreads, 0, st>>>(A);
+      TEL_END(&h->tel, KC_FITNESS, 1, st);
+      B2R_CUDA(cudaGetLastError());
+    }
+    B2R_CUDA(cudaMemcpyAsync(fit.data(), d_fit, m * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+    B2R_CUDA(cudaStreamSynchronize(st));
+    h->tel.d2h += m * 3 * sizeof(double);
+  }
+  for (size_t i = 0; i < m; i++) {
+    PairReport& R = rep[i];
+    std::memset(&R, 0, sizeof(R));
+    for (int r = 0; r < 4; r++)
+      for (int c = 0; c < 4; c++) R.r.T[c * 4 + r] = S[i].Tfinal[r * 4 + c];
+    const double nr = fit[3 * i + 1];
+    R.r.fitness = !want_fitness ? NAN : (nr > 0 ? fit[3 * i] / nr : DBL_MAX);
+    R.r.converged = S[i].converged ? 1 : 0;
+    R.r.iterations = S[i].nr_iterations;
+    R.rounds = S[i].passes;
+  }
+  return B2R_OK;
+}
+
 __global__ void k_pack_results(const PairReport* rep, int n, b2r_result* out, int n_out, unsigned long long* round_sum) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_out) return;
@@ -489,7 +699,10 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   if (rc) return rc;
   std::vector<int32_t> named(2 * n_pairs);
   for (size_t i = 0; i < n_pairs; i++) { named[2 * i] = pairs[i].source; named[2 * i + 1] = pairs[i].target; }
-  rc = batch_build_structures(b, named.data(), named.size(), !fit_only);
+  const bool ndt = h->cfg.method == B2R_METHOD_NDT;
+  rc = batch_build_structures(b, named.data(), named.size(), !fit_only && !ndt);
+  if (rc) return rc;
+  if (ndt) rc = batch_ndt_maps(b, pairs, n_pairs, fit_only);
   if (rc) return rc;
   const auto t_b = std::chrono::steady_clock::now();
   const size_t chunk = std::min(b->max_chunk, std::max<size_t>(n_pairs, 1));
@@ -500,9 +713,13 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   b->last_rounds = b->last_pair_rounds = 0;
   for (size_t c0 = 0; c0 < n_pairs; c0 += chunk) {
     const size_t m = std::min(chunk, n_pairs - c0);
-    rc = batch_run_chunk(b, pairs + c0, m, cfg, b->d_reports.p + c0, fit_only);
+    // an NDT align runs its own rounds; a stand-alone fitness evaluation is the same search on either engine
+    if (ndt && !fit_only) rc = batch_run_ndt_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports + c0);
+    else rc = batch_run_chunk(b, pairs + c0, m, cfg, b->d_reports.p + c0, fit_only);
     if (rc) return rc;
   }
+  if (ndt && !fit_only)  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
+    B2R_CUDA(cudaMemcpyAsync(b->d_reports.p, b->h_reports, n_pairs * sizeof(PairReport), cudaMemcpyHostToDevice, h->st));
   if (dbg) {
     const auto t_c = std::chrono::steady_clock::now();
     fprintf(stderr, "[b2r rank %d] batch_run: build enqueue %.3f ms, rounds (host follows the device) %.3f ms, %llu rounds\n", b->rank,

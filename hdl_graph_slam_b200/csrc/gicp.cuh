@@ -324,29 +324,46 @@ __device__ __forceinline__ void block_reduce(double* v, double* smem /* NV * 32 
 // checksum word (out[NV+1]; out[NV] carries `extra` or is unused) and `flag` = `seq`, so the host can spin on it instead of paying a
 // memcpy + stream sync.
 // finish_stored: thread 0 of every block has already written the block's NV sums to partials[blockIdx.x][0..NV)
+// nrow_in: blocks that take part (0 = gridDim.x; a batched launch whose grid.x covers its largest pair passes the pair's own count).
+// round / round_n: several reductions publish under ONE flag (a batched NDT round): each bumps *round after writing its message and
+// the last of round_n writes flag = seq; every message still carries its own checksum.
 template <int NV>
 __device__ __forceinline__ void finish_stored(double* partials, double* out, unsigned int* counter, unsigned long long* flag = nullptr,
-                                              unsigned long long seq = 0, unsigned long long* extra = nullptr);
+                                              unsigned long long seq = 0, unsigned long long* extra = nullptr, unsigned int nrow_in = 0,
+                                              unsigned int* round = nullptr, unsigned int round_n = 0);
 
 template <int NV>
 __device__ __forceinline__ void finish_partials(const double* v, double* partials, double* out, unsigned int* counter,
                                                 unsigned long long* flag = nullptr, unsigned long long seq = 0,
-                                                unsigned long long* extra = nullptr) {
+                                                unsigned long long* extra = nullptr, unsigned int nrow_in = 0,
+                                                unsigned int* round = nullptr, unsigned int round_n = 0) {
   if (threadIdx.x == 0) {
 #pragma unroll
     for (int i = 0; i < NV; i++) partials[(size_t)blockIdx.x * NV + i] = v[i];
   }
-  finish_stored<NV>(partials, out, counter, flag, seq, extra);
+  finish_stored<NV>(partials, out, counter, flag, seq, extra, nrow_in, round, round_n);
+}
+
+// the last message of a round publishes the round's flag (round == nullptr: every message has its own flag)
+__device__ __forceinline__ void publish_flag(unsigned long long* flag, unsigned long long seq, unsigned int* round, unsigned int round_n) {
+  if (round) {
+    __threadfence();
+    if (atomicAdd(round, 1u) != round_n - 1) return;
+    *round = 0;  // all of this round's messages are in: re-armed for the next round
+  }
+  *reinterpret_cast<volatile unsigned long long*>(flag) = seq;
 }
 
 template <int NV>
 __device__ __forceinline__ void finish_stored(double* partials, double* out, unsigned int* counter, unsigned long long* flag,
-                                              unsigned long long seq, unsigned long long* extra) {
+                                              unsigned long long seq, unsigned long long* extra, unsigned int nrow_in,
+                                              unsigned int* round, unsigned int round_n) {
   __shared__ bool is_last;
+  const unsigned int nrow = nrow_in ? nrow_in : gridDim.x;
   if (threadIdx.x == 0) {
     __threadfence();
     unsigned int t = atomicAdd(counter, 1u);
-    is_last = (t == gridDim.x - 1);
+    is_last = (t == nrow - 1);
   }
   __syncthreads();
   if (is_last) {
@@ -357,7 +374,6 @@ __device__ __forceinline__ void finish_stored(double* partials, double* out, uns
     __shared__ double fin[8 * NV];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int nw = (blockDim.x >> 5) < 8 ? (int)(blockDim.x >> 5) : 8;
-    const unsigned int nrow = gridDim.x;
     if (warp < nw) {
       for (int i = lane; i < NV; i += 32) {
         double s = 0.0;
@@ -396,7 +412,7 @@ __device__ __forceinline__ void finish_stored(double* partials, double* out, uns
         // does not matter (wait_host_result re-reads until the message is self-consistent).
         for (int i = 0; i < NV; i++) x ^= msg_mix((unsigned long long)__double_as_longlong(fin[i]), i);
         reinterpret_cast<unsigned long long*>(out)[NV + 1] = x;
-        *reinterpret_cast<volatile unsigned long long*>(flag) = seq;
+        publish_flag(flag, seq, round, round_n);
       }
     }
   }

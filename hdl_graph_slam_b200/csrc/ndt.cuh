@@ -229,6 +229,8 @@ struct NdtArgs {
   unsigned long long* pairs;
   unsigned long long* flag;  // host-mapped completion flag
   unsigned long long seq;
+  unsigned int* round;       // batched round: every pair's message bumps it, the last of round_n publishes `flag` (nullptr: single pass)
+  unsigned int round_n;
 };
 
 __device__ __forceinline__ float dot3f(const float* a, float x, float y, float z) {
@@ -286,7 +288,7 @@ __device__ __forceinline__ void ndt_rows_sum(const double* rows, int R, double* 
 }
 
 template <bool HESS>
-__global__ void __launch_bounds__(kNdtThreads, 4) k_ndt_derivatives(const __grid_constant__ NdtArgs A) {
+__device__ __forceinline__ void ndt_derivatives_body(const NdtArgs& A) {
   __shared__ __align__(16) NdtCell s_cell[kNdtSlots];  // staged voxel records; after the pair loop: rows of the register sums
   __shared__ double s_low[kNdtAccB][kNdtRow];          // strict lower triangle of H: one float64 column per thread (no conflicts, no sync)
   __shared__ double s_fin[kNdtAcc];
@@ -547,16 +549,25 @@ __global__ void __launch_bounds__(kNdtThreads, 4) k_ndt_derivatives(const __grid
         x ^= msg_mix(e, kNdtAcc);
         for (int i = 0; i < kNdtAcc; i++) x ^= msg_mix((unsigned long long)__double_as_longlong(s_fin[i]), i);
         reinterpret_cast<unsigned long long*>(A.out)[kNdtAcc + 1] = x;
-        *reinterpret_cast<volatile unsigned long long*>(A.flag) = A.seq;
+        publish_flag(A.flag, A.seq, A.round, A.round_n);
       }
     }
   }
   }
 }
 
+template <bool HESS>
+__global__ void __launch_bounds__(kNdtThreads, 4) k_ndt_derivatives(const __grid_constant__ NdtArgs A) { ndt_derivatives_body<HESS>(A); }
 
-// float64 Hessian-only pass (ndt_omp computeHessian/updateHessian)
-__global__ void __launch_bounds__(kNdtThreads) k_ndt_hessian(const __grid_constant__ NdtArgs A) {
+// The same pass for many pairs at once: blockIdx.y = the pair's record.  Each pair draws its chunks from its own ticket counter
+// and reduces through its own rows and counters, i.e. through exactly the partition and tree of k_ndt_derivatives: its sums do
+// not depend on which pairs share the launch or on how the blocks are scheduled.
+template <bool HESS>
+__global__ void __launch_bounds__(kNdtThreads, 4) k_ndt_derivatives_batch(const NdtArgs* __restrict__ recs) { ndt_derivatives_body<HESS>(recs[blockIdx.y]); }
+
+
+// float64 Hessian-only pass (ndt_omp computeHessian/updateHessian); nrow = the source's 128-point blocks
+__device__ __forceinline__ void ndt_hessian_body(const NdtArgs& A, unsigned int nrow) {
   __shared__ double red[36 * 32];
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   double acc[36];
@@ -620,7 +631,17 @@ __global__ void __launch_bounds__(kNdtThreads) k_ndt_hessian(const __grid_consta
     }
   }
   block_reduce<36>(acc, red);
-  finish_partials<36>(acc, A.partials, A.out, A.counter, A.flag, A.seq);
+  finish_partials<36>(acc, A.partials, A.out, A.counter, A.flag, A.seq, nullptr, nrow, A.round, A.round_n);
+}
+
+__global__ void __launch_bounds__(kNdtThreads) k_ndt_hessian(const __grid_constant__ NdtArgs A) { ndt_hessian_body(A, gridDim.x); }
+
+// many pairs: blockIdx.y = the pair's record, grid.x covers the largest source; block b of a pair is block b of its own pass
+__global__ void __launch_bounds__(kNdtThreads) k_ndt_hessian_batch(const NdtArgs* __restrict__ recs) {
+  const NdtArgs& A = recs[blockIdx.y];
+  const unsigned int nb = (unsigned int)A.n_sorted / kNdtThreads;
+  if (blockIdx.x >= nb) return;  // block-uniform
+  ndt_hessian_body(A, nb);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -917,10 +938,10 @@ inline unsigned ndt_resident_blocks(bool hess) {
   return c;
 }
 
-inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& W, cudaStream_t st, const NdtScalars& K, const float* Tf_row,
-                        bool compute_hessian, bool hessian_only, NdtPass* out) {
-  NdtVoxelMap& M = *tgt.ndt;
-  NdtArgs A;
+// the pass's inputs: source points, target voxel map, pose and angle derivatives (workspace and publication are the caller's)
+inline void ndt_fill_args(const b2r_config& cfg, const Cloud& src, const Cloud& tgt, const NdtScalars& K, const float* Tf_row, bool compute_hessian,
+                          NdtArgs& A) {
+  const NdtVoxelMap& M = *tgt.ndt;
   A.src = src.sorted.p; A.n_sorted = src.nsup * 1024;
   A.geom = M.geom; A.table = M.table.p; A.mask = M.mask; A.cells = M.cells.p; A.vox = M.vox.p;
   for (int i = 0; i < 12; i++) A.Tf[i] = Tf_row[i];
@@ -929,6 +950,31 @@ inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& 
   A.d1 = K.d1; A.d2 = K.d2;
   A.ncell_search = (cfg.ndt_search_method == 1) ? 1 : 7;
   A.compute_hessian = compute_hessian ? 1 : 0;
+  A.round = nullptr; A.round_n = 0;
+}
+
+// a published result message -> NdtPass (a Hessian-only pass delivers H alone)
+inline void ndt_read_pass(const double* msg, bool compute_hessian, bool hessian_only, NdtPass* out) {
+  if (hessian_only) {
+    std::memcpy(out->H, msg, 36 * sizeof(double));
+    return;
+  }
+  out->score = msg[0];
+  std::memcpy(out->g, msg + 1, 6 * sizeof(double));
+  if (compute_hessian) {
+    int k = 7;
+    for (int r = 0; r < 6; r++)
+      for (int c = r; c < 6; c++) out->H[r * 6 + c] = msg[k++];     // first sweep: ii <= jj
+    for (int r = 1; r < 6; r++)
+      for (int c = 0; c < r; c++) out->H[r * 6 + c] = msg[k++];     // second sweep: ii > jj
+  }
+  std::memcpy(&out->pairs, msg + kNdtAcc, sizeof(unsigned long long));
+}
+
+inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& W, cudaStream_t st, const NdtScalars& K, const float* Tf_row,
+                        bool compute_hessian, bool hessian_only, NdtPass* out) {
+  NdtArgs A;
+  ndt_fill_args(cfg, src, tgt, K, Tf_row, compute_hessian, A);
   const unsigned nb = (unsigned)((size_t)src.nsup * 1024 / kNdtThreads);  // 128-point chunks of the source
   B2R_CUDA(W.partials.reserve((size_t)(nb + 1) * kNdtAcc));  // derivative pass: [chunks][kNdtAcc]; Hessian pass: [blocks][36]
   const unsigned ngroups = (nb + 31) / 32;
@@ -948,7 +994,7 @@ inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& 
     B2R_CUDA(cudaGetLastError());
     int rc = wait_host_result(W.h_flag, A.seq, W.h_out, 36, false, st);
     if (rc) return rc;
-    std::memcpy(out->H, W.h_out, 36 * sizeof(double));
+    ndt_read_pass(W.h_out, true, true, out);
     return B2R_OK;
   }
   { TEL_BEGIN(W.tel, st);  // W.d_pairs is zero here: allocated zeroed, and the last block of every pass resets it after reading it
@@ -964,16 +1010,7 @@ inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& 
   B2R_CUDA(cudaGetLastError());
   int rc = wait_host_result(W.h_flag, A.seq, W.h_out, kNdtAcc, true, st);
   if (rc) return rc;
-  out->score = W.h_out[0];
-  std::memcpy(out->g, W.h_out + 1, 6 * sizeof(double));
-  if (compute_hessian) {
-    int k = 7;
-    for (int r = 0; r < 6; r++)
-      for (int c = r; c < 6; c++) out->H[r * 6 + c] = W.h_out[k++];     // first sweep: ii <= jj
-    for (int r = 1; r < 6; r++)
-      for (int c = 0; c < r; c++) out->H[r * 6 + c] = W.h_out[k++];     // second sweep: ii > jj
-  }
-  std::memcpy(&out->pairs, W.h_out + kNdtAcc, sizeof(unsigned long long));
+  ndt_read_pass(W.h_out, compute_hessian, false, out);
   return B2R_OK;
 }
 
@@ -1047,95 +1084,82 @@ inline bool mt_update(double& a_l, double& f_l, double& g_l, double& a_u, double
   return true;
 }
 
-// pclomp::NormalDistributionsTransform::computeTransformation (A.2).  guess: column-major float (ABI); Tfinal: row-major.
-inline int ndt_align(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& W, cudaStream_t st, const float* guess_col, float* Tfinal,
-                     bool* converged_out, int* iters_out) {
-  for (int i = 0; i < 16; i++) Tfinal[i] = (i % 5 == 0) ? 1.f : 0.f;
-  *converged_out = false;
-  *iters_out = 0;
-  if (src.n == 0 || tgt.n == 0) return B2R_OK;  // initCompute fails silently
-  int rc = ndt_ensure_map(cfg, tgt, W, st);
-  if (rc) return rc;
-  rc = ndt_sync_geom(*tgt.ndt, W, st);
-  if (rc) return rc;
-  if (tgt.ndt->h_geom.empty) return B2R_OK;
+// pclomp::NormalDistributionsTransform::computeTransformation (A.2) as a resumable state machine: next() names the pass the
+// registration needs (pose matrix Tf and angle derivatives K), consume() takes its result and runs the host scalar code up to the
+// next request.  ndt_align drives one pair with it; the batch (batch.cuh) drives many, one batched pass per round.  Both run these
+// very statements, so a pair's result does not depend on which driver ran it.
+enum NdtPassKind : int { NDT_PASS_DERIV_HESS = 0, NDT_PASS_DERIV = 1, NDT_PASS_HESS = 2, NDT_PASS_DONE = 3 };
+
+struct NdtPairState {
+  enum Stage : int { FIRST, LS_FIRST, LS_ITER, HESS_ONLY, DONE };
+  const b2r_config* cfg = nullptr;
   NdtScalars K;
-  ndt_gauss(cfg, K);
-  float guess[16];
-  for (int r = 0; r < 4; r++)
-    for (int c = 0; c < 4; c++) guess[r * 4 + c] = guess_col[c * 4 + r];
-  bool is_identity = true;
-  for (int i = 0; i < 16; i++) is_identity &= (guess[i] == ((i % 5 == 0) ? 1.f : 0.f));
-  if (!is_identity) std::memcpy(Tfinal, guess, sizeof(guess));
-  double p[6];
-  {
+  float Tfinal[16];  // row-major: the pose matrix of the last pass (the registration's result once DONE)
+  double p[6], score = 0, g[6], H[36], dp[6];
+  int nr_iterations = 0;
+  bool converged = false;
+  int stage = DONE;
+  int passes = 0;
+  // More-Thuente line search of the current iteration
+  double step_max = 0, step_min = 0, phi_0 = 0, d_phi_0 = 0, a_t = 0;
+  double a_l = 0, a_u = 0, f_l = 0, g_l = 0, f_u = 0, g_u = 0;
+  double phi_t = 0, d_phi_t = 0, psi_t = 0, d_psi_t = 0;
+  bool interval_converged = false, open_interval = true;
+  int step_iterations = 0;
+  static constexpr double mu = 1.e-4, nu = 0.9;
+
+  NdtPairState() { for (int i = 0; i < 16; i++) Tfinal[i] = (i % 5 == 0) ? 1.f : 0.f; }
+
+  // guess: column-major float (ABI).  The first pass transforms the cloud by the guess matrix itself.
+  void start(const b2r_config& c, const float* guess_col) {
+    cfg = &c;
+    ndt_gauss(c, K);
+    float guess[16];
+    for (int r = 0; r < 4; r++)
+      for (int cc = 0; cc < 4; cc++) guess[r * 4 + cc] = guess_col[cc * 4 + r];
+    bool is_identity = true;
+    for (int i = 0; i < 16; i++) is_identity &= (guess[i] == ((i % 5 == 0) ? 1.f : 0.f));
+    if (!is_identity) std::memcpy(Tfinal, guess, sizeof(guess));
     float e[3];
     ndt_euler_xyz(Tfinal, e);
     p[0] = Tfinal[3]; p[1] = Tfinal[7]; p[2] = Tfinal[11];
     p[3] = e[0]; p[4] = e[1]; p[5] = e[2];
+    ndt_angle_derivs(p, K);
+    nr_iterations = 0;
+    converged = false;
+    passes = 0;
+    stage = FIRST;
   }
-  ndt_angle_derivs(p, K);
-  NdtPass P;
-  rc = ndt_run_pass(cfg, src, tgt, W, st, K, Tfinal, true, false, &P);  // first pass: cloud transformed by the guess matrix itself
-  if (rc) return rc;
-  double score = P.score, g[6], H[36];
-  std::memcpy(g, P.g, sizeof(g));
-  std::memcpy(H, P.H, sizeof(H));
-  int nr_iterations = 0;
-  bool converged = false;
-  const int max_it = cfg.max_iterations;
-  while (!converged) {
-    double ng[6], dp[6];
-    for (int i = 0; i < 6; i++) ng[i] = -g[i];
-    ndt_svd6_solve(H, ng, dp);
-    double nrm = 0;
-    for (int i = 0; i < 6; i++) nrm += dp[i] * dp[i];
-    nrm = std::sqrt(nrm);
-    if (nrm == 0 || nrm != nrm) { converged = (nrm == nrm); break; }
-    for (int i = 0; i < 6; i++) dp[i] /= nrm;
-    const double step_max = cfg.ndt_step_size, step_min = cfg.transformation_epsilon / 2;
-    const double phi_0 = -score;
-    double d_phi_0 = 0;
-    for (int i = 0; i < 6; i++) d_phi_0 += g[i] * dp[i];
-    d_phi_0 = -d_phi_0;
-    double a_t = 0;
-    bool skip = false;
-    if (d_phi_0 >= 0) {
-      if (d_phi_0 == 0) { skip = true; a_t = 0; }
-      else { d_phi_0 *= -1; for (int i = 0; i < 6; i++) dp[i] *= -1; }
+
+  int next() const {
+    switch (stage) {
+      case FIRST: case LS_FIRST: return NDT_PASS_DERIV_HESS;
+      case LS_ITER: return NDT_PASS_DERIV;
+      case HESS_ONLY: return NDT_PASS_HESS;
+      default: return NDT_PASS_DONE;
     }
-    if (!skip) {
-      const double mu = 1.e-4, nu = 0.9;
-      double a_l = 0, a_u = 0;
-      double f_l = mt_psi(a_l, phi_0, phi_0, d_phi_0, mu), g_l = mt_dpsi(d_phi_0, d_phi_0, mu);
-      double f_u = mt_psi(a_u, phi_0, phi_0, d_phi_0, mu), g_u = mt_dpsi(d_phi_0, d_phi_0, mu);
-      bool interval_converged = cfg.ndt_mt_interval_flag ? ((step_max - step_min) < 0) : ((step_max - step_min) > 0);
-      bool open_interval = true;
-      int step_iterations = 0;
-      a_t = nrm;
-      a_t = std::min(a_t, step_max);
-      a_t = std::max(a_t, step_min);
-      double x_t[6];
-      for (int i = 0; i < 6; i++) x_t[i] = p[i] + dp[i] * a_t;
-      ndt_pose_to_matrix(x_t, Tfinal);
-      ndt_angle_derivs(x_t, K);
-      rc = ndt_run_pass(cfg, src, tgt, W, st, K, Tfinal, true, false, &P);
-      if (rc) return rc;
-      score = P.score; std::memcpy(g, P.g, sizeof(g)); std::memcpy(H, P.H, sizeof(H));
-      double phi_t = -score, d_phi_t = 0;
-      for (int i = 0; i < 6; i++) d_phi_t += g[i] * dp[i];
-      d_phi_t = -d_phi_t;
-      double psi_t = mt_psi(a_t, phi_t, phi_0, d_phi_0, mu), d_psi_t = mt_dpsi(d_phi_t, d_phi_0, mu);
-      while (!interval_converged && step_iterations < 10 && !(psi_t <= 0 && d_phi_t <= -nu * d_phi_0)) {
-        if (open_interval) a_t = mt_trial(a_l, f_l, g_l, a_u, f_u, g_u, a_t, psi_t, d_psi_t);
-        else a_t = mt_trial(a_l, f_l, g_l, a_u, f_u, g_u, a_t, phi_t, d_phi_t);
-        a_t = std::min(a_t, step_max);
-        a_t = std::max(a_t, step_min);
-        for (int i = 0; i < 6; i++) x_t[i] = p[i] + dp[i] * a_t;
-        ndt_pose_to_matrix(x_t, Tfinal);
-        ndt_angle_derivs(x_t, K);
-        rc = ndt_run_pass(cfg, src, tgt, W, st, K, Tfinal, false, false, &P);
-        if (rc) return rc;
+  }
+
+  void consume(const NdtPass& P) {
+    passes++;
+    switch (stage) {
+      case FIRST:
+        score = P.score;
+        std::memcpy(g, P.g, sizeof(g));
+        std::memcpy(H, P.H, sizeof(H));
+        iterate();
+        return;
+      case LS_FIRST:
+        score = P.score; std::memcpy(g, P.g, sizeof(g)); std::memcpy(H, P.H, sizeof(H));
+        phi_t = -score;
+        d_phi_t = 0;
+        for (int i = 0; i < 6; i++) d_phi_t += g[i] * dp[i];
+        d_phi_t = -d_phi_t;
+        psi_t = mt_psi(a_t, phi_t, phi_0, d_phi_0, mu);
+        d_psi_t = mt_dpsi(d_phi_t, d_phi_0, mu);
+        line_search();
+        return;
+      case LS_ITER:
         score = P.score; std::memcpy(g, P.g, sizeof(g));
         phi_t = -score;
         d_phi_t = 0;
@@ -1153,24 +1177,118 @@ inline int ndt_align(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& W, 
         if (open_interval) interval_converged = mt_update(a_l, f_l, g_l, a_u, f_u, g_u, a_t, psi_t, d_psi_t);
         else interval_converged = mt_update(a_l, f_l, g_l, a_u, f_u, g_u, a_t, phi_t, d_phi_t);
         step_iterations++;
-      }
-      if (step_iterations) {
-        rc = ndt_run_pass(cfg, src, tgt, W, st, K, Tfinal, true, true, &P);
-        if (rc) return rc;
+        line_search();
+        return;
+      case HESS_ONLY:
         std::memcpy(H, P.H, sizeof(H));
-      }
+        end_iteration();
+        iterate();
+        return;
+      default:
+        return;
     }
+  }
+
+ private:
+  // the top of the Newton loop (while (!converged)) up to the next pass request, or to its end
+  void iterate() {
+    while (!converged) {
+      double ng[6];
+      for (int i = 0; i < 6; i++) ng[i] = -g[i];
+      ndt_svd6_solve(H, ng, dp);
+      double nrm = 0;
+      for (int i = 0; i < 6; i++) nrm += dp[i] * dp[i];
+      nrm = std::sqrt(nrm);
+      if (nrm == 0 || nrm != nrm) { converged = (nrm == nrm); break; }
+      for (int i = 0; i < 6; i++) dp[i] /= nrm;
+      step_max = cfg->ndt_step_size; step_min = cfg->transformation_epsilon / 2;
+      phi_0 = -score;
+      d_phi_0 = 0;
+      for (int i = 0; i < 6; i++) d_phi_0 += g[i] * dp[i];
+      d_phi_0 = -d_phi_0;
+      a_t = 0;
+      bool skip = false;
+      if (d_phi_0 >= 0) {
+        if (d_phi_0 == 0) { skip = true; a_t = 0; }
+        else { d_phi_0 *= -1; for (int i = 0; i < 6; i++) dp[i] *= -1; }
+      }
+      if (!skip) {
+        a_l = 0; a_u = 0;
+        f_l = mt_psi(a_l, phi_0, phi_0, d_phi_0, mu); g_l = mt_dpsi(d_phi_0, d_phi_0, mu);
+        f_u = mt_psi(a_u, phi_0, phi_0, d_phi_0, mu); g_u = mt_dpsi(d_phi_0, d_phi_0, mu);
+        interval_converged = cfg->ndt_mt_interval_flag ? ((step_max - step_min) < 0) : ((step_max - step_min) > 0);
+        open_interval = true;
+        step_iterations = 0;
+        a_t = nrm;
+        a_t = std::min(a_t, step_max);
+        a_t = std::max(a_t, step_min);
+        request_trial(LS_FIRST);
+        return;
+      }
+      end_iteration();
+    }
+    stage = DONE;
+  }
+
+  // x_t = p + dp * a_t: the pose of the next trial pass
+  void request_trial(int next_stage) {
+    double x_t[6];
+    for (int i = 0; i < 6; i++) x_t[i] = p[i] + dp[i] * a_t;
+    ndt_pose_to_matrix(x_t, Tfinal);
+    ndt_angle_derivs(x_t, K);
+    stage = next_stage;
+  }
+
+  // the More-Thuente loop condition after a trial pass; then the Hessian-only pass if the loop ran, or the end of the iteration
+  void line_search() {
+    if (!interval_converged && step_iterations < 10 && !(psi_t <= 0 && d_phi_t <= -nu * d_phi_0)) {
+      if (open_interval) a_t = mt_trial(a_l, f_l, g_l, a_u, f_u, g_u, a_t, psi_t, d_psi_t);
+      else a_t = mt_trial(a_l, f_l, g_l, a_u, f_u, g_u, a_t, phi_t, d_phi_t);
+      a_t = std::min(a_t, step_max);
+      a_t = std::max(a_t, step_min);
+      request_trial(LS_ITER);
+      return;
+    }
+    if (step_iterations) { stage = HESS_ONLY; return; }
+    end_iteration();
+    iterate();
+  }
+
+  void end_iteration() {
     const double delta_p_norm = a_t;
     for (int i = 0; i < 6; i++) { dp[i] *= delta_p_norm; p[i] += dp[i]; }
-    if (cfg.ndt_fixed_iterations > 0) {
-      if (nr_iterations + 1 >= cfg.ndt_fixed_iterations) converged = true;
-    } else if (nr_iterations > max_it || (nr_iterations && (std::fabs(delta_p_norm) < cfg.transformation_epsilon))) {
+    if (cfg->ndt_fixed_iterations > 0) {
+      if (nr_iterations + 1 >= cfg->ndt_fixed_iterations) converged = true;
+    } else if (nr_iterations > cfg->max_iterations || (nr_iterations && (std::fabs(delta_p_norm) < cfg->transformation_epsilon))) {
       converged = true;
     }
     nr_iterations++;
   }
-  *converged_out = converged;
-  *iters_out = nr_iterations;
+};
+
+// one pair on the handle's stream: one host wait per pass.  guess: column-major float (ABI); Tfinal: row-major.
+inline int ndt_align(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& W, cudaStream_t st, const float* guess_col, float* Tfinal,
+                     bool* converged_out, int* iters_out) {
+  for (int i = 0; i < 16; i++) Tfinal[i] = (i % 5 == 0) ? 1.f : 0.f;
+  *converged_out = false;
+  *iters_out = 0;
+  if (src.n == 0 || tgt.n == 0) return B2R_OK;  // initCompute fails silently
+  int rc = ndt_ensure_map(cfg, tgt, W, st);
+  if (rc) return rc;
+  rc = ndt_sync_geom(*tgt.ndt, W, st);
+  if (rc) return rc;
+  if (tgt.ndt->h_geom.empty) return B2R_OK;
+  NdtPairState S;
+  S.start(cfg, guess_col);
+  for (int kind = S.next(); kind != NDT_PASS_DONE; kind = S.next()) {
+    NdtPass P;
+    rc = ndt_run_pass(cfg, src, tgt, W, st, S.K, S.Tfinal, kind != NDT_PASS_DERIV, kind == NDT_PASS_HESS, &P);
+    if (rc) return rc;
+    S.consume(P);
+  }
+  std::memcpy(Tfinal, S.Tfinal, sizeof(S.Tfinal));
+  *converged_out = S.converged;
+  *iters_out = S.nr_iterations;
   return B2R_OK;
 }
 

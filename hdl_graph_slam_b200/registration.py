@@ -551,7 +551,7 @@ def loop_argmin(results, fitness_score_thresh):
 
 
 class RegistrationBatch:
-    """Batched, device-resident GICP registration (include/b200reg.h: b2r_batch_*): keyframe clouds are registered once and many
+    """Batched, device-resident GICP or NDT registration (include/b200reg.h: b2r_batch_*): keyframe clouds are registered once and many
     (source, target, guess) pairs are aligned per launch — the candidate loop of LoopDetector::matching
     (include/hdl_graph_slam/loop_detector.hpp:135-154) for one or many new keyframes."""
 

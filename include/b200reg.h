@@ -329,11 +329,15 @@ int b2r_loop_matching(b2r_handle* h, const void* new_keyframe, size_t n_new, siz
 
 /* ---- batched, device-resident registration (north_star's multi-GPU split; loop_detector.hpp:135-154) --------------------
  * A b2r_batch lives on ONE GPU (cfg->device_id).  Keyframe clouds are registered once (b2r_batch_add_cloud: upload, search
- * structure, GICP covariances) and named by id; b2r_batch_align runs MANY (source, target, guess) registrations at once:
- * one pair of kernel launches per LM iteration covers every pair still in flight, the LM step (6x6 solve, se3_exp, rho test,
- * convergence) runs on the device, and the host reads the 80-byte records back once per batch.  Results are bitwise identical
- * to running each pair alone through b2r_set_target / b2r_set_source / b2r_align (+ b2r_fitness-equivalent score).
- * GICP engine only (the reference's loop closure uses FAST_GICP: launch/hdl_graph_slam.launch:127).
+ * structure, GICP covariances) and named by id; b2r_batch_align runs MANY (source, target, guess) registrations at once.
+ * GICP config: one pair of kernel launches per LM iteration covers every pair still in flight, the LM step (6x6 solve, se3_exp,
+ * rho test, convergence) runs on the device, and the host reads the 80-byte records back once per batch.  Results are bitwise
+ * identical to running each pair alone through b2r_set_target / b2r_set_source / b2r_align (+ b2r_fitness-equivalent score).
+ * NDT config (B2R_METHOD_NDT, the factory's default NDT_OMP): a cloud used as a target gets its voxel map at the first call
+ * that uses it (a cloud added from device memory at the first call that names it); every pair runs the single handle's
+ * Newton / More-Thuente driver and each round of derivative passes covers every pair in flight (one host wait per round).
+ * Pose, flag, iteration count and fitness are bitwise those of b2r_set_target / b2r_set_source / b2r_align / b2r_fitness on
+ * one NDT handle; b2r_batch_last_rounds counts batched rounds and, per pair, derivative / Hessian passes.
  *
  * Host buffers passed to b2r_batch_add_cloud may be pageable (copied before the call returns) or pinned (DMA'd in place:
  * keep them unmodified until the next b2r_batch_align / b2r_batch_loop_detect / b2r_batch_synchronize returns). */
