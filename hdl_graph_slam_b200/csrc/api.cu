@@ -42,16 +42,16 @@ using namespace b2r;
 
 struct b2r_handle {
   b2r_config cfg;
-  cudaStream_t st = nullptr;
+  Stream st;
   Cloud aux;                        // scratch cloud of the prefilter entry points (never a registration input)
   Cloud clouds[3];
   int src = 0, tgt = 1, nxt = 2;   // nxt: cloud being prefetched for the next set_source (software pipelining)
-  cudaStream_t st2 = nullptr;       // prefetch stream (upload + BVH + covariances of the next source overlap the current align)
-  cudaEvent_t ev_prefetch = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;  // first LM round beside the source's k-NN covariance kernel (run_single_pair)
+  Stream st2;                       // prefetch stream (upload + BVH + covariances of the next source overlap the current align)
+  Event ev_prefetch;
+  Event ev_fork, ev_join;           // first LM round beside the source's k-NN covariance kernel (run_single_pair)
   bool prefetched = false;
   unsigned long long prefetch_stamp = 0;   // content stamp of the prefetched host cloud (content_stamp)
-  cudaEvent_t upload_ev = nullptr;         // end of the last DMA out of a caller-owned pinned buffer
+  Event upload_ev;                         // end of the last DMA out of a caller-owned pinned buffer
   bool upload_pending = false;
   // per-align workspaces (sized by the source)
   DevBuf<int> corr[2], cpos[2];     // double-buffered: a speculative linearisation writes the other set
@@ -59,21 +59,20 @@ struct b2r_handle {
   DevBuf<double> mahal[2], partials;
   int cur = 0;                      // buffer set holding the correspondences of the last ACCEPTED linearisation
   // device-resident LM (pair_engine.cuh): the handle's single pair record and its host-mapped mailbox
-  PairDev* d_pair = nullptr;
+  DevBuf<PairDev> d_pair;
+  MappedBuf<char> mailbox;          // [0,128) report, [128,144) flag + progress, [256,512) tap values
   PairReport* h_rep = nullptr; PairReport* h_rep_dev = nullptr;          // report record (128 B, checksummed message)
   unsigned long long* h_pflag = nullptr; unsigned long long* h_pflag_dev = nullptr;  // [0] publication flag, [1] progress word
   double* h_tap = nullptr; double* h_tap_dev = nullptr;                  // parity taps: 29 reduced values
   int last_rounds = 0;              // rounds the previous align needed: that many (+1) are enqueued up front by the next one
   struct b2r_batch* loop_batch = nullptr;  // b2r_loop_matching runs the candidates of a keyframe as one batch (created on first use)
-  double* d_out = nullptr;          // 64 doubles
-  unsigned int* d_counter = nullptr;
-  double* h_out = nullptr;          // pinned + mapped, 64 doubles + flags: reduction kernels write results here directly
-  double* h_out_dev = nullptr;      // device alias
+  DevBuf<double> d_out;             // 64 doubles
+  DevBuf<unsigned int> d_counter;   // 4 words
+  MappedBuf<double> h_out;          // 64 doubles + flags: reduction kernels write results here directly
   unsigned long long* h_flag = nullptr; unsigned long long* h_flag_dev = nullptr; unsigned long long seq = 0;
   // staging for pageable uploads
-  void* staging[3] = {nullptr, nullptr, nullptr};
-  size_t staging_cap[3] = {0, 0, 0};
-  cudaEvent_t staging_ev[3] = {nullptr, nullptr, nullptr};
+  PinnedBuf<char> staging[3];
+  Event staging_ev[3];
   // misc device scratch (queries / outputs)
   DevBuf<float> tmp_f;
   DevBuf<int> tmp_i;
@@ -84,14 +83,14 @@ struct b2r_handle {
   DevBuf<int> pf_blocks;
   DevBuf<char> ingest_blob;         // PointCloud2 / PCD bodies as uploaded, and their PointXYZI unpacking
   DevBuf<float> ingest_out;
-  void* ingest_pinned = nullptr; size_t ingest_pinned_cap = 0;
+  PinnedBuf<char> ingest_pinned;
   DevBuf<char> map_kf;              // MapCloudGenerator: keyframe descriptors, voxel keys
   DevBuf<unsigned long long> map_keys[2];
-  MapGeom* map_geom = nullptr;
-  int* map_h = nullptr;
-  SorStats* pf_stats = nullptr;
-  int* pf_total = nullptr;
-  int* pf_h_total = nullptr; int* pf_h_total_dev = nullptr;
+  DevBuf<char> map_geom;            // MapGeom, then the first violator's index
+  PinnedBuf<int> map_h;             // 16 ints
+  DevBuf<SorStats> pf_stats;
+  DevBuf<int> pf_total;             // 4 ints
+  MappedBuf<int> pf_h_total;        // 4 ints
   BuildCtx bc[2];                   // per-stream build scratch (main stream, prefetch stream)
   bool knn_smem_attr = false, stat_smem_attr = false;
   int n_sm = 132;
@@ -183,7 +182,7 @@ extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
   if (e != cudaSuccess || ndev <= 0) return fail(B2R_ENODEVICE, std::string("no CUDA device: ") + cudaGetErrorString(e));
   if (cfg->device_id < 0 || cfg->device_id >= ndev) return fail(B2R_EINVAL, "device_id out of range");
   B2R_CUDA(cudaSetDevice(cfg->device_id));
-  b2r_handle* h = new b2r_handle();
+  std::unique_ptr<b2r_handle> h(new b2r_handle());  // on failure its members are freed on this (current) device
   h->cfg = *cfg;
   if (!(h->cfg.grid_cell_min > 0.f)) h->cfg.grid_cell_min = 0.5f;
   {  // round the cell size to a power of two
@@ -191,7 +190,6 @@ extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
     float m = std::frexp(h->cfg.grid_cell_min, &ex);
     h->cfg.grid_cell_min = std::ldexp(1.0f, m > 0.5f ? ex : ex - 1);
   }
-  auto bail = [&](int code) { b2r_destroy(h); return code; };
   cudaDeviceGetAttribute(&h->n_sm, cudaDevAttrMultiProcessorCount, cfg->device_id);
   if (h->n_sm <= 0) h->n_sm = 132;
   {  // the align path (latency-critical chain of small kernels) outranks the prefetch path (throughput work for the NEXT frame)
@@ -199,87 +197,47 @@ extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
     cudaDeviceGetStreamPriorityRange(&lo, &hi);
     if (getenv("B2R_NO_PRIORITY")) lo = hi = 0;
     if (getenv("B2R_PREFETCH_PRIORITY")) { const int t = lo; lo = hi; hi = t; }  // diagnostic: the prefetch path outranks the align chain
-    if (cudaStreamCreateWithPriority(&h->st, cudaStreamNonBlocking, hi) != cudaSuccess) return bail(fail(B2R_ECUDA, "cudaStreamCreate failed"));
-    if (cudaStreamCreateWithPriority(&h->st2, cudaStreamNonBlocking, lo) != cudaSuccess) return bail(fail(B2R_ECUDA, "cudaStreamCreate failed"));
+    if (h->st.create(cudaStreamNonBlocking, hi) != cudaSuccess) return fail(B2R_ECUDA, "cudaStreamCreate failed");
+    if (h->st2.create(cudaStreamNonBlocking, lo) != cudaSuccess) return fail(B2R_ECUDA, "cudaStreamCreate failed");
   }
-  if (cudaEventCreateWithFlags(&h->ev_prefetch, cudaEventDisableTiming) != cudaSuccess) return bail(fail(B2R_ECUDA, "cudaEventCreate failed"));
-  if (cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming) != cudaSuccess)
-    return bail(fail(B2R_ECUDA, "cudaEventCreate failed"));
-  if (cudaEventCreateWithFlags(&h->upload_ev, cudaEventDisableTiming) != cudaSuccess) return bail(fail(B2R_ECUDA, "cudaEventCreate failed"));
-  for (int i = 0; i < 3; i++) {
-    if (cudaEventCreateWithFlags(&h->staging_ev[i], cudaEventDisableTiming) != cudaSuccess) return bail(fail(B2R_ECUDA, "cudaEventCreate failed"));
-  }
+  if (h->ev_prefetch.create() != cudaSuccess || h->ev_fork.create() != cudaSuccess || h->ev_join.create() != cudaSuccess ||
+      h->upload_ev.create() != cudaSuccess)
+    return fail(B2R_ECUDA, "cudaEventCreate failed");
+  for (int i = 0; i < 3; i++)
+    if (h->staging_ev[i].create() != cudaSuccess) return fail(B2R_ECUDA, "cudaEventCreate failed");
   for (int i = 0; i < 2; i++)
-    if (cudaMalloc(&h->bc[i].mm, 8 * sizeof(int)) != cudaSuccess) return bail(fail(B2R_ECUDA, "device allocation failed"));
-  if (cudaMalloc(&h->d_out, 64 * sizeof(double)) != cudaSuccess ||
-      cudaMalloc(&h->d_counter, 4 * sizeof(unsigned int)) != cudaSuccess || cudaHostAlloc(&h->h_out, 72 * sizeof(double), cudaHostAllocMapped) != cudaSuccess ||
-      cudaHostGetDevicePointer((void**)&h->h_out_dev, h->h_out, 0) != cudaSuccess)
-    return bail(fail(B2R_ECUDA, "device allocation failed"));
-  h->h_flag = reinterpret_cast<unsigned long long*>(h->h_out + 64);
-  h->h_flag_dev = reinterpret_cast<unsigned long long*>(h->h_out_dev + 64);
+    if (h->bc[i].mm.alloc(8) != cudaSuccess) return fail(B2R_ECUDA, "device allocation failed");
+  if (h->d_out.alloc(64) != cudaSuccess || h->d_counter.alloc(4) != cudaSuccess || h->h_out.alloc(72) != cudaSuccess)
+    return fail(B2R_ECUDA, "device allocation failed");
+  h->h_flag = reinterpret_cast<unsigned long long*>(h->h_out.p + 64);
+  h->h_flag_dev = reinterpret_cast<unsigned long long*>(h->h_out.d + 64);
   h->h_flag[0] = h->h_flag[1] = h->h_flag[2] = 0;
-  {  // mailbox of the device-resident LM: [0,128) report, [128,144) flag + progress, [256,512) tap values
-    char* mb = nullptr; char* mb_dev = nullptr;
-    if (cudaMalloc(&h->d_pair, sizeof(PairDev)) != cudaSuccess || cudaHostAlloc(&mb, 512, cudaHostAllocMapped) != cudaSuccess ||
-        cudaHostGetDevicePointer((void**)&mb_dev, mb, 0) != cudaSuccess)
-      return bail(fail(B2R_ECUDA, "device allocation failed"));
+  {  // mailbox of the device-resident LM
+    if (h->d_pair.alloc(1) != cudaSuccess || h->mailbox.alloc(512) != cudaSuccess) return fail(B2R_ECUDA, "device allocation failed");
+    char* mb = h->mailbox.p; char* mb_dev = h->mailbox.d;
     std::memset(mb, 0, 512);
     h->h_rep = reinterpret_cast<PairReport*>(mb); h->h_rep_dev = reinterpret_cast<PairReport*>(mb_dev);
     h->h_pflag = reinterpret_cast<unsigned long long*>(mb + 128); h->h_pflag_dev = reinterpret_cast<unsigned long long*>(mb_dev + 128);
     h->h_tap = reinterpret_cast<double*>(mb + 256); h->h_tap_dev = reinterpret_cast<double*>(mb_dev + 256);
   }
-  cudaMemsetAsync(h->d_counter, 0, 4 * sizeof(unsigned int), h->st);
-  if (cudaStreamSynchronize(h->st) != cudaSuccess) return bail(fail(B2R_ECUDA, "initialisation failed"));
+  cudaMemsetAsync(h->d_counter.p, 0, 4 * sizeof(unsigned int), h->st);
+  if (cudaStreamSynchronize(h->st) != cudaSuccess) return fail(B2R_ECUDA, "initialisation failed");
   for (int i = 0; i < 16; i++) h->final_T[i] = (i % 5 == 0) ? 1.f : 0.f;
   h->ndt_work.bc = &h->bc[0];
   h->ndt_work.tel = &h->tel;
   h->vg_work.tel = &h->tel;
   h->vg_work.wide_clusters = cluster16_allowed();
-  *out = h;
+  *out = h.release();
   return B2R_OK;
 }
 
 extern "C" void b2r_batch_destroy(struct b2r_batch* b);
 extern "C" void b2r_destroy(b2r_handle* h) {
   if (!h) return;
-  if (h->loop_batch) { b2r_batch_destroy(h->loop_batch); h->loop_batch = nullptr; }
-  cudaSetDevice(h->cfg.device_id);
-  if (h->st) cudaStreamSynchronize(h->st);
-  if (h->st2) cudaStreamSynchronize(h->st2);
-  h->aux.raw.release(); h->aux.sorted.release(); h->aux.leaf_lo.release(); h->aux.leaf_hi.release(); h->aux.sup_lo.release(); h->aux.sup_hi.release(); h->aux.pos_of.release(); h->aux.cov.release();
-  for (int i = 0; i < 3; i++) {
-    Cloud& c = h->clouds[i];
-    c.raw.release(); c.sorted.release(); c.leaf_lo.release(); c.leaf_hi.release(); c.sup_lo.release(); c.sup_hi.release(); c.pos_of.release(); c.cov.release();
-    ndt_free_map(c.ndt);
-    if (h->staging[i]) cudaFreeHost(h->staging[i]);
-    if (h->staging_ev[i]) cudaEventDestroy(h->staging_ev[i]);
-  }
-  for (int i = 0; i < 2; i++) { h->corr[i].release(); h->cpos[i].release(); h->mahal[i].release(); }
-  h->d2.release(); h->partials.release();
-  h->tmp_f.release(); h->tmp_i.release(); h->tmp_f4.release(); h->bc[0].release(); h->bc[1].release();
-  h->pf_buf[0].release(); h->pf_buf[1].release(); h->pf_flags.release(); h->pf_blocks.release();
-  h->ingest_blob.release(); h->ingest_out.release();
-  if (h->ingest_pinned) cudaFreeHost(h->ingest_pinned);
-  h->map_kf.release(); h->map_keys[0].release(); h->map_keys[1].release();
-  if (h->map_geom) cudaFree(h->map_geom);
-  if (h->map_h) cudaFreeHost(h->map_h);
-  if (h->pf_stats) cudaFree(h->pf_stats);
-  if (h->pf_total) cudaFree(h->pf_total);
-  if (h->pf_h_total) cudaFreeHost(h->pf_h_total);
-  h->ndt_work.release();
-  h->vg_work.release();
-  h->tel.release();
-  if (h->d_out) cudaFree(h->d_out);
-  if (h->d_counter) cudaFree(h->d_counter);
-  if (h->h_out) cudaFreeHost(h->h_out);
-  if (h->h_rep) cudaFreeHost(h->h_rep);
-  if (h->d_pair) cudaFree(h->d_pair);
-  if (h->st) cudaStreamDestroy(h->st);
-  if (h->st2) cudaStreamDestroy(h->st2);
-  if (h->ev_prefetch) cudaEventDestroy(h->ev_prefetch);
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  if (h->ev_join) cudaEventDestroy(h->ev_join);
-  if (h->upload_ev) cudaEventDestroy(h->upload_ev);
+  cudaSetDevice(h->cfg.device_id);  // the members are freed on the handle's device
+  b2r_batch_destroy(h->loop_batch);
+  cudaStreamSynchronize(h->st);
+  cudaStreamSynchronize(h->st2);
   delete h;
 }
 
@@ -327,19 +285,17 @@ static int upload(b2r_handle* h, int which, const void* pts, size_t n, size_t st
         h->upload_pending = true;
         h->tel.h2d += bytes;
       } else {
-        int sidx = which;
-        if (h->staging_cap[sidx] < bytes) {
-          if (h->staging[sidx]) { cudaEventSynchronize(h->staging_ev[sidx]); cudaFreeHost(h->staging[sidx]); h->staging[sidx] = nullptr; }
-          size_t want = bytes + bytes / 4 + 4096;
-          B2R_CUDA(cudaMallocHost(&h->staging[sidx], want));
-          h->staging_cap[sidx] = want;
+        PinnedBuf<char>& stage = h->staging[which];
+        if (stage.cap < bytes) {
+          if (stage.p) cudaEventSynchronize(h->staging_ev[which]);  // the last copy out of the old buffer has finished before it is freed
+          B2R_CUDA(stage.alloc(bytes + bytes / 4 + 4096));
         } else {
-          B2R_CUDA(cudaEventSynchronize(h->staging_ev[sidx]));
+          B2R_CUDA(cudaEventSynchronize(h->staging_ev[which]));
         }
-        std::memcpy(h->staging[sidx], pts, bytes);
-        B2R_CUDA(cudaMemcpyAsync(c.raw.p, h->staging[sidx], bytes, cudaMemcpyHostToDevice, st));
+        std::memcpy(stage.p, pts, bytes);
+        B2R_CUDA(cudaMemcpyAsync(c.raw.p, stage.p, bytes, cudaMemcpyHostToDevice, st));
         h->tel.h2d += bytes;
-        B2R_CUDA(cudaEventRecord(h->staging_ev[sidx], st));
+        B2R_CUDA(cudaEventRecord(h->staging_ev[which], st));
       }
     }
   }
@@ -453,10 +409,10 @@ static int build_bvh(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
   B2R_CUDA(B.sort_tmp.reserve(tmp_bytes + 256));
   TEL_BEGIN(&h->tel, st);
   const unsigned nb = (unsigned)((n + 255) / 256);
-  k_grid_reset<<<1, 32, 0, st>>>(B.mm);
-  k_bbox<<<nb > 1184 ? 1184 : nb, 256, 0, st>>>(c.raw_view, c.stride_f, N, B.mm);
+  k_grid_reset<<<1, 32, 0, st>>>(B.mm.p);
+  k_bbox<<<nb > 1184 ? 1184 : nb, 256, 0, st>>>(c.raw_view, c.stride_f, N, B.mm.p);
   k_fill_i32<<<nb, 256, 0, st>>>(c.pos_of.p, N, -1);
-  k_morton_keys<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, N, B.mm, B.keys_a.p, B.vals_a.p);
+  k_morton_keys<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, N, B.mm.p, B.keys_a.p, B.vals_a.p);
   size_t tb = B.sort_tmp.cap;
   // stable LSD sort over all 32 bits: ties keep ascending index.  Keys are 30-bit Hilbert indices, or 0xffffffff for dropped
   // points, which therefore sort behind every valid key and are recognised by their key afterwards
@@ -808,29 +764,29 @@ static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, co
     // covariances, waits for both.
     B2R_CUDA(cudaEventRecord(h->ev_fork, h->st));  // behind the structure build and whatever the previous align left on the main stream
     B2R_CUDA(cudaStreamWaitEvent(h->st2, h->ev_fork, 0));
-    k_pair_init<<<1, 128, 0, h->st2>>>(P, h->d_pair);
+    k_pair_init<<<1, 128, 0, h->st2>>>(P, h->d_pair.p);
     B2R_CUDA(cudaGetLastError());
     { TEL_BEGIN(&h->tel, h->st2);
-      cudaError_t e = copies == 1 ? launch_search<1>(h->d_pair, nullptr, 1, max_sorted, cfg, h->st2, false)
-                    : copies == 2 ? launch_search<2>(h->d_pair, nullptr, 1, max_sorted, cfg, h->st2, false)
-                                  : launch_search<4>(h->d_pair, nullptr, 1, max_sorted, cfg, h->st2, false);
+      cudaError_t e = copies == 1 ? launch_search<1>(h->d_pair.p, nullptr, 1, max_sorted, cfg, h->st2, false)
+                    : copies == 2 ? launch_search<2>(h->d_pair.p, nullptr, 1, max_sorted, cfg, h->st2, false)
+                                  : launch_search<4>(h->d_pair.p, nullptr, 1, max_sorted, cfg, h->st2, false);
       B2R_CUDA(e);
       TEL_END(&h->tel, KC_GICP_CORR, 1, h->st2); }
     B2R_CUDA(cudaEventRecord(h->ev_join, h->st2));
     int rc0 = ensure_cov(h, s);  // main stream: the k-NN covariance kernel
     if (rc0) return rc0;
     B2R_CUDA(cudaStreamWaitEvent(h->st, h->ev_join, 0));
-    rc0 = launch_round(h->d_pair, nullptr, 1, max_sorted, copies, cfg, h->st, &h->tel, false);  // accumulate + LM step of round 1
+    rc0 = launch_round(h->d_pair.p, nullptr, 1, max_sorted, copies, cfg, h->st, &h->tel, false);  // accumulate + LM step of round 1
     if (rc0) return rc0;
     enq = 1;
     first_batch--;
   } else {
-    k_pair_init<<<1, 128, 0, h->st>>>(P, h->d_pair);
+    k_pair_init<<<1, 128, 0, h->st>>>(P, h->d_pair.p);
     B2R_CUDA(cudaGetLastError());
   }
   auto enqueue = [&](int n) -> int {
     for (int i = 0; i < n; i++) {
-      int rc = launch_round(h->d_pair, nullptr, 1, max_sorted, copies, cfg, h->st, &h->tel, true);
+      int rc = launch_round(h->d_pair.p, nullptr, 1, max_sorted, copies, cfg, h->st, &h->tel, true);
       if (rc) return rc;
       enq++;
     }
@@ -991,15 +947,15 @@ static int fitness_impl(b2r_handle* h, const float* T_row, double max_range, flo
   A.src = s.bvh(); A.tgt = t.bvh();
   for (int i = 0; i < 12; i++) A.Tf[i] = T_row[i];
   A.max_range = max_range; A.inlier_thresh_sq = inl;
-  A.partials = h->partials.p; A.out = h->d_out + 40; A.counter = h->d_counter + 2;
+  A.partials = h->partials.p; A.out = h->d_out.p + 40; A.counter = h->d_counter.p + 2;
   { TEL_BEGIN(&h->tel, h->st);
     k_fitness<<<(unsigned)nb, kLinThreads, 0, h->st>>>(A);
     TEL_END(&h->tel, KC_FITNESS, 1, h->st); }
   h->tel.d2h += 3 * sizeof(double);
   B2R_CUDA(cudaGetLastError());
-  B2R_CUDA(cudaMemcpyAsync(h->h_out + 40, h->d_out + 40, 3 * sizeof(double), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaMemcpyAsync(h->h_out.p + 40, h->d_out.p + 40, 3 * sizeof(double), cudaMemcpyDeviceToHost, h->st));
   B2R_CUDA(cudaStreamSynchronize(h->st));
-  double sum = h->h_out[40], nr = h->h_out[41], ni = h->h_out[42];
+  double sum = h->h_out.p[40], nr = h->h_out.p[41], ni = h->h_out.p[42];
   if (score) *score = nr > 0 ? sum / nr : DBL_MAX;
   if (n_used) *n_used = (uint32_t)nr;
   if (n_inl) *n_inl = (uint32_t)ni;
@@ -1233,11 +1189,10 @@ static int pf_reserve(b2r_handle* h, size_t n, int sf) {
   B2R_CUDA(h->pf_flags.reserve(n + 8));
   B2R_CUDA(h->pf_blocks.reserve((n + kCompactBlock - 1) / kCompactBlock + 8));
   B2R_CUDA(h->tmp_f.reserve(n + 8));
-  if (!h->pf_stats) {
-    B2R_CUDA(cudaMalloc(&h->pf_stats, sizeof(SorStats)));
-    B2R_CUDA(cudaMalloc(&h->pf_total, 4 * sizeof(int)));
-    B2R_CUDA(cudaHostAlloc(&h->pf_h_total, 4 * sizeof(int), cudaHostAllocMapped));
-    B2R_CUDA(cudaHostGetDevicePointer((void**)&h->pf_h_total_dev, h->pf_h_total, 0));
+  if (!h->pf_stats.p) {
+    B2R_CUDA(h->pf_stats.alloc(1));
+    B2R_CUDA(h->pf_total.alloc(4));
+    B2R_CUDA(h->pf_h_total.alloc(4));
   }
   return B2R_OK;
 }
@@ -1248,13 +1203,13 @@ static int pf_compact(b2r_handle* h, const float* d_in, size_t n, int sf, float*
   unsigned char* flags = h->pf_flags.p;
   { TEL_BEGIN(&h->tel, h->st);
     k_compact_count<<<nb, kCompactBlock, 0, h->st>>>(flags, (int)n, h->pf_blocks.p);
-    k_compact_scan<<<1, 1024, 0, h->st>>>(h->pf_blocks.p, (int)nb, h->pf_total, h->pf_h_total_dev);
+    k_compact_scan<<<1, 1024, 0, h->st>>>(h->pf_blocks.p, (int)nb, h->pf_total.p, h->pf_h_total.d);
     k_compact_scatter<<<nb, kCompactBlock, 0, h->st>>>(d_in, sf, flags, (int)n, h->pf_blocks.p, d_out);
     TEL_END(&h->tel, KC_MISC, 3, h->st); }
   B2R_CUDA(cudaGetLastError());
   B2R_CUDA(cudaStreamSynchronize(h->st));
   h->tel.d2h += 4;
-  *m = (size_t)h->pf_h_total[0];
+  *m = (size_t)h->pf_h_total.p[0];
   return B2R_OK;
 }
 
@@ -1302,8 +1257,8 @@ static int pf_radius(b2r_handle* h, const float* d_in, size_t n, int sf, double 
 static int pf_statistical(b2r_handle* h, const float* d_in, size_t n, int sf, int mean_k, double stddev_mul, float* d_out, size_t* m) {
   int rc = pf_knn_stat(h, d_in, n, sf, mean_k + 1, 1);
   if (rc) return rc;
-  k_sor_stats<<<1, kSorThreads, 0, h->st>>>(h->tmp_f.p, (int)n, stddev_mul, h->pf_stats);
-  k_sor_flags<<<(unsigned)((n + 255) / 256), 256, 0, h->st>>>(h->tmp_f.p, (int)n, h->pf_stats, h->pf_flags.p);
+  k_sor_stats<<<1, kSorThreads, 0, h->st>>>(h->tmp_f.p, (int)n, stddev_mul, h->pf_stats.p);
+  k_sor_flags<<<(unsigned)((n + 255) / 256), 256, 0, h->st>>>(h->tmp_f.p, (int)n, h->pf_stats.p, h->pf_flags.p);
   return pf_compact(h, d_in, n, sf, d_out, m);
 }
 
@@ -1552,21 +1507,18 @@ extern "C" int b2r_ingest_pcd(b2r_handle* h, const char* path, const void** d_po
   *d_points = nullptr; *n_points = 0;
   if (n == 0) return B2R_OK;
   const size_t bytes = n * L.point_step;
-  if (h->ingest_pinned_cap < bytes) {  // the file body is read straight into pinned memory: no intermediate PointCloud, no repack
-    if (h->ingest_pinned) cudaFreeHost(h->ingest_pinned);
-    h->ingest_pinned = nullptr; h->ingest_pinned_cap = 0;
-    B2R_CUDA(cudaMallocHost(&h->ingest_pinned, bytes + bytes / 4 + 4096));
-    h->ingest_pinned_cap = bytes + bytes / 4 + 4096;
+  if (h->ingest_pinned.cap < bytes) {  // the file body is read straight into pinned memory: no intermediate PointCloud, no repack
+    B2R_CUDA(h->ingest_pinned.alloc(bytes + bytes / 4 + 4096));
   } else {
     B2R_CUDA(cudaStreamSynchronize(h->st));  // a previous upload from this buffer may still be in flight
   }
   FILE* f = fopen(path, "rb");
   if (!f) return fail(B2R_EINVAL, std::string("cannot open ") + path);
-  bool ok = fseek(f, (long)off, SEEK_SET) == 0 && fread(h->ingest_pinned, 1, bytes, f) == bytes;
+  bool ok = fseek(f, (long)off, SEEK_SET) == 0 && fread(h->ingest_pinned.p, 1, bytes, f) == bytes;
   fclose(f);
   if (!ok) return fail(B2R_EINVAL, "PCD body shorter than its header says");
   B2R_CUDA(h->ingest_blob.reserve(bytes + 16));
-  B2R_CUDA(cudaMemcpyAsync(h->ingest_blob.p, h->ingest_pinned, bytes, cudaMemcpyHostToDevice, h->st));
+  B2R_CUDA(cudaMemcpyAsync(h->ingest_blob.p, h->ingest_pinned.p, bytes, cudaMemcpyHostToDevice, h->st));
   h->tel.h2d += bytes;
   rc = ingest_device(h, reinterpret_cast<const unsigned char*>(h->ingest_blob.p), n, L, d_points);
   if (rc) return rc;
@@ -1594,35 +1546,36 @@ static int map_voxel_centres(b2r_handle* h, const float* cloud, int cloud_sf, si
   B2R_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, tmp_sort, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st));
   B2R_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, flags, slots, (int)total, st));
   B2R_CUDA(h->bc[0].sort_tmp.reserve(std::max(tmp_sort, tmp_scan) + 256));
-  if (!h->map_geom) {
-    B2R_CUDA(cudaMalloc(&h->map_geom, sizeof(MapGeom) + 64));
-    B2R_CUDA(cudaMallocHost(&h->map_h, 64));
+  if (!h->map_geom.p) {
+    B2R_CUDA(h->map_geom.alloc(sizeof(MapGeom) + 64));
+    B2R_CUDA(h->map_h.alloc(16));
   }
-  unsigned long long* first_idx = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(h->map_geom) + sizeof(MapGeom));
+  MapGeom* geom = reinterpret_cast<MapGeom*>(h->map_geom.p);
+  unsigned long long* first_idx = reinterpret_cast<unsigned long long*>(h->map_geom.p + sizeof(MapGeom));
   int* n_dev = reinterpret_cast<int*>(first_idx + 1);
   { TEL_BEGIN(&h->tel, st);
     // replay of the octree's bounding-box growth: each round finds the first point outside the box and grows the box for it; the
     // box settles after ~log2(extent / resolution) rounds, further rounds exit at once (G.done)
-    k_oct_init<<<1, 1, 0, st>>>(h->map_geom, resolution, first_idx);
+    k_oct_init<<<1, 1, 0, st>>>(geom, resolution, first_idx);
     for (int round = 0; round < 48; round++) {
-      k_oct_first_violator<<<nb, 256, 0, st>>>(cloud, cloud_sf, T, h->map_geom, first_idx);
-      k_oct_grow<<<1, 1, 0, st>>>(cloud, cloud_sf, h->map_geom, first_idx);
+      k_oct_first_violator<<<nb, 256, 0, st>>>(cloud, cloud_sf, T, geom, first_idx);
+      k_oct_grow<<<1, 1, 0, st>>>(cloud, cloud_sf, geom, first_idx);
     }
-    k_map_keys<<<nb, 256, 0, st>>>(cloud, cloud_sf, T, h->map_geom, h->map_keys[0].p);
+    k_map_keys<<<nb, 256, 0, st>>>(cloud, cloud_sf, T, geom, h->map_keys[0].p);
     size_t tb = h->bc[0].sort_tmp.cap;
     B2R_CUDA(cub::DeviceRadixSort::SortKeys(h->bc[0].sort_tmp.p, tb, h->map_keys[0].p, h->map_keys[1].p, (int)total, 0, 64, st));
     k_map_heads<<<nb, 256, 0, st>>>(h->map_keys[1].p, T, flags);
     tb = h->bc[0].sort_tmp.cap;
     B2R_CUDA(cub::DeviceScan::ExclusiveSum(h->bc[0].sort_tmp.p, tb, flags, slots, (int)total, st));
-    k_map_centers<<<nb, 256, 0, st>>>(h->map_keys[1].p, flags, slots, T, h->map_geom, out_sf, out, n_dev);
+    k_map_centers<<<nb, 256, 0, st>>>(h->map_keys[1].p, flags, slots, T, geom, out_sf, out, n_dev);
     TEL_END(&h->tel, KC_MISC, 106, st); }
   B2R_CUDA(cudaGetLastError());
-  B2R_CUDA(cudaMemcpyAsync(h->map_h, n_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
-  B2R_CUDA(cudaMemcpyAsync(h->map_h + 1, &h->map_geom->overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(h->map_h.p, n_dev, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(h->map_h.p + 1, &geom->overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2R_CUDA(cudaStreamSynchronize(st));
   // the octree keys hold 21 bits per axis: a deeper box leaves every point uninserted, which must not pass for an empty map
-  if (h->map_h[1]) return fail(B2R_EUNSUPPORTED, "map extent needs more than 21 octree levels at this resolution");
-  *m = (size_t)h->map_h[0];
+  if (h->map_h.p[1]) return fail(B2R_EUNSUPPORTED, "map extent needs more than 21 octree levels at this resolution");
+  *m = (size_t)h->map_h.p[0];
   return B2R_OK;
 }
 
@@ -1715,7 +1668,7 @@ struct b2r_odometry {
   // Each slot's `in` holds a host cloud's upload, its `out` the filtered records.
   VoxelWork vw[2];
   int cur = 0;
-  cudaEvent_t ev_free = nullptr;
+  Event ev_free;
   int device_id = 0;
   // the prefetched frame: identity of the announced RAW cloud, and its filtered copy as handed to b2r_prefetch_source_device
   bool pf_valid = false;
@@ -1783,7 +1736,7 @@ extern "C" int b2r_odometry_create(b2r_handle* reg, const b2r_odometry_params* p
     return fail(B2R_EINVAL, "downsample_resolution must be positive");
   if (p && p->downsample_method == B2R_DOWNSAMPLE_APPROX_VOXELGRID && !(p->downsample_resolution > 0.f && std::isfinite(p->downsample_resolution)))
     return fail(B2R_EINVAL, "downsample_resolution must be finite and positive");
-  b2r_odometry* o = new b2r_odometry();
+  std::unique_ptr<b2r_odometry> o(new b2r_odometry());
   o->reg = reg;
   if (p) o->p = *p;
   else {  // and downsample_method NONE
@@ -1792,24 +1745,18 @@ extern "C" int b2r_odometry_create(b2r_handle* reg, const b2r_odometry_params* p
   }
   o->device_id = reg->cfg.device_id;
   if (odometry_downsamples(o->p)) {
-    if (cudaSetDevice(o->device_id) != cudaSuccess || cudaEventCreateWithFlags(&o->ev_free, cudaEventDisableTiming) != cudaSuccess) {
-      delete o;
-      return fail(B2R_ECUDA, "cudaEventCreate failed");
-    }
+    if (cudaSetDevice(o->device_id) != cudaSuccess || o->ev_free.create() != cudaSuccess) return fail(B2R_ECUDA, "cudaEventCreate failed");
     for (VoxelWork& W : o->vw) { W.tel = &reg->tel; W.wide_clusters = cluster16_allowed(); }
   }
   mat4_identity(o->prev_trans);
   mat4_identity(o->keyframe_pose);
-  *out = o;
+  *out = o.release();
   return B2R_OK;
 }
 extern "C" void b2r_odometry_destroy(b2r_odometry* o) {
   if (!o) return;
-  if (o->ev_free) {
-    cudaSetDevice(o->device_id);
-    o->vw[0].release(); o->vw[1].release();  // (cudaFree waits for kernels still reading them, e.g. an unadopted prefetch)
-    cudaEventDestroy(o->ev_free);
-  }
+  // the voxel-grid slots are freed on their device (cudaFree waits for kernels still reading them, e.g. an unadopted prefetch)
+  if (o->ev_free) cudaSetDevice(o->device_id);
   delete o;
 }
 

@@ -136,13 +136,13 @@ inline int approx_voxelgrid_device(VoxelWork& W, cudaStream_t st, const float* d
   k_avg_runs<<<nb, kAvgBlock, 0, st>>>(d_in, sf, N, inv_leaf, W.keys_b.p, W.vals_b.p, heads, W.flags.p, W.buckets.p);
   tb = W.tmp.cap;
   B2R_CUDA(cub::DeviceScan::ExclusiveSum(W.tmp.p, tb, W.flags.p, W.slots.p, N, st));
-  k_avg_rank<<<1, kAvgSlots, 0, st>>>(W.buckets.p, W.flags.p, W.slots.p, N, W.mm + 6);
+  k_avg_rank<<<1, kAvgSlots, 0, st>>>(W.buckets.p, W.flags.p, W.slots.p, N, W.mm.p + 6);
   k_avg_centroid<<<nb, kAvgBlock, 0, st>>>(d_in, sf, N, W.keys_b.p, W.vals_b.p, heads, W.slots.p, W.buckets.p, W.out.p, W.ocounts.p);
   TEL_END(W.tel, KC_VOXELGRID, 9, st);
   B2R_CUDA(cudaGetLastError());
-  B2R_CUDA(cudaMemcpyAsync(W.h_total, W.mm + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(W.h_total.p, W.mm.p + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2R_CUDA(cudaStreamSynchronize(st));
-  *m = (size_t)W.h_total[0];
+  *m = (size_t)W.h_total.p[0];
   return B2R_OK;
 }
 

@@ -15,15 +15,17 @@
 #include <chrono>
 
 struct b2r_batch {
-  b2r_handle* eng = nullptr;  // engine context of this device: config, main stream, telemetry
+  struct EngineDeleter { void operator()(b2r_handle* h) const { b2r_destroy(h); } };
+  // engine context of this device: config, main stream, telemetry.  Declared first: destroyed after everything below
+  std::unique_ptr<b2r_handle, EngineDeleter> eng;
   static constexpr int kBuildStreams = 4;
-  cudaStream_t bst[kBuildStreams] = {nullptr, nullptr, nullptr, nullptr};
+  Stream bst[kBuildStreams];
   BuildCtx bctx[kBuildStreams];
-  cudaEvent_t bev[kBuildStreams] = {nullptr, nullptr, nullptr, nullptr};
+  Event bev[kBuildStreams];
   int next_stream = 0;
-  std::vector<Cloud*> clouds;
+  std::vector<std::unique_ptr<Cloud>> clouds;
   std::vector<int> free_ids;
-  std::vector<Cloud*> recycled;  // removed clouds keep their device buffers for the next add (no cudaMalloc churn per keyframe)
+  std::vector<std::unique_ptr<Cloud>> recycled;  // removed clouds keep their device buffers for the next add (no cudaMalloc churn per keyframe)
   // pair slots.  A chunk of pairs can be split over kLanes independent round sequences ("lanes"), each on its own stream, so that a
   // lane's search kernel (instruction-issue bound) runs beside the other lane's accumulate kernel and a lane's thin tail rounds
   // overlap the other's fat ones.  Two lanes did not beat one on 256 pairs x 64k points — the block
@@ -31,8 +33,9 @@ struct b2r_batch {
   // is ONE lane (B2R_BATCH_LANES=2 enables the second).  Lane 0 runs on the engine's main stream.
   static constexpr int kLanes = 2;
   struct Lane {
-    cudaStream_t st = nullptr;
-    cudaEvent_t ev = nullptr;
+    cudaStream_t st = nullptr;  // lane 0: the engine's main stream; the others: `own`
+    Stream own;
+    Event ev;
     DevBuf<PairDev> d_pairs;
     DevBuf<int> d_active;
     unsigned long long* h_word = nullptr;  // host-mapped: (seq << 32) | pairs still active
@@ -40,15 +43,13 @@ struct b2r_batch {
     unsigned long long seq = 0;
   };
   Lane lane[kLanes];
-  cudaEvent_t fork_ev = nullptr;
+  Event fork_ev;
   int n_lanes = 1;
   DevBuf<PairReport> d_reports;
   DevBuf<char> ws;
-  PairDev* h_pairs = nullptr;       // pinned staging
-  PairReport* h_reports = nullptr;  // pinned staging
-  size_t h_cap = 0;
-  unsigned long long* h_word = nullptr;  // host-mapped: [0..kLanes) = the lanes' words, [kLanes] = sum of the pairs' executed rounds
-  unsigned long long* h_word_dev = nullptr;
+  PinnedBuf<PairDev> h_pairs;       // staging
+  PinnedBuf<PairReport> h_reports;  // staging
+  MappedBuf<unsigned long long> h_word;  // [0..kLanes) = the lanes' words, [kLanes] = sum of the pairs' executed rounds
   size_t max_chunk = 1024;  // pairs in flight per launch sequence (~7.7 MB of workspace per 64k-point pair)
   int copies = 1;           // lanes per query of the batched 1-NN search
   // multi-GPU
@@ -56,25 +57,27 @@ struct b2r_batch {
   int rank = 0, world = 1;
   DevBuf<b2r_result> d_send, d_recv;
   DevBuf<BuildItem> d_build;        // descriptor list of the batched cluster builds
-  BuildItem* h_build = nullptr;     // pinned staging
-  size_t h_build_cap = 0;
+  PinnedBuf<BuildItem> h_build;     // staging
   DevBuf<KnnBatchItem> d_knn;       // descriptor list of one batched k-NN covariance launch
-  KnnBatchItem* h_knn = nullptr;    // pinned staging
-  size_t h_knn_cap = 0;
-  b2r_result* h_gather = nullptr;
-  size_t h_gather_cap = 0;
+  PinnedBuf<KnnBatchItem> h_knn;    // staging
+  PinnedBuf<b2r_result> h_gather;
   // NDT batch (batch_run_ndt_chunk)
   DevBuf<char> ndt_ws;              // per pair in flight: chunk rows, group rows, counters, ticket counter; fitness partials
   DevBuf<NdtArgs> d_ndt_args;       // the round's pass records, grouped by pass kind
-  NdtArgs* h_ndt_args = nullptr;    // pinned staging
-  size_t h_ndt_cap = 0;
-  double* h_ndt_msg = nullptr;      // host-mapped: one result message per record of the round, then the round's flag
-  double* h_ndt_msg_dev = nullptr;
-  size_t ndt_msg_cap = 0;
-  unsigned int* d_ndt_round = nullptr;  // messages of the current round (the last one publishes the flag and re-arms it)
+  PinnedBuf<NdtArgs> h_ndt_args;    // staging
+  MappedBuf<double> h_ndt_msg;      // one result message per record of the round, then the round's flag (8 doubles)
+  DevBuf<unsigned int> d_ndt_round; // messages of the current round (the last one publishes the flag and re-arms it)
   unsigned long long ndt_seq = 0;
   // telemetry of the last b2r_batch_align
   unsigned long long last_rounds = 0, last_pair_rounds = 0;
+  ~b2r_batch() {  // what is not a plain free; the members then go in reverse order, the engine last
+    if (!eng) return;
+    cudaSetDevice(eng->cfg.device_id);
+    cudaStreamSynchronize(eng->st);
+    for (const Stream& s : bst) if (s) cudaStreamSynchronize(s);
+    for (const Lane& L : lane) if (L.st) cudaStreamSynchronize(L.st);
+    if (comm) ncclCommDestroy(comm);  // before the send / receive buffers go
+  }
 };
 
 #define B2R_NCCL(expr)                                                                                     \
@@ -83,84 +86,44 @@ struct b2r_batch {
     if (_r != ncclSuccess) return b2r::fail(B2R_ENCCL, std::string(#expr) + ": " + ncclGetErrorString(_r)); \
   } while (0)
 
-static void free_cloud(Cloud* c) {
-  if (!c) return;
-  c->raw.release(); c->sorted.release(); c->leaf_lo.release(); c->leaf_hi.release(); c->sup_lo.release(); c->sup_hi.release(); c->pos_of.release(); c->cov.release();
-  ndt_free_map(c->ndt);
-  delete c;
-}
-
-extern "C" void b2r_batch_destroy(b2r_batch* b) {
-  if (!b) return;
-  if (b->eng) cudaSetDevice(b->eng->cfg.device_id);
-  if (b->eng && b->eng->st) cudaStreamSynchronize(b->eng->st);
-  for (int i = 0; i < b2r_batch::kBuildStreams; i++) {
-    if (b->bst[i]) { cudaStreamSynchronize(b->bst[i]); cudaStreamDestroy(b->bst[i]); }
-    if (b->bev[i]) cudaEventDestroy(b->bev[i]);
-    b->bctx[i].release();
-  }
-  if (b->comm) ncclCommDestroy(b->comm);
-  for (Cloud* c : b->clouds) free_cloud(c);
-  for (Cloud* c : b->recycled) free_cloud(c);
-  for (int l = 0; l < b2r_batch::kLanes; l++) {
-    b2r_batch::Lane& L = b->lane[l];
-    if (l > 0 && L.st) { cudaStreamSynchronize(L.st); cudaStreamDestroy(L.st); }
-    if (L.ev) cudaEventDestroy(L.ev);
-    L.d_pairs.release(); L.d_active.release();
-  }
-  if (b->fork_ev) cudaEventDestroy(b->fork_ev);
-  b->d_reports.release(); b->ws.release(); b->d_send.release(); b->d_recv.release();
-  if (b->h_pairs) cudaFreeHost(b->h_pairs);
-  if (b->h_reports) cudaFreeHost(b->h_reports);
-  if (b->h_word) cudaFreeHost(b->h_word);
-  if (b->h_gather) cudaFreeHost(b->h_gather);
-  if (b->h_knn) cudaFreeHost(b->h_knn);
-  if (b->h_build) cudaFreeHost(b->h_build);
-  b->d_knn.release(); b->d_build.release();
-  b->ndt_ws.release(); b->d_ndt_args.release();
-  if (b->h_ndt_args) cudaFreeHost(b->h_ndt_args);
-  if (b->h_ndt_msg) cudaFreeHost(b->h_ndt_msg);
-  if (b->d_ndt_round) cudaFree(b->d_ndt_round);
-  if (b->eng) b2r_destroy(b->eng);
-  delete b;
-}
+extern "C" void b2r_batch_destroy(b2r_batch* b) { delete b; }
 
 extern "C" int b2r_batch_create(const b2r_config* cfg, b2r_batch** out) {
   if (!cfg || !out) return fail(B2R_EINVAL, "NULL argument");
   *out = nullptr;
   if (cfg->method != B2R_METHOD_GICP && cfg->method != B2R_METHOD_NDT) return fail(B2R_EINVAL, "unknown method");
-  b2r_batch* b = new b2r_batch();
-  int rc = b2r_create(cfg, &b->eng);
-  if (rc) { delete b; return rc; }
-  auto bail = [&](int code) { b2r_batch_destroy(b); return code; };
+  std::unique_ptr<b2r_batch> b(new b2r_batch());
+  b2r_handle* eng = nullptr;
+  int rc = b2r_create(cfg, &eng);
+  if (rc) return rc;
+  b->eng.reset(eng);
   for (int i = 0; i < b2r_batch::kBuildStreams; i++) {
-    if (cudaStreamCreateWithFlags(&b->bst[i], cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&b->bev[i], cudaEventDisableTiming) != cudaSuccess ||
-        cudaMalloc(&b->bctx[i].mm, 8 * sizeof(int)) != cudaSuccess)
-      return bail(fail(B2R_ECUDA, "stream / scratch creation failed"));
+    if (b->bst[i].create(cudaStreamNonBlocking) != cudaSuccess || b->bev[i].create() != cudaSuccess || b->bctx[i].mm.alloc(8) != cudaSuccess)
+      return fail(B2R_ECUDA, "stream / scratch creation failed");
   }
-  if (cudaHostAlloc(&b->h_word, 64, cudaHostAllocMapped) != cudaSuccess || cudaHostGetDevicePointer((void**)&b->h_word_dev, b->h_word, 0) != cudaSuccess)
-    return bail(fail(B2R_ECUDA, "host allocation failed"));
-  for (int i = 0; i < 8; i++) b->h_word[i] = 0;
-  if (cudaEventCreateWithFlags(&b->fork_ev, cudaEventDisableTiming) != cudaSuccess) return bail(fail(B2R_ECUDA, "event creation failed"));
-  if (cudaMalloc(&b->d_ndt_round, sizeof(unsigned int)) != cudaSuccess || cudaMemset(b->d_ndt_round, 0, sizeof(unsigned int)) != cudaSuccess)
-    return bail(fail(B2R_ECUDA, "device allocation failed"));
+  if (b->h_word.alloc(8) != cudaSuccess) return fail(B2R_ECUDA, "host allocation failed");
+  for (int i = 0; i < 8; i++) b->h_word.p[i] = 0;
+  if (b->fork_ev.create() != cudaSuccess) return fail(B2R_ECUDA, "event creation failed");
+  if (b->d_ndt_round.alloc(1) != cudaSuccess || cudaMemset(b->d_ndt_round.p, 0, sizeof(unsigned int)) != cudaSuccess)
+    return fail(B2R_ECUDA, "device allocation failed");
   for (int l = 0; l < b2r_batch::kLanes; l++) {
     b2r_batch::Lane& L = b->lane[l];
-    L.h_word = b->h_word + l; L.h_word_dev = b->h_word_dev + l;
+    L.h_word = b->h_word.p + l; L.h_word_dev = b->h_word.d + l;
     if (l == 0) L.st = b->eng->st;
-    else if (cudaStreamCreateWithFlags(&L.st, cudaStreamNonBlocking) != cudaSuccess) return bail(fail(B2R_ECUDA, "stream creation failed"));
-    if (cudaEventCreateWithFlags(&L.ev, cudaEventDisableTiming) != cudaSuccess) return bail(fail(B2R_ECUDA, "event creation failed"));
+    else if (L.own.create(cudaStreamNonBlocking) != cudaSuccess) return fail(B2R_ECUDA, "stream creation failed");
+    else L.st = L.own;
+    if (L.ev.create() != cudaSuccess) return fail(B2R_ECUDA, "event creation failed");
   }
   if (const char* e = getenv("B2R_BATCH_LANES")) { const int c = atoi(e); if (c >= 1 && c <= b2r_batch::kLanes) b->n_lanes = c; }
   if (const char* e = getenv("B2R_BATCH_COPIES")) { const int c = atoi(e); if (c == 1 || c == 2 || c == 4) b->copies = c; }
   if (const char* e = getenv("B2R_BATCH_CHUNK")) { const long c = atol(e); if (c > 0) b->max_chunk = (size_t)c; }
-  *out = b;
+  *out = b.release();
   return B2R_OK;
 }
 
 extern "C" int b2r_batch_get_engine(b2r_batch* b, b2r_handle** out) {
   if (!b || !out) return fail(B2R_EINVAL, "NULL argument");
-  *out = b->eng;
+  *out = b->eng.get();
   return B2R_OK;
 }
 
@@ -170,9 +133,9 @@ static int batch_add(b2r_batch* b, const void* pts, size_t n, size_t stride_byte
   if (n > 0 && !pts) return fail(B2R_EINVAL, "points is NULL");
   if (n > (size_t)0x3fffffff) return fail(B2R_EINVAL, "too many points");
   B2R_CUDA(cudaSetDevice(b->eng->cfg.device_id));
-  Cloud* c;
-  if (!b->recycled.empty()) { c = b->recycled.back(); b->recycled.pop_back(); c->invalidate(); }
-  else c = new Cloud();
+  std::unique_ptr<Cloud> c;
+  if (!b->recycled.empty()) { c = std::move(b->recycled.back()); b->recycled.pop_back(); c->invalidate(); }
+  else c.reset(new Cloud());
   c->n = n;
   c->stride_f = (int)(stride_bytes / 4);
   c->host_ptr = pts;
@@ -183,20 +146,20 @@ static int batch_add(b2r_batch* b, const void* pts, size_t n, size_t stride_byte
     c->raw_view = (const float*)pts;
   } else {
     cudaError_t e = c->raw.reserve(n * c->stride_f + 4);
-    if (e != cudaSuccess) { free_cloud(c); return fail(B2R_ECUDA, std::string("device allocation failed: ") + cudaGetErrorString(e)); }
+    if (e != cudaSuccess) return fail(B2R_ECUDA, std::string("device allocation failed: ") + cudaGetErrorString(e));
     c->raw_view = c->raw.p;
     if (n) {
       // pinned buffers are DMA'd in place (asynchronously: see b200reg.h for the lifetime rule); pageable ones are staged by the driver
       e = cudaMemcpyAsync(c->raw.p, pts, n * stride_bytes, cudaMemcpyHostToDevice, st);
-      if (e != cudaSuccess) { free_cloud(c); return fail(B2R_ECUDA, std::string("upload failed: ") + cudaGetErrorString(e)); }
+      if (e != cudaSuccess) return fail(B2R_ECUDA, std::string("upload failed: ") + cudaGetErrorString(e));
       b->eng->tel.h2d += n * stride_bytes;
     }
   }
   // the upload is all that happens here (4 copy streams); the search structures and k-NN covariances of ALL new clouds are built
   // together at the next align: one cluster-build launch per cluster size and one k-NN launch (batch_build_structures)
   int id;
-  if (!b->free_ids.empty()) { id = b->free_ids.back(); b->free_ids.pop_back(); b->clouds[id] = c; }
-  else { id = (int)b->clouds.size(); b->clouds.push_back(c); }
+  if (!b->free_ids.empty()) { id = b->free_ids.back(); b->free_ids.pop_back(); b->clouds[id] = std::move(c); }
+  else { id = (int)b->clouds.size(); b->clouds.push_back(std::move(c)); }
   *id_out = id;
   return B2R_OK;
 }
@@ -228,8 +191,7 @@ extern "C" int b2r_batch_remove_cloud(b2r_batch* b, int32_t id) {
   if (id < 0 || (size_t)id >= b->clouds.size() || !b->clouds[id]) return fail(B2R_EINVAL, "unknown cloud id");
   int rc = b2r_batch_synchronize(b);  // nothing in flight may still read it
   if (rc) return rc;
-  b->recycled.push_back(b->clouds[id]);
-  b->clouds[id] = nullptr;
+  b->recycled.push_back(std::move(b->clouds[id]));
   b->free_ids.push_back(id);
   return B2R_OK;
 }
@@ -243,13 +205,13 @@ extern "C" int b2r_batch_cloud_count(const b2r_batch* b) {
 // any order, repeats allowed) that does not have them yet: one cluster-build launch per cluster size and one k-NN launch for all of
 // them (what setInputSource / setInputTarget make the reference pay per call: kd-tree build + covariances, loop_detector.hpp:122,136)
 static int batch_build_structures(b2r_batch* b, const int32_t* ids, size_t n_ids, bool need_cov) {
-  b2r_handle* h = b->eng;
+  b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
   std::vector<Cloud*> todo;
   std::vector<char> queued(b->clouds.size(), 0);
   for (size_t i = 0; i < n_ids; i++) {
     const int32_t id = ids[i];
-    Cloud* c = b->clouds[id];
+    Cloud* c = b->clouds[id].get();
     if (queued[id] || c->n == 0 || (c->bvh_ready && (c->cov_ready || !need_cov))) continue;
     queued[id] = 1;
     todo.push_back(c);
@@ -269,16 +231,11 @@ static int batch_build_structures(b2r_batch* b, const int32_t* ids, size_t n_ids
     }
     if (total) {
       B2R_CUDA(b->d_build.reserve(total));
-      if (b->h_build_cap < total) {
-        if (b->h_build) cudaFreeHost(b->h_build);
-        b->h_build = nullptr; b->h_build_cap = 0;
-        B2R_CUDA(cudaMallocHost(&b->h_build, (total + 64) * sizeof(BuildItem)));
-        b->h_build_cap = total + 64;
-      }
+      if (b->h_build.cap < total) B2R_CUDA(b->h_build.alloc(total + 64));
       size_t k0 = 0;
       for (int g = 0; g < kBuildShapes; g++)
-        for (Cloud* c : by_cl[g]) b->h_build[k0++] = build_item(*c);
-      B2R_CUDA(cudaMemcpyAsync(b->d_build.p, b->h_build, total * sizeof(BuildItem), cudaMemcpyHostToDevice, st));
+        for (Cloud* c : by_cl[g]) b->h_build.p[k0++] = build_item(*c);
+      B2R_CUDA(cudaMemcpyAsync(b->d_build.p, b->h_build.p, total * sizeof(BuildItem), cudaMemcpyHostToDevice, st));
       k0 = 0;
       for (int g = 0; g < kBuildShapes; g++) {
         if (by_cl[g].empty()) continue;
@@ -304,20 +261,15 @@ static int batch_build_structures(b2r_batch* b, const int32_t* ids, size_t n_ids
     return B2R_OK;
   }
   B2R_CUDA(b->d_knn.reserve(todo.size()));
-  if (b->h_knn_cap < todo.size()) {
-    if (b->h_knn) cudaFreeHost(b->h_knn);
-    b->h_knn = nullptr; b->h_knn_cap = 0;
-    B2R_CUDA(cudaMallocHost(&b->h_knn, (todo.size() + 64) * sizeof(KnnBatchItem)));
-    b->h_knn_cap = todo.size() + 64;
-  }
+  if (b->h_knn.cap < todo.size()) B2R_CUDA(b->h_knn.alloc(todo.size() + 64));
   unsigned max_blocks = 0;
   for (size_t i = 0; i < todo.size(); i++) {
     Cloud* c = todo[i];
-    KnnBatchItem& it = b->h_knn[i];
+    KnnBatchItem& it = b->h_knn.p[i];
     it.b = c->bvh(); it.raw = c->raw_view; it.cov = c->cov.p; it.stride_f = c->stride_f; it.pad = 0;
     max_blocks = std::max(max_blocks, (unsigned)((size_t)c->nsup * 1024 / kKnnThreads));
   }
-  B2R_CUDA(cudaMemcpyAsync(b->d_knn.p, b->h_knn, todo.size() * sizeof(KnnBatchItem), cudaMemcpyHostToDevice, st));
+  B2R_CUDA(cudaMemcpyAsync(b->d_knn.p, b->h_knn.p, todo.size() * sizeof(KnnBatchItem), cudaMemcpyHostToDevice, st));
   { TEL_BEGIN(&h->tel, st);
     k_knn_cov_reg_batch<kKnnRegK><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
     TEL_END(&h->tel, KC_KNN_COV, 1, st); }
@@ -349,14 +301,10 @@ static void degenerate_report(PairReport& r, const float* guess_col) {
 }
 
 static int batch_host_staging(b2r_batch* b, size_t n) {
-  if (b->h_cap >= n) return B2R_OK;
+  if (b->h_pairs.cap >= n && b->h_reports.cap >= n) return B2R_OK;
   const size_t want = n + n / 4 + 16;
-  if (b->h_pairs) cudaFreeHost(b->h_pairs);
-  if (b->h_reports) cudaFreeHost(b->h_reports);
-  b->h_pairs = nullptr; b->h_reports = nullptr; b->h_cap = 0;
-  B2R_CUDA(cudaMallocHost(&b->h_pairs, want * sizeof(PairDev)));
-  B2R_CUDA(cudaMallocHost(&b->h_reports, want * sizeof(PairReport)));
-  b->h_cap = want;
+  B2R_CUDA(b->h_pairs.alloc(want));
+  B2R_CUDA(b->h_reports.alloc(want));
   return B2R_OK;
 }
 
@@ -381,7 +329,7 @@ static int wait_word(const b2r_batch::Lane& L, unsigned long long need_seq, size
 // One chunk: pairs[0..m) -> d_rep[0..m) (device).  Every pair of the chunk is in flight at once, split over the lanes; a lane's
 // rounds cover all of its pairs.
 static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const LmCfg& cfg, PairReport* d_rep, bool fit_only) {
-  b2r_handle* h = b->eng;
+  b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
   // per-launch kernel timing (b2r_set_profiling) wants every kernel alone on the device; tiny chunks are not worth a second stream
   const int n_lanes = (h->tel.on || m < 16) ? 1 : b->n_lanes;
@@ -410,14 +358,14 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
     B2R_CUDA(L.d_pairs.reserve(R.m));
     B2R_CUDA(L.d_active.reserve(R.m + 1));
     for (size_t i = R.i0; i < R.i0 + R.m; i++) {
-      PairDev& P = b->h_pairs[i];
+      PairDev& P = b->h_pairs.p[i];
       const Cloud& s = *b->clouds[pairs[i].source];
       const Cloud& t = *b->clouds[pairs[i].target];
       if (s.n == 0 || t.n == 0) {
         std::memset(&P, 0, sizeof(P));
         P.mode = PM_DONE;
-        degenerate_report(b->h_reports[i], pairs[i].guess);
-        B2R_CUDA(cudaMemcpyAsync(d_rep + i, &b->h_reports[i], sizeof(PairReport), cudaMemcpyHostToDevice, L.st));
+        degenerate_report(b->h_reports.p[i], pairs[i].guess);
+        B2R_CUDA(cudaMemcpyAsync(d_rep + i, &b->h_reports.p[i], sizeof(PairReport), cudaMemcpyHostToDevice, L.st));
         continue;
       }
       fill_pair_geometry(P, s, t);
@@ -437,7 +385,7 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
       R.known++;
       if (n_pad > R.max_pad) R.max_pad = n_pad;
     }
-    B2R_CUDA(cudaMemcpyAsync(L.d_pairs.p, b->h_pairs + R.i0, R.m * sizeof(PairDev), cudaMemcpyHostToDevice, L.st));
+    B2R_CUDA(cudaMemcpyAsync(L.d_pairs.p, b->h_pairs.p + R.i0, R.m * sizeof(PairDev), cudaMemcpyHostToDevice, L.st));
     h->tel.h2d += R.m * sizeof(PairDev);
     k_pair_compact<<<1, 1024, 0, L.st>>>(L.d_pairs.p, (int)R.m, L.d_active.p, L.h_word_dev, ++L.seq);
     B2R_CUDA(cudaGetLastError());
@@ -487,7 +435,7 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
 // Voxel maps of the clouds a call names: every align target, and every cloud added from device memory (its records are the
 // caller's only until this call returns, so the map is built now even if the cloud is a target only later).
 static int batch_ndt_maps(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool fit_only) {
-  b2r_handle* h = b->eng;
+  b2r_handle* h = b->eng.get();
   for (size_t i = 0; i < n_pairs; i++) {
     for (int side = 0; side < 2; side++) {
       Cloud& c = *b->clouds[side ? pairs[i].target : pairs[i].source];
@@ -520,7 +468,7 @@ static NdtPairWs ndt_pair_ws(const Cloud& s) {
 // each active pair asks for into at most three launches (derivatives with Hessian, without, float64 Hessian only), waits once for
 // the round's flag and hands every pair its result.  A pair reduces through its own rows and counters, exactly as alone.
 static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, double fit_max_range, PairReport* rep) {
-  b2r_handle* h = b->eng;
+  b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
   const b2r_config& cfg = h->cfg;
   std::vector<NdtPairState> S(m);
@@ -546,22 +494,14 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
   char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->ndt_ws.p), 256));
   B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
   B2R_CUDA(b->d_ndt_args.reserve(m));
-  if (b->h_ndt_cap < m) {
-    if (b->h_ndt_args) cudaFreeHost(b->h_ndt_args);
-    b->h_ndt_args = nullptr; b->h_ndt_cap = 0;
-    B2R_CUDA(cudaMallocHost(&b->h_ndt_args, m * sizeof(NdtArgs)));
-    b->h_ndt_cap = m;
+  B2R_CUDA(b->h_ndt_args.alloc(m));
+  if (b->h_ndt_msg.cap < m * kNdtMsg + 8) {
+    B2R_CUDA(b->h_ndt_msg.alloc(m * kNdtMsg + 8));
+    std::memset(b->h_ndt_msg.p, 0, b->h_ndt_msg.cap * sizeof(double));
   }
-  if (b->ndt_msg_cap < m) {
-    if (b->h_ndt_msg) cudaFreeHost(b->h_ndt_msg);
-    b->h_ndt_msg = nullptr; b->ndt_msg_cap = 0;
-    B2R_CUDA(cudaHostAlloc(&b->h_ndt_msg, (m * kNdtMsg + 8) * sizeof(double), cudaHostAllocMapped));
-    B2R_CUDA(cudaHostGetDevicePointer((void**)&b->h_ndt_msg_dev, b->h_ndt_msg, 0));
-    std::memset(b->h_ndt_msg, 0, (m * kNdtMsg + 8) * sizeof(double));
-    b->ndt_msg_cap = m;
-  }
-  unsigned long long* flag = reinterpret_cast<unsigned long long*>(b->h_ndt_msg + b->ndt_msg_cap * kNdtMsg);
-  unsigned long long* flag_dev = reinterpret_cast<unsigned long long*>(b->h_ndt_msg_dev + b->ndt_msg_cap * kNdtMsg);
+  const size_t flag_at = b->h_ndt_msg.cap - 8;  // behind the last message the buffer holds
+  unsigned long long* flag = reinterpret_cast<unsigned long long*>(b->h_ndt_msg.p + flag_at);
+  unsigned long long* flag_dev = reinterpret_cast<unsigned long long*>(b->h_ndt_msg.d + flag_at);
   std::vector<unsigned long long> qnext(m, 0);
   std::vector<size_t> order;
   std::vector<int> kind_of;
@@ -587,7 +527,7 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       const int k = kind_of[r];
       Cloud& s = *b->clouds[pairs[i].source];
       Cloud& t = *b->clouds[pairs[i].target];
-      NdtArgs& A = b->h_ndt_args[r];
+      NdtArgs& A = b->h_ndt_args.p[r];
       ndt_fill_args(cfg, s, t, S[i].K, S[i].Tfinal, k != NDT_PASS_DERIV, A);
       const NdtPairWs w = ndt_pair_ws(s);
       char* p = base + off[i];
@@ -599,13 +539,13 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       A.queue = reinterpret_cast<unsigned long long*>(p + w.small + 24);
       A.qbase = qnext[i];
       if (k != NDT_PASS_HESS) qnext[i] += (unsigned long long)(s.nsup * 1024 / kNdtThreads) + G[k];  // chunks + one closing draw per block
-      A.out = b->h_ndt_msg_dev + r * kNdtMsg;
+      A.out = b->h_ndt_msg.d + r * kNdtMsg;
       A.flag = flag_dev;
       A.seq = seq;
-      A.round = b->d_ndt_round;
+      A.round = b->d_ndt_round.p;
       A.round_n = (unsigned)order.size();
     }
-    B2R_CUDA(cudaMemcpyAsync(b->d_ndt_args.p, b->h_ndt_args, order.size() * sizeof(NdtArgs), cudaMemcpyHostToDevice, st));
+    B2R_CUDA(cudaMemcpyAsync(b->d_ndt_args.p, b->h_ndt_args.p, order.size() * sizeof(NdtArgs), cudaMemcpyHostToDevice, st));
     h->tel.h2d += order.size() * sizeof(NdtArgs);
     size_t r0 = 0;
     for (int k = 0; k < 3; k++) {
@@ -623,7 +563,7 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
     b->last_rounds++;
     for (size_t r = 0; r < order.size(); r++) {  // the first wait covers the round; the rest only check each message
       const int k = kind_of[r];
-      const double* msg = b->h_ndt_msg + r * kNdtMsg;
+      const double* msg = b->h_ndt_msg.p + r * kNdtMsg;
       int rc = (k == NDT_PASS_HESS) ? wait_host_result(flag, seq, msg, 36, false, st) : wait_host_result(flag, seq, msg, kNdtAcc, true, st);
       if (rc) return rc;
       NdtPass P;
@@ -685,7 +625,7 @@ __global__ void k_pack_results(const PairReport* rep, int n, b2r_result* out, in
 
 // pairs[0..n) -> d_reports[0..n) on the device (no host copy of the results)
 static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool want_fitness, double fit_max_range, bool fit_only = false) {
-  b2r_handle* h = b->eng;
+  b2r_handle* h = b->eng.get();
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   for (size_t i = 0; i < n_pairs; i++) {
     const b2r_pair& pr = pairs[i];
@@ -714,12 +654,12 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   for (size_t c0 = 0; c0 < n_pairs; c0 += chunk) {
     const size_t m = std::min(chunk, n_pairs - c0);
     // an NDT align runs its own rounds; a stand-alone fitness evaluation is the same search on either engine
-    if (ndt && !fit_only) rc = batch_run_ndt_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports + c0);
+    if (ndt && !fit_only) rc = batch_run_ndt_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
     else rc = batch_run_chunk(b, pairs + c0, m, cfg, b->d_reports.p + c0, fit_only);
     if (rc) return rc;
   }
   if (ndt && !fit_only)  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
-    B2R_CUDA(cudaMemcpyAsync(b->d_reports.p, b->h_reports, n_pairs * sizeof(PairReport), cudaMemcpyHostToDevice, h->st));
+    B2R_CUDA(cudaMemcpyAsync(b->d_reports.p, b->h_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyHostToDevice, h->st));
   if (dbg) {
     const auto t_c = std::chrono::steady_clock::now();
     fprintf(stderr, "[b2r rank %d] batch_run: build enqueue %.3f ms, rounds (host follows the device) %.3f ms, %llu rounds\n", b->rank,
@@ -734,13 +674,13 @@ extern "C" int b2r_batch_align(b2r_batch* b, const b2r_pair* pairs, size_t n_pai
   int rc = batch_run(b, pairs, n_pairs, want_fitness != 0, fitness_max_range);
   if (rc) return rc;
   cudaStream_t st = b->eng->st;
-  B2R_CUDA(cudaMemcpyAsync(b->h_reports, b->d_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(b->h_reports.p, b->d_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyDeviceToHost, st));
   B2R_CUDA(cudaStreamSynchronize(st));
   b->eng->tel.d2h += n_pairs * sizeof(PairReport);
   b->last_pair_rounds = 0;
   for (size_t i = 0; i < n_pairs; i++) {
-    out[i] = b->h_reports[i].r;
-    b->last_pair_rounds += (unsigned long long)b->h_reports[i].rounds;
+    out[i] = b->h_reports.p[i].r;
+    b->last_pair_rounds += (unsigned long long)b->h_reports.p[i].rounds;
     if (!want_fitness) out[i].fitness = NAN;
   }
   return B2R_OK;
@@ -757,10 +697,10 @@ extern "C" int b2r_batch_calc_fitness_score(b2r_batch* b, const b2r_pair* pairs,
   int rc = batch_run(b, pairs, n_pairs, true, max_range, true);
   if (rc) return rc;
   cudaStream_t st = b->eng->st;
-  B2R_CUDA(cudaMemcpyAsync(b->h_reports, b->d_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(b->h_reports.p, b->d_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyDeviceToHost, st));
   B2R_CUDA(cudaStreamSynchronize(st));
   b->eng->tel.d2h += n_pairs * sizeof(PairReport);
-  for (size_t i = 0; i < n_pairs; i++) scores[i] = b->h_reports[i].r.fitness;
+  for (size_t i = 0; i < n_pairs; i++) scores[i] = b->h_reports.p[i].r.fitness;
   return B2R_OK;
 }
 
@@ -791,7 +731,7 @@ extern "C" int b2r_batch_map_cloud_generate(b2r_batch* b, const int32_t* ids, co
   if (total >= (size_t)0x7fffffff) return fail(B2R_EINVAL, "map cloud too large (>= 2^31 points)");
   if (total == 0) return B2R_OK;
   if (out_host && !voxels && out_capacity < total) return fail(B2R_EINVAL, "output capacity too small");
-  b2r_handle* h = b->eng;
+  b2r_handle* h = b->eng.get();
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   cudaStream_t st = h->st;
   int rc = batch_sync_builds(b, false);  // the uploads of the named clouds
@@ -967,15 +907,10 @@ extern "C" int b2r_batch_loop_detect(b2r_batch* b, const b2r_pair* pairs, size_t
   const auto t_b = std::chrono::steady_clock::now();
   B2R_CUDA(b->d_send.reserve(M));
   B2R_CUDA(b->d_recv.reserve(M * (size_t)b->world));
-  if (b->h_gather_cap < M * (size_t)b->world) {
-    if (b->h_gather) cudaFreeHost(b->h_gather);
-    b->h_gather = nullptr; b->h_gather_cap = 0;
-    B2R_CUDA(cudaMallocHost(&b->h_gather, M * (size_t)b->world * sizeof(b2r_result)));
-    b->h_gather_cap = M * (size_t)b->world;
-  }
+  B2R_CUDA(b->h_gather.alloc(M * (size_t)b->world));
   B2R_CUDA(b->d_reports.reserve(1));
-  b->h_word[b2r_batch::kLanes] = 0;
-  k_pack_results<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(b->d_reports.p, (int)mine, b->d_send.p, (int)M, b->h_word_dev + b2r_batch::kLanes);
+  b->h_word.p[b2r_batch::kLanes] = 0;
+  k_pack_results<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(b->d_reports.p, (int)mine, b->d_send.p, (int)M, b->h_word.d + b2r_batch::kLanes);
   B2R_CUDA(cudaGetLastError());
   const b2r_result* gathered = b->d_send.p;
   if (b->world > 1) {
@@ -984,17 +919,17 @@ extern "C" int b2r_batch_loop_detect(b2r_batch* b, const b2r_pair* pairs, size_t
     B2R_NCCL(ncclAllGather(b->d_send.p, b->d_recv.p, M * sizeof(b2r_result), ncclChar, b->comm, st));
     gathered = b->d_recv.p;
   }
-  B2R_CUDA(cudaMemcpyAsync(b->h_gather, gathered, M * (size_t)b->world * sizeof(b2r_result), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(b->h_gather.p, gathered, M * (size_t)b->world * sizeof(b2r_result), cudaMemcpyDeviceToHost, st));
   B2R_CUDA(cudaStreamSynchronize(st));
   b->eng->tel.d2h += M * (size_t)b->world * sizeof(b2r_result);
-  b->last_pair_rounds = b->h_word[b2r_batch::kLanes];  // exact: every pair's own round count (the stream has been synchronised)
+  b->last_pair_rounds = b->h_word.p[b2r_batch::kLanes];  // exact: every pair's own round count (the stream has been synchronised)
   if (dbg) {
     const auto t_c = std::chrono::steady_clock::now();
     fprintf(stderr, "[b2r rank %d] loop_detect: batch_run + sync %.3f ms, pack + all-gather + readback %.3f ms\n", b->rank,
             std::chrono::duration<double, std::milli>(t_b - t_a).count(), std::chrono::duration<double, std::milli>(t_c - t_b).count());
   }
   for (int r = 0; r < b->world; r++)
-    for (size_t i = p0[r]; i < p1[r]; i++) all_results[i] = b->h_gather[(size_t)r * M + (i - p0[r])];
+    for (size_t i = p0[r]; i < p1[r]; i++) all_results[i] = b->h_gather.p[(size_t)r * M + (i - p0[r])];
   for (size_t g = 0; g < n_groups; g++) {
     rc = b2r_loop_argmin(all_results + group_first[g], (size_t)(group_first[g + 1] - group_first[g]), fitness_score_thresh, &best[g]);
     if (rc) return rc;

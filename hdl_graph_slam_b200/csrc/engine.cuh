@@ -1,7 +1,10 @@
 // engine.cuh — handle state of libb200reg: per-cloud device buffers, workspaces, stream.
 #pragma once
 #include <cuda_runtime.h>
+#include <memory>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 #include <cstring>
 #include <cstdio>
@@ -26,25 +29,70 @@ inline int fail(int code, const std::string& msg) {
     }                                                                                                    \
   } while (0)
 
-// growable device buffer
-template <class T>
-struct DevBuf {
+// ---- ownership: every device, pinned and mapped buffer, stream and event of the engine is owned by one of the types below and
+// freed by its destructor.  A destructor frees on the CURRENT device: each destroy entry point sets its object's device first.
+struct DeviceMem {
+  static cudaError_t alloc(void** p, void**, size_t bytes) { return cudaMalloc(p, bytes); }
+  static void free(void* p) { cudaFree(p); }
+};
+struct PinnedMem {
+  static cudaError_t alloc(void** p, void**, size_t bytes) { return cudaMallocHost(p, bytes); }
+  static void free(void* p) { cudaFreeHost(p); }
+};
+struct MappedMem {  // pinned host memory that kernels read and write in place, at the device alias `d`
+  static cudaError_t alloc(void** p, void** d, size_t bytes) {
+    cudaError_t e = cudaHostAlloc(p, bytes, cudaHostAllocMapped);
+    return e == cudaSuccess ? cudaHostGetDevicePointer(d, *p, 0) : e;
+  }
+  static void free(void* p) { cudaFreeHost(p); }
+};
+
+template <class T, class Mem>
+struct Buf {
   T* p = nullptr;
+  T* d = nullptr;  // MappedMem: the device's address of p
   size_t cap = 0;
-  cudaError_t reserve(size_t n) {
+  Buf() = default;
+  Buf(const Buf&) = delete;
+  Buf& operator=(const Buf&) = delete;
+  Buf(Buf&& o) noexcept : p(o.p), d(o.d), cap(o.cap) { o.p = o.d = nullptr; o.cap = 0; }
+  Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(d, o.d); std::swap(cap, o.cap); return *this; }
+  ~Buf() { if (p) Mem::free(p); }
+  // exactly n elements, unless it holds n already (the old contents are not kept)
+  cudaError_t alloc(size_t n) {
     if (n <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr;
-    size_t want = n + n / 8 + 64;
-    cudaError_t e = cudaMalloc(&p, want * sizeof(T));
-    cap = (e == cudaSuccess) ? want : 0;
+    if (p) Mem::free(p);
+    p = d = nullptr;
+    cudaError_t e = Mem::alloc((void**)&p, (void**)&d, n * sizeof(T));
+    cap = (e == cudaSuccess) ? n : 0;
     return e;
   }
-  void release() {
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-  }
+  // growable workspace: n elements and an eighth (+64) more, so that a slowly growing input does not reallocate on every call
+  cudaError_t reserve(size_t n) { return n <= cap ? cudaSuccess : alloc(n + n / 8 + 64); }
+};
+template <class T> using DevBuf = Buf<T, DeviceMem>;
+template <class T> using PinnedBuf = Buf<T, PinnedMem>;
+template <class T> using MappedBuf = Buf<T, MappedMem>;
+static_assert(!std::is_copy_constructible<DevBuf<char>>::value, "DevBuf owns its memory");
+
+struct Event {
+  cudaEvent_t e = nullptr;
+  Event() = default;
+  Event(const Event&) = delete;
+  Event& operator=(const Event&) = delete;
+  ~Event() { if (e) cudaEventDestroy(e); }
+  cudaError_t create() { return cudaEventCreateWithFlags(&e, cudaEventDisableTiming); }
+  operator cudaEvent_t() const { return e; }
+};
+struct Stream {
+  cudaStream_t s = nullptr;
+  Stream() = default;
+  Stream(const Stream&) = delete;
+  Stream& operator=(const Stream&) = delete;
+  ~Stream() { if (s) cudaStreamDestroy(s); }
+  // priority 0 is the default priority, the one cudaStreamCreateWithFlags gives
+  cudaError_t create(unsigned flags, int priority = 0) { return cudaStreamCreateWithPriority(&s, flags, priority); }
+  operator cudaStream_t() const { return s; }
 };
 
 // ---- telemetry: copy byte counters, launch counters and (optional) CUDA-event timing per kernel class
@@ -62,6 +110,13 @@ struct Telemetry {
   struct Span { cudaEvent_t a, b; int cls; };
   std::vector<Span> spans;
   std::vector<cudaEvent_t> pool;
+  Telemetry() = default;
+  Telemetry(const Telemetry&) = delete;
+  Telemetry& operator=(const Telemetry&) = delete;
+  ~Telemetry() {
+    resolve();
+    for (auto e : pool) cudaEventDestroy(e);
+  }
   cudaEvent_t get() {
     if (!pool.empty()) { cudaEvent_t e = pool.back(); pool.pop_back(); return e; }
     cudaEvent_t e = nullptr;
@@ -94,11 +149,6 @@ struct Telemetry {
   void reset() {
     h2d = d2h = 0;
     for (int i = 0; i < KC_COUNT; i++) { launches[i] = calls[i] = 0; ms[i] = 0; }
-  }
-  void release() {
-    resolve();
-    for (auto e : pool) cudaEventDestroy(e);
-    pool.clear();
   }
 };
 #define TEL_BEGIN(tel, st) cudaEvent_t _tel_ev = (tel) ? (tel)->begin(st) : nullptr
@@ -139,7 +189,7 @@ inline int wait_host_result(const unsigned long long* flag, unsigned long long s
   return fail(B2R_ECUDA, "reduction kernel finished without signalling its result");
 }
 
-struct NdtVoxelMap;  // ndt.cuh
+struct NdtVoxelMap;  // ndt.cuh: complete wherever a Cloud is destroyed
 
 // One point cloud resident on the device with everything derived from it.
 struct Cloud {
@@ -157,7 +207,7 @@ struct Cloud {
   DevBuf<double> cov;              // sorted order, 6 per point
   bool cov_ready = false;
   // NDT (target only)
-  NdtVoxelMap* ndt = nullptr;
+  std::unique_ptr<NdtVoxelMap> ndt;
   bool ndt_ready = false;
   void invalidate() { bvh_ready = cov_ready = ndt_ready = false; }
   Bvh bvh() const {
@@ -173,8 +223,8 @@ struct BuildCtx {
   DevBuf<unsigned int> keys_a, keys_b;
   DevBuf<int> vals_a, vals_b;
   DevBuf<char> sort_tmp;
-  int* mm = nullptr;
-  void release() { keys_a.release(); keys_b.release(); vals_a.release(); vals_b.release(); sort_tmp.release(); if (mm) cudaFree(mm); mm = nullptr; }
+  DevBuf<int> mm;  // 8 ints
 };
+static_assert(!std::is_copy_constructible<Cloud>::value && !std::is_copy_constructible<BuildCtx>::value, "a Cloud / BuildCtx owns its buffers");
 
 }  // namespace b2r

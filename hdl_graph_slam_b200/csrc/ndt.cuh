@@ -48,7 +48,7 @@ constexpr unsigned long long kNdtEmpty = 0xffffffffffffffffull;
 // and an open-addressing hash table (key -> position).  No dense table: a 200 m extent at 0.5 m resolution (16 M cells, the
 // effective setting of hdl_graph_slam_imu.launch) costs what its ~10^4 occupied voxels cost.
 struct NdtVoxelMap {
-  VoxGeom* geom = nullptr;      // device
+  DevBuf<VoxGeom> geom;         // one record
   VoxGeom h_geom;               // host copy (valid after ndt_sync_geom)
   bool h_geom_valid = false;
   DevBuf<unsigned int> keys;    // sorted voxel keys (n), 0xffffffff = dropped (non-finite) point
@@ -64,36 +64,18 @@ struct NdtWork {
   DevBuf<double> partials;
   DevBuf<double> grows;           // derivative pass: group rows of the two-level sum
   DevBuf<unsigned int> gcount;    // derivative pass: per-group arrival counters (zero between launches)
-  unsigned long long* d_queue = nullptr;  // chunk ticket counter, monotone over launches
+  DevBuf<unsigned long long> d_queue;  // chunk ticket counter, monotone over launches
   unsigned long long qnext = 0;   // first ticket of the next launch
-  double* d_out = nullptr;        // 64 doubles
-  unsigned int* d_counter = nullptr;
-  double* h_out = nullptr;        // pinned + mapped: kernels write their results here directly
-  double* h_out_dev = nullptr;    // device alias of h_out
+  DevBuf<double> d_out;           // 64 doubles
+  DevBuf<unsigned int> d_counter;
+  MappedBuf<double> h_out;        // 64 doubles + flags: kernels write their results here directly
   unsigned long long* h_flag = nullptr; unsigned long long* h_flag_dev = nullptr; unsigned long long seq = 0;
-  VoxGeom* h_geom_pinned = nullptr;
-  unsigned long long* d_pairs = nullptr;
+  PinnedBuf<VoxGeom> h_geom_pinned;
+  DevBuf<unsigned long long> d_pairs;
   BuildCtx* bc = nullptr;         // build scratch of the handle's main stream (keys / values / sort space)
   Telemetry* tel = nullptr;
-  void release() {
-    partials.release(); grows.release(); gcount.release();
-    if (d_queue) cudaFree(d_queue);
-    d_queue = nullptr;
-    if (d_out) cudaFree(d_out);
-    if (d_counter) cudaFree(d_counter);
-    if (h_out) cudaFreeHost(h_out);
-    if (h_geom_pinned) cudaFreeHost(h_geom_pinned);
-    if (d_pairs) cudaFree(d_pairs);
-    d_out = nullptr; d_counter = nullptr; h_out = nullptr; h_geom_pinned = nullptr; d_pairs = nullptr;
-  }
 };
-
-inline void ndt_free_map(NdtVoxelMap* m) {
-  if (!m) return;
-  if (m->geom) cudaFree(m->geom);
-  m->keys.release(); m->sorted.release(); m->vox.release(); m->cells.release(); m->table.release();
-  delete m;
-}
+static_assert(!std::is_copy_constructible<NdtWork>::value, "an NdtWork owns its buffers");
 
 // ------------------------------------------------------------------------------------------------ voxel build kernels
 // VoxelGridCovariance::applyFilter geometry (A.3): min_b = floor(min_p * inv_leaf) ...
@@ -646,21 +628,20 @@ __global__ void __launch_bounds__(kNdtThreads) k_ndt_hessian_batch(const NdtArgs
 
 // ------------------------------------------------------------------------------------------------ host side
 inline int ndt_init_work(NdtWork& W) {
-  if (W.d_out) return B2R_OK;
-  B2R_CUDA(cudaMalloc(&W.d_out, 64 * sizeof(double)));
-  B2R_CUDA(cudaMalloc(&W.d_counter, 4 * sizeof(unsigned int)));
-  B2R_CUDA(cudaMemset(W.d_counter, 0, 4 * sizeof(unsigned int)));
-  B2R_CUDA(cudaMalloc(&W.d_pairs, sizeof(unsigned long long)));
-  B2R_CUDA(cudaMemset(W.d_pairs, 0, sizeof(unsigned long long)));
-  B2R_CUDA(cudaMalloc(&W.d_queue, sizeof(unsigned long long)));
-  B2R_CUDA(cudaMemset(W.d_queue, 0, sizeof(unsigned long long)));
+  if (W.d_out.p) return B2R_OK;
+  B2R_CUDA(W.d_out.alloc(64));
+  B2R_CUDA(W.d_counter.alloc(4));
+  B2R_CUDA(cudaMemset(W.d_counter.p, 0, 4 * sizeof(unsigned int)));
+  B2R_CUDA(W.d_pairs.alloc(1));
+  B2R_CUDA(cudaMemset(W.d_pairs.p, 0, sizeof(unsigned long long)));
+  B2R_CUDA(W.d_queue.alloc(1));
+  B2R_CUDA(cudaMemset(W.d_queue.p, 0, sizeof(unsigned long long)));
   W.qnext = 0;
-  B2R_CUDA(cudaHostAlloc(&W.h_out, 72 * sizeof(double), cudaHostAllocMapped));
-  B2R_CUDA(cudaHostGetDevicePointer((void**)&W.h_out_dev, W.h_out, 0));
-  W.h_flag = reinterpret_cast<unsigned long long*>(W.h_out + 64);
-  W.h_flag_dev = reinterpret_cast<unsigned long long*>(W.h_out_dev + 64);
+  B2R_CUDA(W.h_out.alloc(72));
+  W.h_flag = reinterpret_cast<unsigned long long*>(W.h_out.p + 64);
+  W.h_flag_dev = reinterpret_cast<unsigned long long*>(W.h_out.d + 64);
   *W.h_flag = 0;
-  B2R_CUDA(cudaMallocHost(&W.h_geom_pinned, sizeof(VoxGeom)));
+  B2R_CUDA(W.h_geom_pinned.alloc(1));
   return B2R_OK;
 }
 
@@ -671,8 +652,8 @@ inline int ndt_ensure_map(const b2r_config& cfg, Cloud& c, NdtWork& W, cudaStrea
   BuildCtx* B = W.bc;
   if (!B) return fail(B2R_ESTATE, "internal: NDT build scratch not attached");
   if (!c.ndt) {
-    c.ndt = new NdtVoxelMap();
-    B2R_CUDA(cudaMalloc(&c.ndt->geom, sizeof(VoxGeom)));
+    c.ndt.reset(new NdtVoxelMap());
+    B2R_CUDA(c.ndt->geom.alloc(1));
   }
   NdtVoxelMap& M = *c.ndt;
   const int n = (int)c.n;
@@ -691,14 +672,14 @@ inline int ndt_ensure_map(const b2r_config& cfg, Cloud& c, NdtWork& W, cudaStrea
   B2R_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, B->keys_a.p, M.keys.p, B->vals_a.p, B->vals_b.p, n, 0, 32, st));
   B2R_CUDA(B->sort_tmp.reserve(tmp_bytes + 256));
   TEL_BEGIN(W.tel, st);
-  k_grid_reset<<<1, 32, 0, st>>>(B->mm);
+  k_grid_reset<<<1, 32, 0, st>>>(B->mm.p);
   int nb = n > 0 ? (n + 255) / 256 : 1;
   if (nb > 1184) nb = 1184;
-  if (n > 0) k_bbox<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, n, B->mm);
-  k_vox_params<<<1, 1, 0, st>>>(B->mm, M.geom, n, (float)cfg.ndt_resolution);
+  if (n > 0) k_bbox<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, n, B->mm.p);
+  k_vox_params<<<1, 1, 0, st>>>(B->mm.p, M.geom.p, n, (float)cfg.ndt_resolution);
   B2R_CUDA(cudaMemsetAsync(M.table.p, 0xff, tsize * sizeof(unsigned long long), st));
   if (n > 0) {
-    k_vox_keys<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, n, M.geom, B->keys_a.p, B->vals_a.p);
+    k_vox_keys<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, n, M.geom.p, B->keys_a.p, B->vals_a.p);
     size_t tb = B->sort_tmp.cap;
     // stable LSD radix sort by voxel key: inside a voxel the points stay in ascending index, the order the moments are summed in
     B2R_CUDA(cub::DeviceRadixSort::SortPairs(B->sort_tmp.p, tb, B->keys_a.p, M.keys.p, B->vals_a.p, B->vals_b.p, n, 0, 32, st));
@@ -713,9 +694,9 @@ inline int ndt_ensure_map(const b2r_config& cfg, Cloud& c, NdtWork& W, cudaStrea
 
 inline int ndt_sync_geom(NdtVoxelMap& M, NdtWork& W, cudaStream_t st) {
   if (M.h_geom_valid) return B2R_OK;
-  B2R_CUDA(cudaMemcpyAsync(W.h_geom_pinned, M.geom, sizeof(VoxGeom), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(W.h_geom_pinned.p, M.geom.p, sizeof(VoxGeom), cudaMemcpyDeviceToHost, st));
   B2R_CUDA(cudaStreamSynchronize(st));
-  M.h_geom = *W.h_geom_pinned;
+  M.h_geom = *W.h_geom_pinned.p;
   M.h_geom_valid = true;
   if (!M.h_geom.ok) return fail(B2R_EUNSUPPORTED, "NDT voxel grid exceeds int32 indices (leaf size too small for the extent; PCL refuses the same input)");
   return B2R_OK;
@@ -943,7 +924,7 @@ inline void ndt_fill_args(const b2r_config& cfg, const Cloud& src, const Cloud& 
                           NdtArgs& A) {
   const NdtVoxelMap& M = *tgt.ndt;
   A.src = src.sorted.p; A.n_sorted = src.nsup * 1024;
-  A.geom = M.geom; A.table = M.table.p; A.mask = M.mask; A.cells = M.cells.p; A.vox = M.vox.p;
+  A.geom = M.geom.p; A.table = M.table.p; A.mask = M.mask; A.cells = M.cells.p; A.vox = M.vox.p;
   for (int i = 0; i < 12; i++) A.Tf[i] = Tf_row[i];
   std::memcpy(A.jang, K.jang, sizeof(A.jang)); std::memcpy(A.hang, K.hang, sizeof(A.hang));
   std::memcpy(A.jang_d, K.jang_d, sizeof(A.jang_d)); std::memcpy(A.hang_d, K.hang_d, sizeof(A.hang_d));
@@ -983,8 +964,8 @@ inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& 
     B2R_CUDA(W.gcount.reserve(ngroups));
     B2R_CUDA(cudaMemsetAsync(W.gcount.p, 0, W.gcount.cap * sizeof(unsigned int), st));  // every launch leaves the counters at zero
   }
-  A.partials = W.partials.p; A.grows = W.grows.p; A.gcount = W.gcount.p; A.queue = W.d_queue; A.qbase = 0;
-  A.out = W.h_out_dev; A.counter = W.d_counter; A.pairs = W.d_pairs;
+  A.partials = W.partials.p; A.grows = W.grows.p; A.gcount = W.gcount.p; A.queue = W.d_queue.p; A.qbase = 0;
+  A.out = W.h_out.d; A.counter = W.d_counter.p; A.pairs = W.d_pairs.p;
   A.flag = W.h_flag_dev; A.seq = ++W.seq;
   if (hessian_only) {
     { TEL_BEGIN(W.tel, st);
@@ -992,9 +973,9 @@ inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& 
       TEL_END(W.tel, KC_NDT_HESS, 1, st); }
     if (W.tel) W.tel->d2h += 36 * sizeof(double);
     B2R_CUDA(cudaGetLastError());
-    int rc = wait_host_result(W.h_flag, A.seq, W.h_out, 36, false, st);
+    int rc = wait_host_result(W.h_flag, A.seq, W.h_out.p, 36, false, st);
     if (rc) return rc;
-    ndt_read_pass(W.h_out, true, true, out);
+    ndt_read_pass(W.h_out.p, true, true, out);
     return B2R_OK;
   }
   { TEL_BEGIN(W.tel, st);  // W.d_pairs is zero here: allocated zeroed, and the last block of every pass resets it after reading it
@@ -1008,9 +989,9 @@ inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& 
   }
   if (W.tel) W.tel->d2h += kNdtAcc * sizeof(double) + 8;
   B2R_CUDA(cudaGetLastError());
-  int rc = wait_host_result(W.h_flag, A.seq, W.h_out, kNdtAcc, true, st);
+  int rc = wait_host_result(W.h_flag, A.seq, W.h_out.p, kNdtAcc, true, st);
   if (rc) return rc;
-  ndt_read_pass(W.h_out, compute_hessian, false, out);
+  ndt_read_pass(W.h_out.p, compute_hessian, false, out);
   return B2R_OK;
 }
 

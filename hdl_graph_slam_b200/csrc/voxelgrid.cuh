@@ -36,23 +36,14 @@ struct VoxelWork {
   DevBuf<int> keys_a, keys_b, vals_a, vals_b, flags, slots, okeys, ocounts;
   DevBuf<int> buckets;  // approx_voxelgrid.cuh: per hash slot, occupied flag, then the output slot of its last run
   DevBuf<char> tmp;
-  int* mm = nullptr;
-  VgGeom* geom = nullptr;
-  VgGeom* h_geom = nullptr;  // pinned
-  int* h_total = nullptr;    // pinned + mapped: [0] voxel count, [1] overflow flag
-  int* h_total_dev = nullptr;
+  DevBuf<int> mm;            // 8 ints
+  DevBuf<VgGeom> geom;
+  PinnedBuf<VgGeom> h_geom;
+  MappedBuf<int> h_total;    // [0] voxel count, [1] overflow flag
   Telemetry* tel = nullptr;
   bool wide_clusters = false;  // 16-CTA clusters may be launched on this device (set by the handle: cluster16_allowed())
-  void release() {
-    in.release(); out.release(); keys_a.release(); keys_b.release(); vals_a.release(); vals_b.release(); flags.release(); slots.release();
-    okeys.release(); ocounts.release(); buckets.release(); tmp.release();
-    if (mm) cudaFree(mm);
-    if (geom) cudaFree(geom);
-    if (h_geom) cudaFreeHost(h_geom);
-    if (h_total) cudaFreeHost(h_total);
-    mm = nullptr; geom = nullptr; h_geom = nullptr; h_total = nullptr;
-  }
 };
+static_assert(!std::is_copy_constructible<VoxelWork>::value, "a VoxelWork owns its buffers");
 
 __global__ void k_vg_params(const int* mm, VgGeom* g, int n, float leaf) {
   VgGeom G;
@@ -327,12 +318,11 @@ static cudaError_t launch_voxelgrid_cluster(int shape_index, const VgArgs& A, cu
 
 // the small device / pinned words of the voxel-grid chains, allocated on first use
 inline int vg_alloc_words(VoxelWork& W) {
-  if (!W.mm) {
-    B2R_CUDA(cudaMalloc(&W.mm, 8 * sizeof(int)));
-    B2R_CUDA(cudaMalloc(&W.geom, sizeof(VgGeom)));
-    B2R_CUDA(cudaMallocHost(&W.h_geom, sizeof(VgGeom)));
-    B2R_CUDA(cudaHostAlloc(&W.h_total, 4 * sizeof(int), cudaHostAllocMapped));
-    B2R_CUDA(cudaHostGetDevicePointer((void**)&W.h_total_dev, W.h_total, 0));
+  if (!W.mm.p) {
+    B2R_CUDA(W.mm.alloc(8));
+    B2R_CUDA(W.geom.alloc(1));
+    B2R_CUDA(W.h_geom.alloc(1));
+    B2R_CUDA(W.h_total.alloc(4));
   }
   return B2R_OK;
 }
@@ -351,14 +341,14 @@ inline int voxelgrid_device(VoxelWork& W, cudaStream_t st, const float* d_in, si
   if (shape.cl && cluster_ok) {
     VgArgs A;
     A.in = d_in; A.stride_f = sf; A.n = N; A.leaf = leaf; A.out = W.out.p; A.okeys = W.okeys.p; A.ocounts = W.ocounts.p;
-    A.total = W.mm + 6; A.h_total = W.h_total_dev;
-    W.h_total[0] = -1;  // the kernel's count lands here (host-mapped); -1 = not yet
+    A.total = W.mm.p + 6; A.h_total = W.h_total.d;
+    W.h_total.p[0] = -1;  // the kernel's count lands here (host-mapped); -1 = not yet
     TEL_BEGIN(W.tel, st);
     B2R_CUDA(launch_voxelgrid_cluster(build_shape_index(shape), A, st));
     TEL_END(W.tel, KC_VOXELGRID, 1, st);
     B2R_CUDA(cudaStreamSynchronize(st));
-    *m = (size_t)(W.h_total[0] < 0 ? 0 : W.h_total[0]);
-    *overflow = W.h_total[1];
+    *m = (size_t)(W.h_total.p[0] < 0 ? 0 : W.h_total.p[0]);
+    *overflow = W.h_total.p[1];
     return B2R_OK;
   }
   // ---- inputs beyond 131 072 points: the kernel chain with the toolkit's radix sort / scan
@@ -370,24 +360,24 @@ inline int voxelgrid_device(VoxelWork& W, cudaStream_t st, const float* d_in, si
   B2R_CUDA(W.tmp.reserve(std::max(tmp_sort, tmp_scan) + 256));
   const unsigned nb = (unsigned)((n + 255) / 256);
   TEL_BEGIN(W.tel, st);
-  k_grid_reset<<<1, 32, 0, st>>>(W.mm);
-  k_bbox<<<nb > 1184 ? 1184 : nb, 256, 0, st>>>(d_in, sf, N, W.mm);
-  k_vg_params<<<1, 1, 0, st>>>(W.mm, W.geom, N, leaf);
-  B2R_CUDA(cudaMemcpyAsync(W.h_geom, W.geom, sizeof(VgGeom), cudaMemcpyDeviceToHost, st));
-  k_vg_keys<<<nb, 256, 0, st>>>(d_in, sf, N, W.geom, W.keys_a.p, W.vals_a.p);
+  k_grid_reset<<<1, 32, 0, st>>>(W.mm.p);
+  k_bbox<<<nb > 1184 ? 1184 : nb, 256, 0, st>>>(d_in, sf, N, W.mm.p);
+  k_vg_params<<<1, 1, 0, st>>>(W.mm.p, W.geom.p, N, leaf);
+  B2R_CUDA(cudaMemcpyAsync(W.h_geom.p, W.geom.p, sizeof(VgGeom), cudaMemcpyDeviceToHost, st));
+  k_vg_keys<<<nb, 256, 0, st>>>(d_in, sf, N, W.geom.p, W.keys_a.p, W.vals_a.p);
   size_t tb = W.tmp.cap;
   B2R_CUDA(cub::DeviceRadixSort::SortPairs(W.tmp.p, tb, W.keys_a.p, W.keys_b.p, W.vals_a.p, W.vals_b.p, N, 0, 32, st));
   k_vg_heads<<<nb, 256, 0, st>>>(W.keys_b.p, N, W.flags.p);
   tb = W.tmp.cap;
   B2R_CUDA(cub::DeviceScan::ExclusiveSum(W.tmp.p, tb, W.flags.p, W.slots.p, N, st));
   k_vg_centroid<<<nb, 256, 0, st>>>(d_in, sf, N, W.keys_b.p, W.vals_b.p, W.flags.p, W.slots.p, W.out.p, sf, W.okeys.p, W.ocounts.p,
-                                    (int*)(W.mm + 6));
+                                    (int*)(W.mm.p + 6));
   TEL_END(W.tel, KC_VOXELGRID, 14, st);
   B2R_CUDA(cudaGetLastError());
-  B2R_CUDA(cudaMemcpyAsync(W.h_total, W.mm + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaMemcpyAsync(W.h_total.p, W.mm.p + 6, sizeof(int), cudaMemcpyDeviceToHost, st));
   B2R_CUDA(cudaStreamSynchronize(st));
-  *m = (size_t)W.h_total[0];
-  *overflow = W.h_geom->overflow;
+  *m = (size_t)W.h_total.p[0];
+  *overflow = W.h_geom.p->overflow;
   return B2R_OK;
 }
 
