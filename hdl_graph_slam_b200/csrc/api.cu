@@ -1428,7 +1428,10 @@ static int ingest_device(b2r_handle* h, const unsigned char* d_blob, size_t n, c
   B2R_CUDA(h->ingest_out.reserve(n * 8 + 8));
   UnpackArgs A;
   A.data = d_blob; A.n = (long long)n; A.point_step = L.point_step; A.off_x = L.off_x; A.off_y = L.off_y; A.off_z = L.off_z;
-  A.off_i = L.off_intensity; A.type_i = L.intensity_datatype; A.bigendian = L.is_bigendian; A.out = h->ingest_out.p;
+  // pcl::PointXYZI's intensity is a float: fromPCLPointCloud2 maps an "intensity" field only when it is FLOAT32 (count 1) and
+  // leaves the point's intensity at 0 for every other datatype
+  A.off_i = L.intensity_datatype == 7 ? L.off_intensity : 0xffffffffu;
+  A.bigendian = L.is_bigendian; A.out = h->ingest_out.p;
   { TEL_BEGIN(&h->tel, h->st);
     k_unpack_points<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)h->n_sm * 16), 256, 0, h->st>>>(A);
     TEL_END(&h->tel, KC_MISC, 1, h->st); }
@@ -1460,9 +1463,14 @@ extern "C" int b2r_ingest_pointcloud2(b2r_handle* h, const void* data, size_t n_
   if (n_points > (size_t)0x3fffffff) return fail(B2R_EINVAL, "too many points");
   const size_t bytes = n_points * layout->point_step;
   B2R_CUDA(h->ingest_blob.reserve(bytes + 16));
+  const bool pinned = is_pinned_host(data);
   B2R_CUDA(cudaMemcpyAsync(h->ingest_blob.p, data, bytes, cudaMemcpyHostToDevice, h->st));  // the message's data[] goes up unconverted
   h->tel.h2d += bytes;
-  return ingest_device(h, reinterpret_cast<const unsigned char*>(h->ingest_blob.p), n_points, *layout, d_points);
+  // a pinned buffer is DMA'd in place: `upload_ev` marks the end of that copy, so the caller has its buffer back on return
+  if (pinned) B2R_CUDA(cudaEventRecord(h->upload_ev, h->st));
+  rc = ingest_device(h, reinterpret_cast<const unsigned char*>(h->ingest_blob.p), n_points, *layout, d_points);
+  if (pinned) B2R_CUDA(cudaEventSynchronize(h->upload_ev));
+  return rc;
 }
 
 extern "C" int b2r_pcd_read_header(const char* path, b2r_point_layout* layout, size_t* n_points, size_t* data_offset) {
@@ -1479,15 +1487,11 @@ extern "C" int b2r_pcd_read_header(const char* path, b2r_point_layout* layout, s
   unsigned int off = 0, found = 0;
   for (size_t i = 0; i < H.fields.size(); i++) {
     const unsigned int sz = (unsigned int)(H.size[i] * H.count[i]);
-    const bool f32 = H.type[i] == 'F' && H.size[i] == 4;
+    const bool f32 = H.type[i] == 'F' && H.size[i] == 4 && H.count[i] == 1;  // the fields pcl::PointXYZI maps: FLOAT32, count 1
     if (H.fields[i] == "x" && f32) { layout->off_x = off; found |= 1; }
     else if (H.fields[i] == "y" && f32) { layout->off_y = off; found |= 2; }
     else if (H.fields[i] == "z" && f32) { layout->off_z = off; found |= 4; }
-    else if (H.fields[i] == "intensity") {
-      layout->off_intensity = off;
-      const char t = H.type[i];
-      layout->intensity_datatype = (t == 'F') ? (H.size[i] == 8 ? 8 : 7) : (t == 'U') ? (H.size[i] == 1 ? 2 : H.size[i] == 2 ? 4 : 6) : (H.size[i] == 1 ? 1 : H.size[i] == 2 ? 3 : 5);
-    }
+    else if (H.fields[i] == "intensity" && f32) layout->off_intensity = off;  // any other intensity type is left unmapped (intensity 0)
     off += sz;
   }
   if (found != 7) return fail(B2R_EINVAL, "PCD has no float32 x / y / z fields");
@@ -1507,11 +1511,9 @@ extern "C" int b2r_ingest_pcd(b2r_handle* h, const char* path, const void** d_po
   *d_points = nullptr; *n_points = 0;
   if (n == 0) return B2R_OK;
   const size_t bytes = n * L.point_step;
-  if (h->ingest_pinned.cap < bytes) {  // the file body is read straight into pinned memory: no intermediate PointCloud, no repack
+  B2R_CUDA(cudaStreamSynchronize(h->st));  // a previous upload from `ingest_pinned` may still be in flight: before it is reused or freed
+  if (h->ingest_pinned.cap < bytes)  // the file body is read straight into pinned memory: no intermediate PointCloud, no repack
     B2R_CUDA(h->ingest_pinned.alloc(bytes + bytes / 4 + 4096));
-  } else {
-    B2R_CUDA(cudaStreamSynchronize(h->st));  // a previous upload from this buffer may still be in flight
-  }
   FILE* f = fopen(path, "rb");
   if (!f) return fail(B2R_EINVAL, std::string("cannot open ") + path);
   bool ok = fseek(f, (long)off, SEEK_SET) == 0 && fread(h->ingest_pinned.p, 1, bytes, f) == bytes;

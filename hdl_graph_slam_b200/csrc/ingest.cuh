@@ -2,8 +2,10 @@
 // uploaded AS THEY ARE and unpacked into PointXYZI records on the device, instead of the host-side pcl::fromROSMsg /
 // pcl::io::loadPCDFile conversions at /root/reference/apps/scan_matching_odometry_nodelet.cpp:118-119,
 // apps/hdl_graph_slam_nodelet.cpp:153-154 and src/hdl_graph_slam/keyframe.cpp:57,141.
-//   k_unpack_points   <- pcl::fromROSMsg / the PCD reader's field mapping: x, y, z (FLOAT32) and intensity (FLOAT32 / UINT8 /
-//                        UINT16 / UINT32 ...) picked from arbitrary byte offsets of a point_step-long record, optional byte swap
+//   k_unpack_points   <- pcl::fromROSMsg / the PCD reader's field mapping for PointXYZI: x, y, z (FLOAT32) and intensity picked from
+//                        arbitrary byte offsets of a point_step-long record.  As in PCL, a field is mapped only when its datatype
+//                        and count match the point type's, so intensity is read only when it is FLOAT32; any other intensity
+//                        field is left unmapped and the point keeps intensity 0.  is_bigendian byte-swaps (PCL copies native bytes).
 #pragma once
 #include <cstdio>
 #include <cstring>
@@ -16,7 +18,7 @@ namespace b2r {
 struct UnpackArgs {
   const unsigned char* data;
   long long n;
-  unsigned int point_step, off_x, off_y, off_z, off_i, type_i, bigendian;
+  unsigned int point_step, off_x, off_y, off_z, off_i, bigendian;  // off_i = 0xffffffff: no FLOAT32 intensity
   float* out;  // 8 floats per point: x y z 1 | intensity 0 0 0  (pcl::PointXYZI)
 };
 
@@ -34,23 +36,8 @@ __global__ void k_unpack_points(const __grid_constant__ UnpackArgs A) {
     o[1] = __uint_as_float(load_u32(r + A.off_y, swap));
     o[2] = __uint_as_float(load_u32(r + A.off_z, swap));
     o[3] = 1.0f;
-    float inten = 0.f;
-    if (A.off_i != 0xffffffffu) {
-      const unsigned char* q = r + A.off_i;
-      switch (A.type_i) {  // sensor_msgs/PointField datatypes
-        case 1: inten = (float)(signed char)q[0]; break;                                   // INT8
-        case 2: inten = (float)q[0]; break;                                                // UINT8
-        case 3: { unsigned int v = swap ? ((unsigned int)q[0] << 8 | q[1]) : ((unsigned int)q[1] << 8 | q[0]); inten = (float)(short)v; break; }  // INT16
-        case 4: { unsigned int v = swap ? ((unsigned int)q[0] << 8 | q[1]) : ((unsigned int)q[1] << 8 | q[0]); inten = (float)v; break; }         // UINT16
-        case 5: inten = (float)(int)load_u32(q, swap); break;                              // INT32
-        case 6: inten = (float)load_u32(q, swap); break;                                   // UINT32
-        case 8: { unsigned long long lo = load_u32(q, false), hi = load_u32(q + 4, false);                                                    // FLOAT64
-                  unsigned long long v = swap ? ((unsigned long long)__byte_perm((unsigned int)lo, 0, 0x0123) << 32 | __byte_perm((unsigned int)hi, 0, 0x0123)) : (hi << 32 | lo);
-                  inten = (float)__longlong_as_double((long long)v); break; }
-        default: inten = __uint_as_float(load_u32(q, swap)); break;                        // 7 = FLOAT32
-      }
-    }
-    o[4] = inten; o[5] = 0.f; o[6] = 0.f; o[7] = 0.f;
+    o[4] = A.off_i != 0xffffffffu ? __uint_as_float(load_u32(r + A.off_i, swap)) : 0.f;
+    o[5] = 0.f; o[6] = 0.f; o[7] = 0.f;
   }
 }
 

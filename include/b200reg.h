@@ -257,18 +257,29 @@ int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot* keyframes
  * pcl::PointXYZI records (32 bytes: x y z 1 | intensity 0 0 0) — the work of pcl::fromROSMsg at
  * apps/scan_matching_odometry_nodelet.cpp:118-119 and apps/hdl_graph_slam_nodelet.cpp:153-154, and of pcl::io::loadPCDFile at
  * src/hdl_graph_slam/keyframe.cpp:141.  *d_points is an engine-owned device buffer (valid until the next ingest call on this
- * handle) for b2r_set_source_device / b2r_set_target_device / b2r_prefilter(device_input = 1) / b2r_batch_add_cloud_device. */
+ * handle) for b2r_set_source_device / b2r_set_target_device / b2r_prefilter(device_input = 1) / b2r_batch_add_cloud_device.
+ *   - Field mapping as PCL's fromPCLPointCloud2 does it for PointXYZI: intensity is read only when its datatype is FLOAT32; an
+ *     intensity field of any other datatype is left unmapped and every point gets intensity 0 (PCL warns and does the same).
+ *   - is_bigendian is honoured: x, y, z and intensity are byte-swapped.  (PCL copies the bytes as they are, so a big-endian
+ *     message on a little-endian host decodes to garbage there; this is a deliberate deviation.)
+ *   - Rows must be contiguous: n_points records of point_step bytes back to back, i.e. row_step == width * point_step.  An
+ *     organized message with padded rows has to be repacked by the caller first.
+ *   - b2r_ingest_pointcloud2 is synchronous with respect to `data`: when it returns, the copy out of the caller's buffer has
+ *     finished (pageable or pinned) and the buffer may be reused. */
 typedef struct b2r_point_layout {
   uint32_t point_step;         /* PointCloud2.point_step */
   uint32_t off_x, off_y, off_z;/* byte offsets of the FLOAT32 fields "x", "y", "z" */
   uint32_t off_intensity;      /* byte offset of "intensity", 0xffffffff = absent (intensity 0) */
-  uint32_t intensity_datatype; /* sensor_msgs/PointField datatype of "intensity": 1 INT8 2 UINT8 3 INT16 4 UINT16 5 INT32 6 UINT32 7 FLOAT32 8 FLOAT64 */
+  uint32_t intensity_datatype; /* sensor_msgs/PointField datatype of "intensity" (1 INT8 2 UINT8 3 INT16 4 UINT16 5 INT32 6 UINT32 7 FLOAT32
+                                  8 FLOAT64): validated against point_step, but only 7 is read; every other type gives intensity 0 */
   uint32_t is_bigendian;       /* PointCloud2.is_bigendian */
 } b2r_point_layout;
 int b2r_ingest_pointcloud2(b2r_handle* h, const void* data, size_t n_points, const b2r_point_layout* layout, const void** d_points);
-/* header of a binary PCD file (the cloud.pcd KeyFrame::save writes with pcl::io::savePCDFileBinary, keyframe.cpp:57) */
+/* header of a binary PCD file (the cloud.pcd KeyFrame::save writes with pcl::io::savePCDFileBinary, keyframe.cpp:57): x, y, z must be
+ * F 4 COUNT 1 (else B2R_EINVAL); "intensity" is reported (datatype 7) only when it is F 4 COUNT 1, otherwise off_intensity = 0xffffffff.
+ * DATA ascii / binary_compressed: B2R_EUNSUPPORTED.  Without POINTS the count is WIDTH * HEIGHT. */
 int b2r_pcd_read_header(const char* path, b2r_point_layout* layout, size_t* n_points, size_t* data_offset);
-/* header parse + fread of the body straight into pinned memory + H2D + device unpack */
+/* header parse + fread of the body straight into engine-owned pinned memory + H2D + device unpack (field mapping as above) */
 int b2r_ingest_pcd(b2r_handle* h, const char* path, const void** d_points, size_t* n_points);
 
 /* ---- host mirrors of the two callers (logic identical to the reference; only the handle is ours) ---------------- */
