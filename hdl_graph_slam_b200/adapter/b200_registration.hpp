@@ -93,7 +93,7 @@ public:
 
   explicit B200Registration(const b2r_config& cfg) {
     if (b2r_create(&cfg, &h_) != B2R_OK) throw std::runtime_error(std::string("b200reg: ") + b2r_last_error());
-    this->reg_name_ = cfg.method == B2R_METHOD_GICP ? "B200_GICP" : "B200_NDT";
+    this->reg_name_ = cfg.method == B2R_METHOD_GICP ? "B200_GICP" : (cfg.method == B2R_METHOD_NDT_PCL ? "B200_NDT_PCL" : "B200_NDT");
     this->max_iterations_ = cfg.max_iterations;
     this->transformation_epsilon_ = cfg.transformation_epsilon;
     this->corr_dist_threshold_ = cfg.max_correspondence_distance;
@@ -168,6 +168,15 @@ private:
 //       cfg.k_correspondences = pnh.param<int>("reg_correspondence_randomness", 20);
 //       cfg.ndt_resolution = pnh.param<double>("reg_resolution", 0.5);
 //       cfg.ndt_search_method = pnh.param<std::string>("reg_nn_search_method", "DIRECT7") == "DIRECT1" ? 1 : 7;
+//       cfg.device_id = pnh.param<int>("reg_device_id", 0);
+//       return pcl::Registration<PointT, PointT>::Ptr(new B200Registration<PointT>(cfg));
+//     }
+//     else if(registration_method == "B200_NDT_PCL") {  // in place of the NDT branch (registrations.cpp:93-100)
+//       b2r_config cfg;
+//       b2r_config_default(&cfg, B2R_METHOD_NDT_PCL);  // pcl::NormalDistributionsTransform: step size 0.1, outlier ratio 0.55
+//       cfg.transformation_epsilon = pnh.param<double>("reg_transformation_epsilon", 0.01);
+//       cfg.max_iterations = pnh.param<int>("reg_maximum_iterations", 64);
+//       cfg.ndt_resolution = pnh.param<double>("reg_resolution", 0.5);
 //       cfg.device_id = pnh.param<int>("reg_device_id", 0);
 //       return pcl::Registration<PointT, PointT>::Ptr(new B200Registration<PointT>(cfg));
 //     }

@@ -126,7 +126,7 @@ extern "C" int b2r_config_default(b2r_config* c, int method) {
   c->ndt_mt_interval_flag = 0;
   c->ndt_fixed_iterations = 0;
   c->grid_cell_min = 0.5f;
-  if (method != B2R_METHOD_GICP && method != B2R_METHOD_NDT) return fail(B2R_EINVAL, "unknown method");
+  if (method != B2R_METHOD_GICP && !ndt_family(method)) return fail(B2R_EINVAL, "unknown method");
   return B2R_OK;
 }
 
@@ -160,6 +160,13 @@ extern "C" int b2r_select_registration_method(const char* const* keys, const cha
     std::string sm = s ? s : "DIRECT7";
     if (sm == "KDTREE") return fail(B2R_EUNSUPPORTED, "reg_nn_search_method=KDTREE is not re-created (DIRECT1/DIRECT7 only)");
     c.ndt_search_method = (sm == "DIRECT1") ? 1 : 7;  // registrations.cpp:112-118: anything else -> DIRECT7
+  } else if (method == "NDT") {
+    // registrations.cpp:93-100: pcl::NormalDistributionsTransform with transformation epsilon, maximum iterations and resolution;
+    // step size and outlier ratio stay PCL's defaults, and neither reg_nn_search_method nor reg_num_threads is read
+    b2r_config_default(&c, B2R_METHOD_NDT_PCL);
+    c.ndt_resolution = dparam("reg_resolution", 0.5);
+    c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
+    c.max_iterations = iparam("reg_maximum_iterations", 64);
   } else {
     return fail(B2R_EUNSUPPORTED, "registration_method '" + method + "' is not re-created by b200reg; keep the reference branch");
   }
@@ -175,7 +182,7 @@ static bool cluster16_allowed();
 extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
   if (!cfg || !out) return fail(B2R_EINVAL, "NULL argument");
   *out = nullptr;
-  if (cfg->method != B2R_METHOD_GICP && cfg->method != B2R_METHOD_NDT) return fail(B2R_EINVAL, "unknown method");
+  if (cfg->method != B2R_METHOD_GICP && !ndt_family(cfg->method)) return fail(B2R_EINVAL, "unknown method");
   if (cfg->k_correspondences < 1 || cfg->k_correspondences > 64) return fail(B2R_EINVAL, "k_correspondences must be in [1,64]");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -265,7 +272,7 @@ static int upload(b2r_handle* h, int which, const void* pts, size_t n, size_t st
   c.host_ptr = pts;  // identity of the caller's buffer (host or device): used to recognise a prefetched cloud
   c.invalidate();
   const size_t bytes = n * stride_bytes;
-  if (device_ptr && h->cfg.method == B2R_METHOD_NDT) {
+  if (device_ptr && ndt_family(h->cfg.method)) {
     // an NDT cloud's voxel map is built lazily, when the cloud has become the TARGET (possibly many calls later): the engine
     // keeps its own copy (device-to-device, ~1 us per MB) so the caller's buffer is free once the call that first uses it returns
     B2R_CUDA(c.raw.reserve(n * c.stride_f + 4));
@@ -1086,7 +1093,7 @@ extern "C" int b2r_gicp_error_at(b2r_handle* h, const double T[16], double* err)
 extern "C" int b2r_ndt_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int64_t* keys, int32_t* npts, double* mean,
                                   double* icov, int32_t min_b[3], int32_t div_b[3]) {
   if (!h || !n_voxels) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_NDT) return fail(B2R_ESTATE, "NDT engine required");
+  if (!ndt_family(h->cfg.method)) return fail(B2R_ESTATE, "NDT engine required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
   if (rc) return rc;
@@ -1095,7 +1102,7 @@ extern "C" int b2r_ndt_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxe
 
 extern "C" int b2r_ndt_derivatives_at(b2r_handle* h, const double p[6], double* score, double* g, double* H, uint64_t* n_pairs) {
   if (!h || !p || !score || !g || !H) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_NDT) return fail(B2R_ESTATE, "NDT engine required");
+  if (!ndt_family(h->cfg.method)) return fail(B2R_ESTATE, "NDT engine required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (SRC(h).n == 0 || TGT(h).n == 0) return fail(B2R_ESTATE, "source/target not set");
   int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
@@ -1107,7 +1114,7 @@ extern "C" int b2r_ndt_derivatives_at(b2r_handle* h, const double p[6], double* 
 
 extern "C" int b2r_ndt_hessian_at(b2r_handle* h, const double p[6], double* H) {
   if (!h || !p || !H) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_NDT) return fail(B2R_ESTATE, "NDT engine required");
+  if (!ndt_family(h->cfg.method)) return fail(B2R_ESTATE, "NDT engine required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (SRC(h).n == 0 || TGT(h).n == 0) return fail(B2R_ESTATE, "source/target not set");
   int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
@@ -1115,6 +1122,68 @@ extern "C" int b2r_ndt_hessian_at(b2r_handle* h, const double p[6], double* H) {
   rc = ensure_grid(h, SRC(h));
   if (rc) return rc;
   return ndt_hessian_at(h->cfg, SRC(h), TGT(h), h->ndt_work, h->st, p, H);
+}
+
+extern "C" int b2r_ndt_get_centroids(b2r_handle* h, size_t capacity, size_t* n_centroids, int64_t* keys, float* xyz) {
+  if (!h || !n_centroids) return fail(B2R_EINVAL, "NULL argument");
+  if (h->cfg.method != B2R_METHOD_NDT_PCL) return fail(B2R_ESTATE, "pcl NDT engine (B2R_METHOD_NDT_PCL) required");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
+  if (rc) return rc;
+  return ndt_pcl_dump_centroids(TGT(h), h->ndt_work, h->st, capacity, n_centroids, keys, xyz);
+}
+
+extern "C" int b2r_ndt_neighbors_at(b2r_handle* h, const double p[6], uint32_t* counts, size_t capacity, int64_t* keys, size_t* total) {
+  if (!h || !p || !total) return fail(B2R_EINVAL, "NULL argument");
+  if (h->cfg.method != B2R_METHOD_NDT_PCL) return fail(B2R_ESTATE, "pcl NDT engine (B2R_METHOD_NDT_PCL) required");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  *total = 0;
+  int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
+  if (rc) return rc;
+  NdtVoxelMap& M = *TGT(h).ndt;
+  rc = ndt_sync_geom(M, h->ndt_work, h->st);
+  if (rc) return rc;
+  Cloud& s = SRC(h);
+  const int n = (int)s.n;
+  if (n == 0) return B2R_OK;
+  float Tf[16];
+  ndt_pose_to_matrix(p, Tf);
+  NdtArgs A;
+  std::memset(&A, 0, sizeof(A));
+  A.geom = M.geom.p; A.vox = M.vox.p;
+  for (int i = 0; i < 12; i++) A.Tf[i] = Tf[i];
+  NdtPclArgs P;
+  ndt_pcl_fill_args(h->cfg, TGT(h), A, P);
+  DevBuf<unsigned int> d_counts;
+  DevBuf<unsigned long long> d_off;
+  B2R_CUDA(d_counts.alloc((size_t)n));
+  const unsigned nb = (unsigned)((n + 127) / 128);
+  k_ndt_pcl_neighbors<<<nb, 128, 0, h->st>>>(P, s.raw_view, s.stride_f, n, d_counts.p, nullptr, nullptr);
+  B2R_CUDA(cudaGetLastError());
+  std::vector<unsigned int> cnt((size_t)n);
+  B2R_CUDA(cudaMemcpyAsync(cnt.data(), d_counts.p, (size_t)n * sizeof(unsigned int), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaStreamSynchronize(h->st));
+  std::vector<unsigned long long> off((size_t)n + 1, 0);
+  for (int i = 0; i < n; i++) off[i + 1] = off[i] + cnt[i];
+  *total = (size_t)off[n];
+  if (counts) std::memcpy(counts, cnt.data(), (size_t)n * sizeof(uint32_t));
+  if (!keys || off[n] == 0) return B2R_OK;
+  DevBuf<int> d_pos;
+  B2R_CUDA(d_off.alloc((size_t)n));
+  B2R_CUDA(d_pos.alloc((size_t)off[n]));
+  B2R_CUDA(cudaMemcpyAsync(d_off.p, off.data(), (size_t)n * sizeof(unsigned long long), cudaMemcpyHostToDevice, h->st));
+  k_ndt_pcl_neighbors<<<nb, 128, 0, h->st>>>(P, s.raw_view, s.stride_f, n, d_counts.p, d_off.p, d_pos.p);
+  B2R_CUDA(cudaGetLastError());
+  std::vector<int> pos((size_t)off[n]);
+  std::vector<unsigned int> vkeys(M.n + 1);
+  B2R_CUDA(cudaMemcpyAsync(pos.data(), d_pos.p, pos.size() * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaMemcpyAsync(vkeys.data(), M.keys.p, M.n * sizeof(unsigned int), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaStreamSynchronize(h->st));
+  for (int i = 0; i < n; i++) {  // leaf keys ascending within each point (positions ascend with the keys)
+    std::sort(pos.begin() + off[i], pos.begin() + off[i + 1]);
+    for (unsigned long long t = off[i]; t < off[i + 1] && t < capacity; t++) keys[t] = (int64_t)vkeys[pos[t]];
+  }
+  return B2R_OK;
 }
 
 extern "C" int b2r_voxelgrid(b2r_handle* h, const void* in, size_t n, size_t stride_bytes, float leaf, void* out, size_t* n_out,

@@ -65,6 +65,8 @@ struct b2r_batch {
   DevBuf<char> ndt_ws;              // per pair in flight: chunk rows, group rows, counters, ticket counter; fitness partials
   DevBuf<NdtArgs> d_ndt_args;       // the round's pass records, grouped by pass kind
   PinnedBuf<NdtArgs> h_ndt_args;    // staging
+  DevBuf<NdtPclArgs> d_pcl_args;    // the same records with the radius-search inputs (B2R_METHOD_NDT_PCL)
+  PinnedBuf<NdtPclArgs> h_pcl_args;
   MappedBuf<double> h_ndt_msg;      // one result message per record of the round, then the round's flag (8 doubles)
   DevBuf<unsigned int> d_ndt_round; // messages of the current round (the last one publishes the flag and re-arms it)
   unsigned long long ndt_seq = 0;
@@ -91,7 +93,7 @@ extern "C" void b2r_batch_destroy(b2r_batch* b) { delete b; }
 extern "C" int b2r_batch_create(const b2r_config* cfg, b2r_batch** out) {
   if (!cfg || !out) return fail(B2R_EINVAL, "NULL argument");
   *out = nullptr;
-  if (cfg->method != B2R_METHOD_GICP && cfg->method != B2R_METHOD_NDT) return fail(B2R_EINVAL, "unknown method");
+  if (cfg->method != B2R_METHOD_GICP && !ndt_family(cfg->method)) return fail(B2R_EINVAL, "unknown method");
   std::unique_ptr<b2r_batch> b(new b2r_batch());
   b2r_handle* eng = nullptr;
   int rc = b2r_create(cfg, &eng);
@@ -471,6 +473,9 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
   b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
   const b2r_config& cfg = h->cfg;
+  // pcl::NormalDistributionsTransform: the Hessian-only pass is the derivative pass with the Hessian (ndt_run_pass)
+  const bool pcl = cfg.method == B2R_METHOD_NDT_PCL;
+  auto kind_of_pass = [&](int k) { return (pcl && k == NDT_PASS_HESS) ? (int)NDT_PASS_DERIV_HESS : k; };
   std::vector<NdtPairState> S(m);
   std::vector<size_t> active, off(m, 0), fit_off(m, 0);
   size_t ws = 0;
@@ -495,6 +500,7 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
   B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
   B2R_CUDA(b->d_ndt_args.reserve(m));
   B2R_CUDA(b->h_ndt_args.alloc(m));
+  if (pcl) { B2R_CUDA(b->d_pcl_args.reserve(m)); B2R_CUDA(b->h_pcl_args.alloc(m)); }
   if (b->h_ndt_msg.cap < m * kNdtMsg + 8) {
     B2R_CUDA(b->h_ndt_msg.alloc(m * kNdtMsg + 8));
     std::memset(b->h_ndt_msg.p, 0, b->h_ndt_msg.cap * sizeof(double));
@@ -511,7 +517,7 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
     unsigned max_nb[3] = {0, 0, 0};
     for (int k = 0; k < 3; k++)
       for (size_t i : active)
-        if (S[i].next() == k) {
+        if (S[i].next() != NDT_PASS_DONE && kind_of_pass(S[i].next()) == k) {
           order.push_back(i); kind_of.push_back(k); cnt[k]++;
           max_nb[k] = std::max(max_nb[k], (unsigned)((size_t)b->clouds[pairs[i].source]->nsup * 1024 / kNdtThreads));
         }
@@ -519,7 +525,10 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
     // pair's blocks draw its chunks from its own ticket counter, so any count gives the same sums
     unsigned G[3] = {0, 0, 0};
     for (int k = 0; k < 2; k++)
-      if (cnt[k]) G[k] = std::max(1u, std::min(max_nb[k], (unsigned)((4ull * ndt_resident_blocks(k == 0) + cnt[k] - 1) / cnt[k])));
+      if (cnt[k]) {
+        const unsigned res = pcl ? ndt_pcl_resident_blocks(k == 0) : ndt_resident_blocks(k == 0);
+        G[k] = std::max(1u, std::min(max_nb[k], (unsigned)((4ull * res + cnt[k] - 1) / cnt[k])));
+      }
     G[2] = max_nb[2];
     const unsigned long long seq = ++b->ndt_seq;
     for (size_t r = 0; r < order.size(); r++) {
@@ -544,15 +553,23 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       A.seq = seq;
       A.round = b->d_ndt_round.p;
       A.round_n = (unsigned)order.size();
+      if (pcl) ndt_pcl_fill_args(cfg, t, A, b->h_pcl_args.p[r]);
     }
-    B2R_CUDA(cudaMemcpyAsync(b->d_ndt_args.p, b->h_ndt_args.p, order.size() * sizeof(NdtArgs), cudaMemcpyHostToDevice, st));
-    h->tel.h2d += order.size() * sizeof(NdtArgs);
+    if (pcl) {
+      B2R_CUDA(cudaMemcpyAsync(b->d_pcl_args.p, b->h_pcl_args.p, order.size() * sizeof(NdtPclArgs), cudaMemcpyHostToDevice, st));
+      h->tel.h2d += order.size() * sizeof(NdtPclArgs);
+    } else {
+      B2R_CUDA(cudaMemcpyAsync(b->d_ndt_args.p, b->h_ndt_args.p, order.size() * sizeof(NdtArgs), cudaMemcpyHostToDevice, st));
+      h->tel.h2d += order.size() * sizeof(NdtArgs);
+    }
     size_t r0 = 0;
     for (int k = 0; k < 3; k++) {
       if (!cnt[k]) continue;
       const dim3 grid(G[k], (unsigned)cnt[k]);
       TEL_BEGIN(&h->tel, st);
-      if (k == NDT_PASS_DERIV_HESS) k_ndt_derivatives_batch<true><<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
+      if (pcl && k == NDT_PASS_DERIV_HESS) k_ndt_pcl_derivatives_batch<true><<<grid, kNdtThreads, 0, st>>>(b->d_pcl_args.p + r0);
+      else if (pcl) k_ndt_pcl_derivatives_batch<false><<<grid, kNdtThreads, 0, st>>>(b->d_pcl_args.p + r0);
+      else if (k == NDT_PASS_DERIV_HESS) k_ndt_derivatives_batch<true><<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
       else if (k == NDT_PASS_DERIV) k_ndt_derivatives_batch<false><<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
       else k_ndt_hessian_batch<<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
       TEL_END(&h->tel, k == NDT_PASS_HESS ? KC_NDT_HESS : KC_NDT_DERIV, 1, st);
@@ -639,7 +656,7 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   if (rc) return rc;
   std::vector<int32_t> named(2 * n_pairs);
   for (size_t i = 0; i < n_pairs; i++) { named[2 * i] = pairs[i].source; named[2 * i + 1] = pairs[i].target; }
-  const bool ndt = h->cfg.method == B2R_METHOD_NDT;
+  const bool ndt = ndt_family(h->cfg.method);
   rc = batch_build_structures(b, named.data(), named.size(), !fit_only && !ndt);
   if (rc) return rc;
   if (ndt) rc = batch_ndt_maps(b, pairs, n_pairs, fit_only);

@@ -58,7 +58,16 @@ struct NdtVoxelMap {
   DevBuf<unsigned long long> table;  // (pos << 32) | key, kNdtEmpty = free
   unsigned int mask = 0;
   size_t n = 0;
+  // B2R_METHOD_NDT_PCL targets only (ndt_pcl.cuh): the leaf centroids and their bucket CSR
+  DevBuf<float4> cent;                   // per sorted position of a voxel's first point: its centroid (x, y, z, bits(position))
+  DevBuf<unsigned long long> bkey, bkey_sorted;  // bucket key per position (kPclNoBucket: no centroid there), and sorted
+  DevBuf<int> bpos_in, bpos;             // positions, and positions in bucket order
+  DevBuf<unsigned long long> btab_key;   // bucket key -> slot
+  DevBuf<uint2> btab_val;                // slot -> (first index into bpos, count)
+  unsigned int bmask = 0;
 };
+
+inline bool ndt_family(int method) { return method == B2R_METHOD_NDT || method == B2R_METHOD_NDT_PCL; }
 
 struct NdtWork {
   DevBuf<double> partials;
@@ -626,6 +635,10 @@ __global__ void __launch_bounds__(kNdtThreads) k_ndt_hessian_batch(const NdtArgs
   ndt_hessian_body(A, nb);
 }
 
+}  // namespace b2r
+#include "ndt_pcl.cuh"
+namespace b2r {
+
 // ------------------------------------------------------------------------------------------------ host side
 inline int ndt_init_work(NdtWork& W) {
   if (W.d_out.p) return B2R_OK;
@@ -685,6 +698,10 @@ inline int ndt_ensure_map(const b2r_config& cfg, Cloud& c, NdtWork& W, cudaStrea
     B2R_CUDA(cub::DeviceRadixSort::SortPairs(B->sort_tmp.p, tb, B->keys_a.p, M.keys.p, B->vals_a.p, B->vals_b.p, n, 0, 32, st));
     k_vox_gather<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, n, M.keys.p, B->vals_b.p, M.sorted.p);
     k_vox_finalize<<<(n + 127) / 128, 128, 0, st>>>(M.keys.p, M.sorted.p, M.vox.p, M.cells.p, M.table.p, M.mask, n);
+  }
+  if (cfg.method == B2R_METHOD_NDT_PCL) {
+    int rc2 = ndt_pcl_build(M, B, n, st);
+    if (rc2) return rc2;
   }
   TEL_END(W.tel, KC_NDT_BUILD, n > 0 ? 10 : 4, st);
   B2R_CUDA(cudaGetLastError());
@@ -967,6 +984,28 @@ inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& 
   A.partials = W.partials.p; A.grows = W.grows.p; A.gcount = W.gcount.p; A.queue = W.d_queue.p; A.qbase = 0;
   A.out = W.h_out.d; A.counter = W.d_counter.p; A.pairs = W.d_pairs.p;
   A.flag = W.h_flag_dev; A.seq = ++W.seq;
+  if (cfg.method == B2R_METHOD_NDT_PCL) {
+    // computeHessian's term is updateDerivatives' Hessian term: the Hessian-only pass is the derivative kernel with the Hessian,
+    // of which the driver reads H alone
+    const bool hess = compute_hessian || hessian_only;
+    NdtPclArgs P;
+    ndt_pcl_fill_args(cfg, tgt, A, P);
+    { TEL_BEGIN(W.tel, st);
+      const unsigned ng = std::min(nb, ndt_pcl_resident_blocks(hess));
+      P.A.qbase = W.qnext;
+      W.qnext += (unsigned long long)nb + ng;
+      if (hess) k_ndt_pcl_derivatives<true><<<ng, kNdtThreads, 0, st>>>(P);
+      else k_ndt_pcl_derivatives<false><<<ng, kNdtThreads, 0, st>>>(P);
+      TEL_END(W.tel, hessian_only ? KC_NDT_HESS : KC_NDT_DERIV, 1, st);
+      if (cudaPeekAtLastError() != cudaSuccess) W.qnext = P.A.qbase;
+    }
+    if (W.tel) W.tel->d2h += kNdtAcc * sizeof(double) + 8;
+    B2R_CUDA(cudaGetLastError());
+    int rc = wait_host_result(W.h_flag, A.seq, W.h_out.p, kNdtAcc, true, st);
+    if (rc) return rc;
+    ndt_read_pass(W.h_out.p, hess, false, out);
+    return B2R_OK;
+  }
   if (hessian_only) {
     { TEL_BEGIN(W.tel, st);
       k_ndt_hessian<<<nb, kNdtThreads, 0, st>>>(A);

@@ -18,7 +18,7 @@ library; nothing here computes.
 import ctypes as C
 import numpy as np
 from . import _capi
-from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT
+from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL  # noqa: F401
 
 
 def _cloud(a):
@@ -234,6 +234,28 @@ class Registration:
         dp = C.POINTER(C.c_double)
         check(self._lib.b2r_ndt_hessian_at(self._h, p.ctypes.data_as(dp), H.ctypes.data_as(dp)))
         return H
+
+    def ndtGetCentroids(self):
+        """(pcl NDT) the searchable centroid cloud of the target: (leaf keys (m,) int64 ascending, centroids (m, 3) float32)"""
+        nc = C.c_size_t()
+        check(self._lib.b2r_ndt_get_centroids(self._h, 0, C.byref(nc), None, None))
+        keys = np.empty(nc.value, np.int64)
+        xyz = np.empty((nc.value, 3), np.float32)
+        check(self._lib.b2r_ndt_get_centroids(self._h, nc.value, C.byref(nc), keys.ctypes.data_as(C.POINTER(C.c_int64)),
+                                              xyz.ctypes.data_as(C.POINTER(C.c_float))))
+        return keys, xyz
+
+    def ndtNeighborsAt(self, p, n_source):
+        """(pcl NDT) radius neighbours of every source point at p: (counts (n,) uint32, leaf keys (sum counts,) int64, CSR)"""
+        p = np.ascontiguousarray(p, np.float64)
+        dp = C.POINTER(C.c_double)
+        counts = np.zeros(max(n_source, 1), np.uint32)
+        total = C.c_size_t()
+        check(self._lib.b2r_ndt_neighbors_at(self._h, p.ctypes.data_as(dp), counts.ctypes.data_as(C.POINTER(C.c_uint32)), 0, None, C.byref(total)))
+        keys = np.empty(max(total.value, 1), np.int64)
+        check(self._lib.b2r_ndt_neighbors_at(self._h, p.ctypes.data_as(dp), counts.ctypes.data_as(C.POINTER(C.c_uint32)), total.value,
+                                             keys.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(total)))
+        return counts[:n_source], keys[:total.value]
 
     # --- companion / prefilter chain
     def _filter(self, fn, cloud, *args):

@@ -46,6 +46,9 @@ extern "C" {
 
 #define B2R_METHOD_GICP 0 /* fast_gicp::FastGICP semantics   (registrations.cpp:27-36)   */
 #define B2R_METHOD_NDT 1  /* pclomp::NormalDistributionsTransform semantics (registrations.cpp:101-120) */
+#define B2R_METHOD_NDT_PCL 2 /* pcl::NormalDistributionsTransform semantics (registrations.cpp:93-100): radius neighbourhood over the
+                                voxel centroids, float64 derivatives; reads ndt_resolution / ndt_step_size / ndt_outlier_ratio /
+                                ndt_mt_interval_flag / ndt_fixed_iterations, not ndt_search_method */
 
 typedef struct b2r_handle b2r_handle;
 
@@ -84,8 +87,8 @@ int b2r_config_default(b2r_config* cfg, int method);
 
 /* replaces select_registration_method(ros::NodeHandle&) (registrations.cpp:22-124): same parameter NAMES and defaults,
  * passed as string key/value pairs (the rosparam namespace of the nodelet).  "FAST_GICP"/"B200_GICP" -> GICP engine,
- * "NDT_OMP"/"B200_NDT" -> NDT engine.  ICP / GICP / GICP_OMP / NDT(pcl) / FAST_VGICP[_CUDA] are not re-created:
- * returns B2R_EUNSUPPORTED so the caller keeps the reference's own branch. */
+ * "NDT_OMP"/"B200_NDT" -> NDT engine, "NDT" -> pcl NDT engine (B2R_METHOD_NDT_PCL).  ICP / GICP / GICP_OMP / FAST_VGICP[_CUDA]
+ * and unknown names are not re-created: returns B2R_EUNSUPPORTED so the caller keeps the reference's own branch. */
 int b2r_select_registration_method(const char* const* keys, const char* const* values, int n_params, int device_id,
                                    b2r_handle** out);
 
@@ -154,13 +157,21 @@ int b2r_get_covariances(b2r_handle* h, int which, double* out, size_t n);
 int b2r_gicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* err);
 /* one compute_error at pose T with the correspondences of the last linearisation */
 int b2r_gicp_error_at(b2r_handle* h, const double T[16], double* err);
-/* NDT voxel table of the target: returns count through *n_voxels; arrays may be NULL.  keys ascending. */
+/* NDT voxel table of the target (either NDT method): returns count through *n_voxels; arrays may be NULL.  keys ascending. */
 int b2r_ndt_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int64_t* keys, int32_t* npts, double* mean, double* icov,
                        int32_t min_b[3], int32_t div_b[3]);
-/* one computeDerivatives pass at p = (tx,ty,tz,rx,ry,rz): score, g[6], H[36] row-major, number of (point,cell) pairs */
+/* one computeDerivatives pass at p = (tx,ty,tz,rx,ry,rz): score, g[6], H[36] row-major, number of (point,cell) pairs
+ * (B2R_METHOD_NDT_PCL: (point, radius neighbour) pairs) */
 int b2r_ndt_derivatives_at(b2r_handle* h, const double p[6], double* score, double* g, double* H, uint64_t* n_pairs);
 /* one float64 computeHessian pass at p (the pass the align runs after an active More-Thuente line search): H[36] row-major */
 int b2r_ndt_hessian_at(b2r_handle* h, const double p[6], double* H);
+/* B2R_METHOD_NDT_PCL: the searchable centroid cloud of the target (VoxelGridCovariance::filter(true)): the leaf key and float32
+ * centroid (xyz: 3 floats each) of every leaf with at least 6 points, keys ascending; *n_centroids = the count; arrays may be NULL */
+int b2r_ndt_get_centroids(b2r_handle* h, size_t capacity, size_t* n_centroids, int64_t* keys, float* xyz);
+/* B2R_METHOD_NDT_PCL: the radiusSearch(T(p) x, resolution) of every source point, in the caller's point order: counts[i] (n source
+ * entries, may be NULL) and one flat array of the neighbours' leaf keys, ascending within each point (CSR by counts; the first
+ * `capacity` entries are written, keys may be NULL); *total = the number of (point, neighbour) pairs */
+int b2r_ndt_neighbors_at(b2r_handle* h, const double p[6], uint32_t* counts, size_t capacity, int64_t* keys, size_t* total);
 
 /* ---- companion: voxel-grid downsample ---------------------------------------------------------------------------
  * replaces pcl::VoxelGrid<PointXYZI>::filter with setLeafSize(leaf,leaf,leaf) (apps/prefiltering_nodelet.cpp:54-58,138-149;
