@@ -102,9 +102,10 @@ public:
   ~B200Registration() override { b2r_destroy(h_); }
 
   void setInputSource(const PointCloudSourceConstPtr& cloud) override {
-    if (cloud == this->input_) return;  // same early-out as fast_gicp
+    if (cloud == this->input_ && !source_promoted_) return;  // same early-out as fast_gicp
     Base::setInputSource(cloud);
     cache_valid_ = false;
+    source_promoted_ = false;
     b2r_set_source(h_, cloud->points.data(), cloud->points.size(), sizeof(PointT));
   }
 
@@ -113,7 +114,8 @@ public:
     const bool promote = (cloud == this->input_);  // keyframe switch: the last source becomes the target (:245-246)
     Base::setInputTarget(cloud);
     cache_valid_ = false;
-    if (promote) b2r_promote_source_to_target(h_);
+    // the engine has no source after a promotion (b200reg.h): the same cloud set as the source again is uploaded, not skipped
+    if (promote) source_promoted_ = b2r_promote_source_to_target(h_) == B2R_OK;
     else b2r_set_target(h_, cloud->points.data(), cloud->points.size(), sizeof(PointT));
   }
 
@@ -148,6 +150,7 @@ protected:
 private:
   b2r_handle* h_ = nullptr;
   // nearest-neighbour cache of the transformed source (see cachedNearest)
+  bool source_promoted_ = false;
   bool cache_valid_ = false;
   size_t cache_cursor_ = 0;
   PointCloudSource cache_cloud_;

@@ -2,6 +2,7 @@
 // adapter can be syntax-checked in an image without PCL (tests/test_adapter_syntax.py).  Signatures follow PCL 1.10
 // (the distro package of ROS noetic, /root/reference/docker/noetic/Dockerfile:6).  Nothing here is shipped or linked.
 #pragma once
+#include <limits>
 #include <memory>
 #include <string>
 #include <vector>
@@ -11,6 +12,11 @@ struct Matrix4f {
   float m[16];
   float* data() { return m; }
   const float* data() const { return m; }
+  static Matrix4f Identity() {
+    Matrix4f I{};
+    for (int i = 0; i < 4; i++) I.m[i * 5] = 1.f;
+    return I;
+  }
 };
 }  // namespace Eigen
 
@@ -48,6 +54,9 @@ protected:
 };
 }  // namespace search
 
+template <typename PointT>
+void transformPointCloud(const PointCloud<PointT>& in, PointCloud<PointT>& out, const Eigen::Matrix4f& T);
+
 template <typename PointSource, typename PointTarget, typename Scalar = float>
 class Registration {
 public:
@@ -65,6 +74,25 @@ public:
   KdTreePtr getSearchMethodTarget() const { return tree_; }
   bool hasConverged() const { return converged_; }
   Matrix4 getFinalTransformation() { return final_transformation_; }
+  // pcl::Registration::getFitnessScore(max_range) as documented: the source transformed by the final transformation, one
+  // nearestKSearch(p, 1) per point in order, the mean of the squared distances that are <= max_range, DBL_MAX when there is none.
+  // NOT virtual, as in PCL: both reference callers reach it through the base pointer.
+  double getFitnessScore(double max_range = std::numeric_limits<double>::max()) {
+    double fitness_score = 0.0;
+    PointCloudSource input_transformed;
+    transformPointCloud(*input_, input_transformed, final_transformation_);
+    std::vector<int> nn_indices(1);
+    std::vector<float> nn_dists(1);
+    int nr = 0;
+    for (size_t i = 0; i < input_transformed.points.size(); ++i) {
+      tree_->nearestKSearch(input_transformed.points[i], 1, nn_indices, nn_dists);
+      if (nn_dists[0] <= max_range) {
+        fitness_score += nn_dists[0];
+        nr++;
+      }
+    }
+    return nr > 0 ? fitness_score / nr : std::numeric_limits<double>::max();
+  }
   void align(PointCloudSource& output, const Matrix4& guess) {
     output.points = input_->points;
     converged_ = false;
@@ -78,7 +106,7 @@ protected:
   PointCloudSourceConstPtr input_;
   PointCloudTargetConstPtr target_;
   int nr_iterations_ = 0, max_iterations_ = 10;
-  Matrix4 final_transformation_, transformation_, previous_transformation_;
+  Matrix4 final_transformation_ = Matrix4::Identity(), transformation_ = Matrix4::Identity(), previous_transformation_ = Matrix4::Identity();
   double transformation_epsilon_ = 0, corr_dist_threshold_ = 0;
   bool converged_ = false, target_cloud_updated_ = true, force_no_recompute_ = false;
 };

@@ -30,6 +30,7 @@
 #include "map_cloud.cuh"
 #include "ingest.cuh"
 #include "loop_gate.cuh"
+#include "odometry_gate.cuh"
 
 #ifndef B2R_PREFETCH_KNN_BLOCKS_DEFAULT
 #define B2R_PREFETCH_KNN_BLOCKS_DEFAULT 0  // 0 = no cap on the prefetch stream's k-NN kernel
@@ -98,6 +99,7 @@ struct b2r_handle {
   float final_T[16];                // row-major
   bool has_final = false;
   bool corr_valid = false;
+  bool src_promoted = false;        // b2r_promote_source_to_target has taken the source away: no source until the next b2r_set_source*
   NdtWork ndt_work;
   VoxelWork vg_work;
   Telemetry tel;
@@ -533,6 +535,12 @@ static unsigned long long content_stamp(const void* pts, size_t n, size_t stride
   return x;
 }
 
+// b2r_align / b2r_fitness / b2r_get_aligned after b2r_promote_source_to_target and before a new source: refused, never served from
+// the slot the promotion left behind
+static int need_source(b2r_handle* h) {
+  return h->src_promoted ? fail(B2R_ESTATE, "no source cloud: it was promoted to target, set a new source first") : B2R_OK;
+}
+
 static int set_cloud(b2r_handle* h, bool is_target, const void* pts, size_t n, size_t stride, bool dev) {
   if (!h) return fail(B2R_EINVAL, "handle is NULL");
   if (!is_target && h->prefetched) {
@@ -545,6 +553,7 @@ static int set_cloud(b2r_handle* h, bool is_target, const void* pts, size_t n, s
       std::swap(h->src, h->nxt);
       B2R_CUDA(cudaStreamWaitEvent(h->st, h->ev_prefetch, 0));
       h->corr_valid = false;
+      h->src_promoted = false;
       return B2R_OK;
     }
   }
@@ -553,6 +562,7 @@ static int set_cloud(b2r_handle* h, bool is_target, const void* pts, size_t n, s
   int rc = upload(h, which, pts, n, stride, dev, h->st);
   if (rc) return rc;
   h->corr_valid = false;
+  if (!is_target) h->src_promoted = false;
   rc = preprocess(h, which, is_target);  // the structure builds are enqueued behind the copy before the host waits for it
   if (h->upload_pending) {
     // the caller keeps ownership of its (pinned) buffer: the copy out of it has finished when this call returns
@@ -626,9 +636,12 @@ extern "C" int b2r_get_stats(b2r_handle* h, b2r_stats* out, int reset) {
 extern "C" int b2r_promote_source_to_target(b2r_handle* h) {
   if (!h) return fail(B2R_EINVAL, "handle is NULL");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (h->src_promoted) return fail(B2R_ESTATE, "the source has already been promoted: set a new source first");
   std::swap(h->src, h->tgt);
   h->corr_valid = false;
-  // the old target becomes a stale source: callers always set a new source before the next align
+  // the source slot now holds the OLD target, whose raw records may be the caller's released device memory: it is not a source
+  // (need_source) until b2r_set_source* fills the slot again
+  h->src_promoted = true;
   return preprocess(h, h->tgt, true);
 }
 
@@ -888,8 +901,9 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out, const 
 static int align_impl(b2r_handle* h, const float guess[16], b2r_result* out, const std::function<int()>* between) {
   if (!h || !guess) return fail(B2R_EINVAL, "NULL argument");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
-  int rc;
-  if (h->cfg.method == B2R_METHOD_GICP) rc = gicp_align(h, guess, out, between);
+  int rc = need_source(h);
+  if (rc != B2R_OK) {}  // reported below like every failed align
+  else if (h->cfg.method == B2R_METHOD_GICP) rc = gicp_align(h, guess, out, between);
   else {
     float Tfinal[16];
     bool conv = false;
@@ -912,6 +926,8 @@ extern "C" int b2r_get_aligned(b2r_handle* h, void* out_points, size_t n, size_t
   if (!h || (!out_points && n)) return fail(B2R_EINVAL, "NULL argument");
   if (stride_bytes < 12 || (stride_bytes & 3)) return fail(B2R_EINVAL, "bad stride");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  int rc = need_source(h);
+  if (rc) return rc;
   Cloud& s = SRC(h);
   if (n != s.n) return fail(B2R_EINVAL, "n does not match the source cloud");
   if (n == 0) return B2R_OK;
@@ -973,6 +989,8 @@ extern "C" int b2r_fitness(b2r_handle* h, const float* T, double max_range, floa
                            uint32_t* n_inliers) {
   if (!h) return fail(B2R_EINVAL, "handle is NULL");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  const int src_rc = need_source(h);
+  if (src_rc) return src_rc;
   float Tr[16];
   if (T) {
     for (int r = 0; r < 4; r++)
@@ -1011,6 +1029,7 @@ extern "C" int b2r_target_nearest(b2r_handle* h, const void* queries, size_t n, 
 extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
   if (!h || !out) return fail(B2R_EINVAL, "NULL argument");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (need_source(h)) return B2R_ESTATE;
   if (!h->corr_valid) return fail(B2R_ESTATE, "no linearisation has run since the clouds were set");
   if (n != SRC(h).n) return fail(B2R_EINVAL, "n does not match the source cloud");
   // a non-finite source point is not in the source's search structure (pos_of = -1): no search writes its entry, and like a PCL
@@ -1028,6 +1047,7 @@ extern "C" int b2r_get_covariances(b2r_handle* h, int which, double* out, size_t
   if (!h || !out) return fail(B2R_EINVAL, "NULL argument");
   if (h->cfg.method != B2R_METHOD_GICP) return fail(B2R_ESTATE, "covariances exist only for the GICP engine");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (!which && need_source(h)) return B2R_ESTATE;
   Cloud& c = which ? TGT(h) : SRC(h);
   if (n != c.n) return fail(B2R_EINVAL, "n does not match the cloud");
   int rc = ensure_cov(h, c);
@@ -1051,6 +1071,7 @@ extern "C" int b2r_gicp_linearize_at(b2r_handle* h, const double T[16], double* 
   if (!h || !T || !H || !b || !err) return fail(B2R_EINVAL, "NULL argument");
   if (h->cfg.method != B2R_METHOD_GICP) return fail(B2R_ESTATE, "GICP engine required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (need_source(h)) return B2R_ESTATE;
   Cloud& s = SRC(h);
   Cloud& t = TGT(h);
   if (s.n == 0 || t.n == 0) return fail(B2R_ESTATE, "source/target not set");
@@ -1104,6 +1125,7 @@ extern "C" int b2r_ndt_derivatives_at(b2r_handle* h, const double p[6], double* 
   if (!h || !p || !score || !g || !H) return fail(B2R_EINVAL, "NULL argument");
   if (!ndt_family(h->cfg.method)) return fail(B2R_ESTATE, "NDT engine required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (need_source(h)) return B2R_ESTATE;
   if (SRC(h).n == 0 || TGT(h).n == 0) return fail(B2R_ESTATE, "source/target not set");
   int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
   if (rc) return rc;
@@ -1116,6 +1138,7 @@ extern "C" int b2r_ndt_hessian_at(b2r_handle* h, const double p[6], double* H) {
   if (!h || !p || !H) return fail(B2R_EINVAL, "NULL argument");
   if (!ndt_family(h->cfg.method)) return fail(B2R_ESTATE, "NDT engine required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (need_source(h)) return B2R_ESTATE;
   if (SRC(h).n == 0 || TGT(h).n == 0) return fail(B2R_ESTATE, "source/target not set");
   int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
   if (rc) return rc;
@@ -1138,6 +1161,7 @@ extern "C" int b2r_ndt_neighbors_at(b2r_handle* h, const double p[6], uint32_t* 
   if (h->cfg.method != B2R_METHOD_NDT_PCL) return fail(B2R_ESTATE, "pcl NDT engine (B2R_METHOD_NDT_PCL) required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   *total = 0;
+  if (need_source(h)) return B2R_ESTATE;
   int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
   if (rc) return rc;
   NdtVoxelMap& M = *TGT(h).ndt;
@@ -1757,43 +1781,7 @@ static bool odometry_downsamples(const b2r_odometry_params& p) {
 }
 
 static void mat4_identity(float* m) { for (int i = 0; i < 16; i++) m[i] = (i % 5 == 0) ? 1.f : 0.f; }
-static void mat4_mul(const float* a, const float* b, float* o) {
-  float t[16];
-  for (int r = 0; r < 4; r++)
-    for (int c = 0; c < 4; c++) {
-      float s = a[r * 4 + 0] * b[0 * 4 + c];
-      s += a[r * 4 + 1] * b[1 * 4 + c];
-      s += a[r * 4 + 2] * b[2 * 4 + c];
-      s += a[r * 4 + 3] * b[3 * 4 + c];
-      t[r * 4 + c] = s;
-    }
-  std::memcpy(o, t, sizeof(t));
-}
-static void mat4_inv_rigid_general(const float* m, float* o) {
-  // general affine inverse of [A t; 0 1] with A 3x3 (Eigen Matrix4f::inverse() on a rigid transform)
-  double A[9] = {m[0], m[1], m[2], m[4], m[5], m[6], m[8], m[9], m[10]}, Ai[9];
-  inv3(A, Ai);
-  for (int r = 0; r < 3; r++) {
-    for (int c = 0; c < 3; c++) o[r * 4 + c] = (float)Ai[r * 3 + c];
-    o[r * 4 + 3] = (float)(-(Ai[r * 3 + 0] * m[3] + Ai[r * 3 + 1] * m[7] + Ai[r * 3 + 2] * m[11]));
-  }
-  o[12] = o[13] = o[14] = 0.f; o[15] = 1.f;
-}
-// w of Eigen::Quaternionf(R) (rotation matrix -> quaternion, Eigen's branchy algorithm)
-static float quat_w_from_R(const float* m) {
-  float t = m[0] + m[5] + m[10];
-  if (t > 0.f) {
-    t = std::sqrt(t + 1.0f);
-    return 0.5f * t;
-  }
-  int i = 0;
-  if (m[5] > m[0]) i = 1;
-  if (m[10] > m[i * 4 + i]) i = 2;
-  int j = (i + 1) % 3, k = (j + 1) % 3;
-  t = std::sqrt(m[i * 4 + i] - m[j * 4 + j] - m[k * 4 + k] + 1.0f);
-  t = 0.5f / t;
-  return (m[k * 4 + j] - m[j * 4 + k]) * t;
-}
+// mat4_mul, the rigid inverse, Eigen's matrix -> quaternion w and the frame decisions live in odometry_gate.cuh (host only, unit-tested)
 static void row_to_col(const float* r, float* c) {
   for (int i = 0; i < 4; i++)
     for (int j = 0; j < 4; j++) c[j * 4 + i] = r[i * 4 + j];
@@ -2005,46 +1993,25 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
     out->matching_error = score;
     out->inlier_fraction = n_reg ? (float)inl / (float)n_reg : 0.f;
   }
-  float odom_row[16];
-  if (!res.converged) {  // :214-218
-    mat4_mul(o->keyframe_pose, o->prev_trans, odom_row);
-    row_to_col(odom_row, out->odom);
+  float trans[16], odom_row[16];
+  for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) trans[r * 4 + c] = res.T[c * 4 + r];
+  const OdometryDecision d = odometry_gate(o->p, o->keyframe_pose, o->prev_trans, trans, res.converged != 0, stamp, o->keyframe_stamp, odom_row);
+  row_to_col(odom_row, out->odom);
+  if (d == ODOM_REJECTED) {  // :214-218, :223-233: prev_trans, prev_time and the keyframe stay as they are
     out->frame_rejected = 1;
     return B2R_OK;
   }
-  float trans[16];
-  for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) trans[r * 4 + c] = res.T[c * 4 + r];
-  mat4_mul(o->keyframe_pose, trans, odom_row);
-  if (o->p.transform_thresholding) {  // :223-233
-    float inv[16], delta[16];
-    mat4_inv_rigid_general(o->prev_trans, inv);
-    mat4_mul(inv, trans, delta);
-    double dx = std::sqrt((double)delta[3] * delta[3] + (double)delta[7] * delta[7] + (double)delta[11] * delta[11]);
-    double da = std::acos((double)quat_w_from_R(delta));
-    if (dx > o->p.max_acceptable_trans || da > o->p.max_acceptable_angle) {
-      mat4_mul(o->keyframe_pose, o->prev_trans, odom_row);
-      row_to_col(odom_row, out->odom);
-      out->frame_rejected = 1;
-      return B2R_OK;
-    }
-  }
-  o->prev_time = stamp;
+  o->prev_time = stamp;  // :235-236
   o->prev_time_zero = false;
   std::memcpy(o->prev_trans, trans, sizeof(trans));
-  float tn = std::sqrt(trans[3] * trans[3] + trans[7] * trans[7] + trans[11] * trans[11]);
-  double delta_trans = tn;
-  double delta_angle = std::acos((double)quat_w_from_R(trans));
-  double delta_time = stamp - o->keyframe_stamp;
-  if (delta_trans > o->p.keyframe_delta_trans || delta_angle > o->p.keyframe_delta_angle || delta_time > o->p.keyframe_delta_time) {  // :241-252
+  if (d == ODOM_KEYFRAME) {  // :241-252
     rc = b2r_promote_source_to_target(reg);  // keyframe = filtered; registration->setInputTarget(keyframe)
     if (rc) return rc;
     std::memcpy(o->keyframe_pose, odom_row, sizeof(odom_row));
     o->keyframe_stamp = stamp;
-    o->prev_time = stamp;
     mat4_identity(o->prev_trans);
     out->keyframe_updated = 1;
   }
-  row_to_col(odom_row, out->odom);
   return B2R_OK;
 }
 

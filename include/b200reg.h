@@ -127,7 +127,12 @@ int b2r_prefetch_source_device(b2r_handle* h, const void* d_points, size_t n, si
 /* block until everything enqueued on the handle's stream (uploads, grid / covariance / voxel builds) has finished */
 int b2r_synchronize(b2r_handle* h);
 /* keyframe switch `keyframe = filtered; registration->setInputTarget(keyframe)` (scan_matching_odometry_nodelet.cpp:245-246):
- * the current source (points, grid, covariances) becomes the target without re-upload or recomputation. */
+ * the current source (points, grid, covariances) becomes the target without re-upload or recomputation.
+ * Afterwards the handle has NO source until the next b2r_set_source* (or an adopted prefetch): b2r_align (which reports converged = 0
+ * and the guess, like every failed align), b2r_fitness, b2r_get_aligned, a second b2r_promote_source_to_target and every parity tap
+ * that reads the source (b2r_get_correspondences, b2r_get_covariances with which = 0, b2r_gicp_linearize_at, b2r_ndt_derivatives_at,
+ * b2r_ndt_hessian_at, b2r_ndt_neighbors_at) return B2R_ESTATE.
+ * The displaced target's records are never read again, so a target registered from device memory may be released by its owner. */
 int b2r_promote_source_to_target(b2r_handle* h);
 
 /* replaces registration->align(*aligned, guess) + hasConverged() + getFinalTransformation()
@@ -135,7 +140,8 @@ int b2r_promote_source_to_target(b2r_handle* h);
 int b2r_align(b2r_handle* h, const float guess[16], b2r_result* out);
 
 /* the `aligned` output cloud of align(): source transformed by the final pose.  Writes x,y,z (and 1.0f at offset 12 when
- * stride_bytes >= 16) of n records; other bytes are left untouched. */
+ * stride_bytes >= 16) of n records; other bytes are left untouched.  n must be the source's size (B2R_EINVAL otherwise).  The pose is
+ * the last successful align's (identity before any; an align that returned an error leaves it as it was). */
 int b2r_get_aligned(b2r_handle* h, void* out_points, size_t n, size_t stride_bytes);
 
 /* replaces registration->getFitnessScore(max_range) (scan_matching_odometry_nodelet.cpp:307; loop_detector.hpp:146;
