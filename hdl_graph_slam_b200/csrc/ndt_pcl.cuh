@@ -395,6 +395,7 @@ inline unsigned ndt_pcl_resident_blocks(bool hess) {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     if (hess) cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_ndt_pcl_derivatives<true>, kNdtThreads, 0);
     else cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per, k_ndt_pcl_derivatives<false>, kNdtThreads, 0);
+    if (const char* e = getenv("B2R_NDT_WAVES")) { const double w = atof(e); if (w > 0) per = std::max(1, (int)(per * w)); }
     c = (unsigned)std::max(1, sms * std::max(per, 1));
   }
   return c;

@@ -143,6 +143,31 @@ def run():
     out["ndt_batch"] = sha(np.stack([r["T"] for r in res]), np.array([[r["iterations"], r["converged"]] for r in res]),
                            np.array([r["fitness"] for r in res]))
     lb.close()
+    # ---- pcl NDT (the factory's NDT branch) on the same 131 072-point source: derivative and Hessian passes at one pose, an
+    # align with each line-search polarity, then the mixed-size batch
+    for flag in (0, 1):
+        pcfg = pkg.default_config(pkg.B2R_METHOD_NDT_PCL)
+        pcfg.ndt_resolution = 1.0
+        pcfg.ndt_mt_interval_flag = flag
+        r = pkg.Registration(pcfg)
+        r.setInputTarget(tgt)
+        r.setInputSource(src)
+        if flag == 0:
+            score, g, H, npairs = r.ndtDerivativesAt(NDT_P)
+            Hh = r.ndtHessianAt(NDT_P)
+            out["ndt_pcl_derivatives"] = sha(np.array([score]), g, H, np.array([npairs]), Hh)
+            anchor["ndt_pcl"] = dict(score=score, g=g.tolist(), H=H.tolist(), npairs=int(npairs))
+        r.align(perturb(11, 0.3, 1.5).astype(np.float32))
+        out[f"ndt_pcl_align_flag{flag}"] = sha(r.getFinalTransformation(), np.array([r.nr_iterations, r.hasConverged()]))
+        r.close()
+    pcfg = pkg.default_config(pkg.B2R_METHOD_NDT_PCL)
+    pcfg.ndt_resolution = 1.0
+    lb = pkg.RegistrationBatch(cfg=pcfg)
+    nids = {k: lb.addCloud(c) for k, c in nclouds.items()}
+    res = lb.align([(nids[s], nids[t], np.asarray(gg, np.float32)) for s, t, gg in npairs_], True, 2.5)
+    out["ndt_pcl_batch"] = sha(np.stack([r["T"] for r in res]), np.array([[r["iterations"], r["converged"]] for r in res]),
+                               np.array([r["fitness"] for r in res]))
+    lb.close()
     return out, anchor
 
 

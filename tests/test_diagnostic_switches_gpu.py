@@ -4,9 +4,9 @@ The engine reads its switches once per process, so each configuration runs tests
 GICP odometry with and without the next frame announced and with the voxel-grid downsample, a single GICP pair, k-NN and
 covariances on a 100 000-point target, the voxel grid and the prefilter (each outlier method) on a KITTI-size scan, NDT
 derivative / Hessian passes and aligns on a 131 072-point source, a 16-pair GICP batch with loop detection and fitness scores,
-and an NDT batch of mixed sizes.  Each configuration's SHA-1 per output must equal the baseline's (no switch set), and the
-baseline itself is pinned to the oracle: its single GICP pair and first odometry step to oracle.gicp_align, its NDT derivatives
-to the oracle's derivative pass."""
+an NDT batch of mixed sizes, and the same passes, aligns (both line-search polarities) and batch for the pcl NDT method.
+Each configuration's SHA-1 per output must equal the baseline's (no switch set), and the baseline itself is pinned to the oracle: its single GICP pair and first odometry step to oracle.gicp_align, its NDT derivatives
+to the oracle's derivative pass, its pcl NDT derivatives to tests/ndt_pcl_ref.cpp."""
 import json
 import os
 import subprocess
@@ -16,6 +16,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import pytest
 from common import rot_err, trans_err, relrel
+from ndt_pcl_ref import Reference
 from switch_workload import NDT_P, sha
 
 pytestmark = pytest.mark.gpu
@@ -73,7 +74,7 @@ def results():
     return {label(c): o for c, o in zip(confs, outs)}
 
 
-def test_baseline_matches_the_oracle(results, synth, oracle):
+def test_baseline_matches_the_oracle(results, synth, oracle, tmp_path):
     assert "error" not in results["baseline"], results["baseline"].get("error")
     a = results["baseline"]["anchor"]
     f0, f1 = synth.scan("vlp16", frame=0, stride=8), synth.scan("vlp16", frame=1, stride=8)
@@ -90,6 +91,12 @@ def test_baseline_matches_the_oracle(results, synth, oracle):
     assert n["npairs"] == od["n_pairs"] > 10000
     assert abs(n["score"] - od["score"]) <= 1e-9 * abs(od["score"])
     assert relrel(n["g"], od["g"]) < 1e-9 and relrel(n["H"], od["H"]) < 1e-9
+    # the pcl NDT passes at the same pose, against the sequential reference of that method (tests/ndt_pcl_ref.cpp)
+    op = Reference(tmp_path).map(tgt, 1.0).derivatives(src, NDT_P)
+    n = a["ndt_pcl"]
+    assert n["npairs"] == op["n_pairs"] > 10000
+    assert abs(n["score"] - op["score"]) <= 1e-9 * abs(op["score"])
+    assert relrel(n["g"], op["g"]) < 1e-9 and relrel(n["H"], op["H"]) < 1e-9
 
 
 @pytest.mark.parametrize("env", SWITCHES, ids=label)
