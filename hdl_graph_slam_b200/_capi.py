@@ -8,7 +8,7 @@ LIB_PATH = os.environ.get("B2R_LIB") or os.path.join(_HERE, "_lib", "libb200reg.
 
 B2R_OK = 0
 B2R_EINVAL, B2R_ENODEVICE, B2R_ECUDA, B2R_ESTATE, B2R_EUNSUPPORTED, B2R_ENCCL = -1, -2, -3, -4, -5, -6
-B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL = 0, 1, 2
+B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP = 0, 1, 2, 3
 B2R_DOWNSAMPLE_NONE, B2R_DOWNSAMPLE_VOXELGRID, B2R_DOWNSAMPLE_APPROX_VOXELGRID = 0, 1, 2
 
 
@@ -119,6 +119,8 @@ SYMBOLS = [
     ("b2r_ndt_hessian_at", C.c_int, [_VP, _F64P, _F64P]),
     ("b2r_ndt_get_centroids", C.c_int, [_VP, _SZ, C.POINTER(_SZ), C.POINTER(C.c_int64), _F32P]),
     ("b2r_ndt_neighbors_at", C.c_int, [_VP, _F64P, C.POINTER(C.c_uint32), _SZ, C.POINTER(C.c_int64), C.POINTER(_SZ)]),
+    ("b2r_vgicp_get_voxels", C.c_int, [_VP, _SZ, C.POINTER(_SZ), C.POINTER(C.c_int32), C.POINTER(C.c_int32), _F64P, _F64P]),
+    ("b2r_vgicp_linearize_at", C.c_int, [_VP, _F64P, _F64P, _F64P, _F64P, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), _SZ]),
     ("b2r_voxelgrid", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_float, _VP, C.POINTER(_SZ), _I32P, _I32P]),
     ("b2r_voxelgrid_device", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_float, C.POINTER(_VP), C.POINTER(_SZ)]),
     ("b2r_approximate_voxelgrid", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_float, _VP, C.POINTER(_SZ), _I32P]),

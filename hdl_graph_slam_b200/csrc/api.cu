@@ -24,6 +24,7 @@
 #include "bvh_build.cuh"
 #include "fitness.cuh"
 #include "ndt.cuh"
+#include "vgicp.cuh"
 #include "voxelgrid.cuh"
 #include "approx_voxelgrid.cuh"
 #include "prefilter.cuh"
@@ -106,6 +107,9 @@ struct b2r_handle {
 };
 
 static Cloud& SRC(b2r_handle* h) { return h->clouds[h->src]; }
+// the methods whose clouds carry FastGICP's covariances and run the device LM (pair_engine.cuh)
+static bool gicp_family(int method) { return method == B2R_METHOD_GICP || method == B2R_METHOD_VGICP; }
+static bool known_method(int method) { return gicp_family(method) || ndt_family(method); }
 static Cloud& TGT(b2r_handle* h) { return h->clouds[h->tgt]; }
 
 extern "C" const char* b2r_last_error(void) { return g_last_error.c_str(); }
@@ -121,14 +125,14 @@ extern "C" int b2r_config_default(b2r_config* c, int method) {
   c->transformation_epsilon = 0.01;   // :31,109
   c->rotation_epsilon = 2e-3;         // fast_gicp default
   c->max_correspondence_distance = 2.5;  // :33
-  c->ndt_resolution = 0.5;            // :93
+  c->ndt_resolution = method == B2R_METHOD_VGICP ? 1.0 : 0.5;  // :93; FAST_VGICP's reg_resolution default (:51)
   c->ndt_step_size = 0.1;             // ndt_omp default (never overridden by the factory)
   c->ndt_outlier_ratio = 0.55;
   c->ndt_search_method = 7;           // :103 DIRECT7
   c->ndt_mt_interval_flag = 0;
   c->ndt_fixed_iterations = 0;
   c->grid_cell_min = 0.5f;
-  if (method != B2R_METHOD_GICP && !ndt_family(method)) return fail(B2R_EINVAL, "unknown method");
+  if (!known_method(method)) return fail(B2R_EINVAL, "unknown method");
   return B2R_OK;
 }
 
@@ -169,6 +173,14 @@ extern "C" int b2r_select_registration_method(const char* const* keys, const cha
     c.ndt_resolution = dparam("reg_resolution", 0.5);
     c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
     c.max_iterations = iparam("reg_maximum_iterations", 64);
+  } else if (method == "FAST_VGICP" || method == "B200_VGICP") {
+    // registrations.cpp:48-56: resolution, transformation epsilon, maximum iterations and correspondence randomness; reg_num_threads
+    // is read and has no effect here, reg_max_correspondence_distance is not read (FastVGICP does not use it)
+    b2r_config_default(&c, B2R_METHOD_VGICP);
+    c.ndt_resolution = dparam("reg_resolution", 1.0);
+    c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
+    c.max_iterations = iparam("reg_maximum_iterations", 64);
+    c.k_correspondences = iparam("reg_correspondence_randomness", 20);
   } else {
     return fail(B2R_EUNSUPPORTED, "registration_method '" + method + "' is not re-created by b200reg; keep the reference branch");
   }
@@ -184,7 +196,9 @@ static bool cluster16_allowed();
 extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
   if (!cfg || !out) return fail(B2R_EINVAL, "NULL argument");
   *out = nullptr;
-  if (cfg->method != B2R_METHOD_GICP && !ndt_family(cfg->method)) return fail(B2R_EINVAL, "unknown method");
+  if (!known_method(cfg->method)) return fail(B2R_EINVAL, "unknown method");
+  if (cfg->method == B2R_METHOD_VGICP && !(cfg->ndt_resolution > 0.0 && std::isfinite(cfg->ndt_resolution)))
+    return fail(B2R_EINVAL, "VGICP: ndt_resolution (reg_resolution) must be finite and positive");
   if (cfg->k_correspondences < 1 || cfg->k_correspondences > 64) return fail(B2R_EINVAL, "k_correspondences must be in [1,64]");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -505,9 +519,18 @@ static int build_cov(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
 
 static int ensure_cov(b2r_handle* h, Cloud& c, int ctx = 0) { return build_cov(h, c, h->bc[ctx], ctx ? h->st2 : h->st); }
 
+// VGICP: the Gaussian voxel map of a target (after its covariances), built once per cloud
+static int vgicp_ensure_map(b2r_handle* h, Cloud& c) {
+  if (c.vgicp_ready) return B2R_OK;
+  int rc = ensure_cov(h, c);
+  if (rc) return rc;
+  return vgicp_build_map(c, h->cfg.ndt_resolution, &h->tel, h->st);
+}
+
 static int preprocess(b2r_handle* h, int which, bool is_target) {
   Cloud& c = h->clouds[which];
-  if (h->cfg.method == B2R_METHOD_GICP) {
+  if (h->cfg.method == B2R_METHOD_VGICP && is_target) return vgicp_ensure_map(h, c);
+  if (gicp_family(h->cfg.method)) {
     // a target gets its covariances now; a SOURCE only its search structure: its k-NN covariance kernel is launched by the align,
     // beside the first correspondence search, which does not read it (run_single_pair) — unless the cloud arrives through the
     // prefetch path, where both have been built ahead on the second stream
@@ -579,7 +602,7 @@ static int prefetch_source(b2r_handle* h, const void* pts, size_t n, size_t stri
   // align that has completed: b2r_align synchronises), so they are free to be overwritten here
   int rc = upload(h, h->nxt, pts, n, stride, dev, h->st2);
   if (rc) return rc;
-  if (h->cfg.method == B2R_METHOD_GICP) {
+  if (gicp_family(h->cfg.method)) {
     rc = ensure_cov(h, h->clouds[h->nxt], 1);
     if (rc) return rc;
   }
@@ -712,9 +735,24 @@ static cudaError_t launch_search(PairDev* d_pairs, const int* d_active, unsigned
 }
 
 // one round (update_correspondences + linearize/compute_error + LM step) over n_slots pair slots
+// vmaps != nullptr: a VGICP round (k_vgicp_round + k_pair_lm; vmaps[k] is the voxel map of pair k's target)
 static int launch_round(PairDev* d_pairs, const int* d_active, unsigned n_slots, unsigned max_sorted, int copies, const LmCfg& cfg, cudaStream_t st,
-                        Telemetry* tel, bool search = true) {
+                        Telemetry* tel, bool search = true, const VgicpMapDev* vmaps = nullptr) {
   static const bool pdl = !getenv("B2R_NO_PDL");
+  if (vmaps) {
+    TEL_BEGIN(tel, st);
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = dim3((unsigned)(max_sorted / kAccThreads), n_slots); lc.blockDim = dim3(kAccThreads); lc.dynamicSmemBytes = 0; lc.stream = st;
+    cudaLaunchAttribute la[1];
+    la[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    la[0].val.programmaticStreamSerializationAllowed = 1;
+    lc.attrs = la; lc.numAttrs = pdl ? 1 : 0;
+    B2R_CUDA(cudaLaunchKernelEx(&lc, k_vgicp_round, d_pairs, d_active, vmaps));
+    lc.gridDim = dim3(n_slots); lc.blockDim = dim3(kLmThreads);
+    B2R_CUDA(cudaLaunchKernelEx(&lc, k_pair_lm, d_pairs, d_active, cfg));
+    TEL_END(tel, KC_VGICP_ROUND, 2, st);
+    return B2R_OK;
+  }
   if (search) {
     TEL_BEGIN(tel, st);
     cudaError_t e = copies == 1 ? launch_search<1>(d_pairs, d_active, n_slots, max_sorted, cfg, st, pdl)
@@ -760,7 +798,7 @@ static bool report_consistent(const volatile unsigned long long* flag, unsigned 
 // `between` (may be null) runs on the host once the first rounds are enqueued and before the wait for the report: host work that
 // blocks on another stream (the odometry's next-frame downsample) then overlaps the align instead of delaying its enqueue.
 static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, const LmCfg& cfg, int first_batch, bool cov_beside_first_search = false,
-                           const std::function<int()>* between = nullptr) {
+                           const std::function<int()>* between = nullptr, const VgicpMapDev* vmaps = nullptr) {
   Cloud& s = SRC(h);
   Cloud& t = TGT(h);
   PairDev P;
@@ -806,7 +844,7 @@ static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, co
   }
   auto enqueue = [&](int n) -> int {
     for (int i = 0; i < n; i++) {
-      int rc = launch_round(h->d_pair.p, nullptr, 1, max_sorted, copies, cfg, h->st, &h->tel, true);
+      int rc = launch_round(h->d_pair.p, nullptr, 1, max_sorted, copies, cfg, h->st, &h->tel, true, vmaps);
       if (rc) return rc;
       enq++;
     }
@@ -869,11 +907,12 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out, const 
     return between ? (*between)() : B2R_OK;
   }
   static const bool overlap = !getenv("B2R_NO_COV_OVERLAP");
-  const bool cov_beside = overlap && !s.cov_ready;  // see run_single_pair
+  const bool vgicp = h->cfg.method == B2R_METHOD_VGICP;
+  const bool cov_beside = overlap && !s.cov_ready && !vgicp;  // see run_single_pair (a VGICP round reads the source covariances at once)
   int rc = cov_beside ? ensure_grid(h, s) : ensure_cov(h, s);
   if (rc) return rc;
   if (cov_beside) B2R_CUDA(s.cov.reserve((size_t)s.nsup * 1024 * 6 + 6));  // the pair record takes the buffer's address before the kernel that fills it is launched
-  rc = ensure_cov(h, t);
+  rc = vgicp ? vgicp_ensure_map(h, t) : ensure_cov(h, t);
   if (rc) return rc;
   rc = ensure_align_ws(h, s.n);
   if (rc) return rc;
@@ -885,7 +924,7 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out, const 
   // enqueue as many rounds as the previous align needed (consecutive frames need the same number almost always): a finished
   // pair's surplus rounds exit at once, a shortfall is topped up while the device works
   const int predicted = h->last_rounds > 0 ? h->last_rounds : 5;
-  rc = run_single_pair(h, x0, PM_FIRST, 0, cfg, predicted < 2 ? 2 : predicted, cov_beside, between);
+  rc = run_single_pair(h, x0, PM_FIRST, 0, cfg, predicted < 2 ? 2 : predicted, cov_beside, between, vgicp ? t.vgicp->d_desc.p : nullptr);
   if (rc) return rc;
   const PairReport& rep = *h->h_rep;
   h->cur = rep.cur;
@@ -903,7 +942,7 @@ static int align_impl(b2r_handle* h, const float guess[16], b2r_result* out, con
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   int rc = need_source(h);
   if (rc != B2R_OK) {}  // reported below like every failed align
-  else if (h->cfg.method == B2R_METHOD_GICP) rc = gicp_align(h, guess, out, between);
+  else if (gicp_family(h->cfg.method)) rc = gicp_align(h, guess, out, between);
   else {
     float Tfinal[16];
     bool conv = false;
@@ -1045,7 +1084,7 @@ extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
 
 extern "C" int b2r_get_covariances(b2r_handle* h, int which, double* out, size_t n) {
   if (!h || !out) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_GICP) return fail(B2R_ESTATE, "covariances exist only for the GICP engine");
+  if (!gicp_family(h->cfg.method)) return fail(B2R_ESTATE, "covariances exist only for the GICP and VGICP engines");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (!which && need_source(h)) return B2R_ESTATE;
   Cloud& c = which ? TGT(h) : SRC(h);
@@ -1098,6 +1137,7 @@ extern "C" int b2r_gicp_linearize_at(b2r_handle* h, const double T[16], double* 
 
 extern "C" int b2r_gicp_error_at(b2r_handle* h, const double T[16], double* err) {
   if (!h || !T || !err) return fail(B2R_EINVAL, "NULL argument");
+  if (h->cfg.method != B2R_METHOD_GICP) return fail(B2R_ESTATE, "GICP engine required");
   if (!h->corr_valid) return fail(B2R_ESTATE, "no linearisation has run");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   double x[16];
@@ -1108,6 +1148,54 @@ extern "C" int b2r_gicp_error_at(b2r_handle* h, const double T[16], double* err)
   if (rc) return rc;
   B2R_CUDA(cudaStreamSynchronize(h->st));
   *err = h->h_tap[28];
+  return B2R_OK;
+}
+
+extern "C" int b2r_vgicp_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int32_t* cells, int32_t* counts, double* mean, double* cov) {
+  if (!h || !n_voxels) return fail(B2R_EINVAL, "NULL argument");
+  *n_voxels = 0;
+  if (h->cfg.method != B2R_METHOD_VGICP) return fail(B2R_ESTATE, "VGICP engine (B2R_METHOD_VGICP) required");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  int rc = vgicp_ensure_map(h, TGT(h));
+  if (rc) return rc;
+  return vgicp_dump(TGT(h), h->st, capacity, n_voxels, cells, counts, mean, cov);
+}
+
+extern "C" int b2r_vgicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* cost, uint64_t* n_corr, int32_t* voxel_of,
+                                      size_t n) {
+  if (!h || !T || !H || !b || !cost) return fail(B2R_EINVAL, "NULL argument");
+  if (h->cfg.method != B2R_METHOD_VGICP) return fail(B2R_ESTATE, "VGICP engine (B2R_METHOD_VGICP) required");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (need_source(h)) return B2R_ESTATE;
+  Cloud& s = SRC(h);
+  Cloud& t = TGT(h);
+  if (s.n == 0 || t.n == 0) return fail(B2R_ESTATE, "source/target not set");
+  if (voxel_of && n != s.n) return fail(B2R_EINVAL, "n does not match the source cloud");
+  int rc = ensure_cov(h, s);
+  if (!rc) rc = vgicp_ensure_map(h, t);
+  if (!rc) rc = ensure_align_ws(h, s.n);
+  if (rc) return rc;
+  double x[16];
+  for (int r = 0; r < 4; r++)
+    for (int c = 0; c < 4; c++) x[r * 4 + c] = T[c * 4 + r];
+  const LmCfg cfg = make_lm_cfg(h->cfg, false, DBL_MAX);
+  rc = run_single_pair(h, x, PM_FIRST, 1, cfg, 1, false, nullptr, t.vgicp->d_desc.p);  // one probe + linearize round, reduced values tapped
+  if (rc) return rc;
+  B2R_CUDA(cudaStreamSynchronize(h->st));
+  h->cur = 0;
+  h->corr_valid = true;
+  int k = 0;
+  for (int r = 0; r < 6; r++)
+    for (int c = r; c < 6; c++) { H[r * 6 + c] = H[c * 6 + r] = h->h_tap[k++]; }
+  for (int i = 0; i < 6; i++) b[i] = h->h_tap[21 + i];
+  *cost = h->h_tap[27];
+  if (n_corr || voxel_of) {
+    std::vector<int32_t> v(s.n);
+    rc = b2r_get_correspondences(h, v.data(), s.n);
+    if (rc) return rc;
+    if (n_corr) { uint64_t c = 0; for (int32_t x : v) c += x >= 0; *n_corr = c; }
+    if (voxel_of) std::memcpy(voxel_of, v.data(), s.n * sizeof(int32_t));
+  }
   return B2R_OK;
 }
 
@@ -1967,7 +2055,7 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
   // the NEXT frame's upload / BVH / covariances overlap this frame's align on a second stream.  Its downsample waits on the host
   // for the filter's output count; on a GICP handle it is therefore issued from inside the align, once the align's first rounds
   // are on the main stream, so that the wait does not hold them back
-  const bool prefetch_in_align = odometry_downsamples(o->p) && reg->cfg.method == B2R_METHOD_GICP;
+  const bool prefetch_in_align = odometry_downsamples(o->p) && gicp_family(reg->cfg.method);
   if (!prefetch_in_align) {
     rc = odometry_issue_prefetch(o);
     if (rc) return rc;

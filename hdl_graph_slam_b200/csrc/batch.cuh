@@ -38,6 +38,7 @@ struct b2r_batch {
     Event ev;
     DevBuf<PairDev> d_pairs;
     DevBuf<int> d_active;
+    DevBuf<VgicpMapDev> d_vmaps;     // VGICP: the voxel map of each pair's target, indexed like d_pairs
     unsigned long long* h_word = nullptr;  // host-mapped: (seq << 32) | pairs still active
     unsigned long long* h_word_dev = nullptr;
     unsigned long long seq = 0;
@@ -49,6 +50,10 @@ struct b2r_batch {
   DevBuf<char> ws;
   PinnedBuf<PairDev> h_pairs;       // staging
   PinnedBuf<PairReport> h_reports;  // staging
+  PinnedBuf<VgicpMapDev> h_vmaps;   // staging (VGICP)
+  DevBuf<char> vfit_ws;             // VGICP getFitnessScore: per pair the reduction partials, counter and sums
+  DevBuf<VgicpFitItem> d_vfit;      // VGICP getFitnessScore: one record per pair of the call
+  PinnedBuf<VgicpFitItem> h_vfit;   // staging (filled once per call, so no chunk overwrites a record still being copied)
   MappedBuf<unsigned long long> h_word;  // [0..kLanes) = the lanes' words, [kLanes] = sum of the pairs' executed rounds
   size_t max_chunk = 1024;  // pairs in flight per launch sequence (~7.7 MB of workspace per 64k-point pair)
   int copies = 1;           // lanes per query of the batched 1-NN search
@@ -93,7 +98,7 @@ extern "C" void b2r_batch_destroy(b2r_batch* b) { delete b; }
 extern "C" int b2r_batch_create(const b2r_config* cfg, b2r_batch** out) {
   if (!cfg || !out) return fail(B2R_EINVAL, "NULL argument");
   *out = nullptr;
-  if (cfg->method != B2R_METHOD_GICP && !ndt_family(cfg->method)) return fail(B2R_EINVAL, "unknown method");
+  if (!known_method(cfg->method)) return fail(B2R_EINVAL, "unknown method");
   std::unique_ptr<b2r_batch> b(new b2r_batch());
   b2r_handle* eng = nullptr;
   int rc = b2r_create(cfg, &eng);
@@ -303,10 +308,11 @@ static void degenerate_report(PairReport& r, const float* guess_col) {
 }
 
 static int batch_host_staging(b2r_batch* b, size_t n) {
-  if (b->h_pairs.cap >= n && b->h_reports.cap >= n) return B2R_OK;
+  if (b->h_pairs.cap >= n && b->h_reports.cap >= n && b->h_vmaps.cap >= n) return B2R_OK;
   const size_t want = n + n / 4 + 16;
   B2R_CUDA(b->h_pairs.alloc(want));
   B2R_CUDA(b->h_reports.alloc(want));
+  B2R_CUDA(b->h_vmaps.alloc(want));
   return B2R_OK;
 }
 
@@ -333,6 +339,7 @@ static int wait_word(const b2r_batch::Lane& L, unsigned long long need_seq, size
 static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const LmCfg& cfg, PairReport* d_rep, bool fit_only) {
   b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
+  const bool vgicp = h->cfg.method == B2R_METHOD_VGICP && !fit_only;  // a stand-alone fitness evaluation runs the GICP search
   // per-launch kernel timing (b2r_set_profiling) wants every kernel alone on the device; tiny chunks are not worth a second stream
   const int n_lanes = (h->tel.on || m < 16) ? 1 : b->n_lanes;
   size_t ws_total = 0;
@@ -359,6 +366,7 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
     if (R.m == 0) continue;
     B2R_CUDA(L.d_pairs.reserve(R.m));
     B2R_CUDA(L.d_active.reserve(R.m + 1));
+    if (vgicp) B2R_CUDA(L.d_vmaps.reserve(R.m));
     for (size_t i = R.i0; i < R.i0 + R.m; i++) {
       PairDev& P = b->h_pairs.p[i];
       const Cloud& s = *b->clouds[pairs[i].source];
@@ -371,6 +379,7 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
         continue;
       }
       fill_pair_geometry(P, s, t);
+      if (vgicp) b->h_vmaps.p[i] = t.vgicp->desc;
       double x[16];
       colmajor_f_to_row_d(pairs[i].guess, x);
       // a stand-alone fitness evaluation (calc_fitness_score) is a pair that starts in its fitness round at the given pose
@@ -389,6 +398,10 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
     }
     B2R_CUDA(cudaMemcpyAsync(L.d_pairs.p, b->h_pairs.p + R.i0, R.m * sizeof(PairDev), cudaMemcpyHostToDevice, L.st));
     h->tel.h2d += R.m * sizeof(PairDev);
+    if (vgicp) {
+      B2R_CUDA(cudaMemcpyAsync(L.d_vmaps.p, b->h_vmaps.p + R.i0, R.m * sizeof(VgicpMapDev), cudaMemcpyHostToDevice, L.st));
+      h->tel.h2d += R.m * sizeof(VgicpMapDev);
+    }
     k_pair_compact<<<1, 1024, 0, L.st>>>(L.d_pairs.p, (int)R.m, L.d_active.p, L.h_word_dev, ++L.seq);
     B2R_CUDA(cudaGetLastError());
   }
@@ -403,7 +416,8 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
       LaneRun& R = run[l];
       if (R.known == 0) continue;
       any = true;
-      int rc = launch_round(L.d_pairs.p, L.d_active.p, (unsigned)R.known, (unsigned)R.max_pad, b->copies, cfg, L.st, &h->tel, true);
+      int rc = launch_round(L.d_pairs.p, L.d_active.p, (unsigned)R.known, (unsigned)R.max_pad, b->copies, cfg, L.st, &h->tel, true,
+                            vgicp ? L.d_vmaps.p : nullptr);
       if (rc) return rc;
       b->last_rounds++;
       sq[l] = ++L.seq;
@@ -430,6 +444,73 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
     B2R_CUDA(cudaEventRecord(b->lane[l].ev, b->lane[l].st));
     B2R_CUDA(cudaStreamWaitEvent(st, b->lane[l].ev, 0));
   }
+  return B2R_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ VGICP batch
+// The voxel map of every cloud a call aligns to (the first use of a keyframe as a target builds it; it stays with the cloud).
+static int batch_vgicp_maps(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs) {
+  b2r_handle* h = b->eng.get();
+  for (size_t i = 0; i < n_pairs; i++) {
+    Cloud& t = *b->clouds[pairs[i].target];
+    if (t.n == 0 || t.vgicp_ready) continue;
+    int rc = vgicp_build_map(t, h->cfg.ndt_resolution, &h->tel, h->st);
+    if (rc) return rc;
+  }
+  return B2R_OK;
+}
+
+// getFitnessScore at the final pose of every pair of the call (reports d_rep[0..m) on the device): one k_vgicp_fitness launch covers
+// every pair with the kernel, grid and reduction of b2r_fitness, so each score is bitwise b2r_fitness's; no host round trip.
+static int batch_vgicp_fitness(b2r_batch* b, const b2r_pair* pairs, size_t m, double fit_max_range, PairReport* d_rep) {
+  b2r_handle* h = b->eng.get();
+  cudaStream_t st = h->st;
+  std::vector<size_t> live, off;
+  size_t ws = 0;
+  unsigned max_nb = 0;
+  for (size_t i = 0; i < m; i++) {
+    const Cloud& s = *b->clouds[pairs[i].source];
+    const Cloud& t = *b->clouds[pairs[i].target];
+    if (s.n == 0 || t.n == 0) continue;  // degenerate_report: DBL_MAX already
+    const size_t nb = (size_t)s.nsup * 1024 / kLinThreads;
+    live.push_back(i);
+    off.push_back(ws);
+    ws += align_up(nb * 3 * sizeof(double), 256) + 256;  // partials, then counter [0, 16) and the three sums [64, 88)
+    max_nb = std::max(max_nb, (unsigned)nb);
+  }
+  if (live.empty()) return B2R_OK;
+  B2R_CUDA(b->vfit_ws.reserve(ws + 256));
+  B2R_CUDA(b->d_vfit.reserve(live.size()));
+  if (b->h_vfit.cap < live.size()) B2R_CUDA(b->h_vfit.alloc(live.size() + live.size() / 4 + 16));
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->vfit_ws.p), 256));
+  B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));  // the reduction counters start at zero (and re-arm themselves)
+  for (size_t k = 0; k < live.size(); k++) {
+    const size_t i = live[k];
+    const Cloud& s = *b->clouds[pairs[i].source];
+    const Cloud& t = *b->clouds[pairs[i].target];
+    const size_t nb = (size_t)s.nsup * 1024 / kLinThreads;
+    VgicpFitItem& it = b->h_vfit.p[k];
+    std::memset(&it, 0, sizeof(it));
+    it.A.src = s.bvh(); it.A.tgt = t.bvh();
+    it.A.max_range = fit_max_range; it.A.inlier_thresh_sq = 0.25f;
+    char* p = base + off[k];
+    it.A.partials = reinterpret_cast<double*>(p);
+    it.A.counter = reinterpret_cast<unsigned int*>(p + align_up(nb * 3 * sizeof(double), 256));
+    it.A.out = reinterpret_cast<double*>(p + align_up(nb * 3 * sizeof(double), 256) + 64);
+    it.rep = d_rep + i;
+    it.nblk = (unsigned)nb;
+  }
+  B2R_CUDA(cudaMemcpyAsync(b->d_vfit.p, b->h_vfit.p, live.size() * sizeof(VgicpFitItem), cudaMemcpyHostToDevice, st));
+  h->tel.h2d += live.size() * sizeof(VgicpFitItem);
+  for (size_t k0 = 0; k0 < live.size(); k0 += 65535) {  // grid.y limit
+    const unsigned ny = (unsigned)std::min<size_t>(65535, live.size() - k0);
+    TEL_BEGIN(&h->tel, st);
+    k_vgicp_fitness<<<dim3(max_nb, ny), kLinThreads, 0, st>>>(b->d_vfit.p + k0);
+    TEL_END(&h->tel, KC_FITNESS, 1, st);
+    B2R_CUDA(cudaGetLastError());
+  }
+  k_vgicp_fitness_store<<<(unsigned)((live.size() + 255) / 256), 256, 0, st>>>(b->d_vfit.p, (int)live.size());
+  B2R_CUDA(cudaGetLastError());
   return B2R_OK;
 }
 
@@ -661,12 +742,16 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   if (rc) return rc;
   if (ndt) rc = batch_ndt_maps(b, pairs, n_pairs, fit_only);
   if (rc) return rc;
+  const bool vgicp = h->cfg.method == B2R_METHOD_VGICP && !fit_only;
+  if (vgicp) rc = batch_vgicp_maps(b, pairs, n_pairs);
+  if (rc) return rc;
   const auto t_b = std::chrono::steady_clock::now();
   const size_t chunk = std::min(b->max_chunk, std::max<size_t>(n_pairs, 1));
   rc = batch_host_staging(b, std::max(chunk, n_pairs));
   if (rc) return rc;
   B2R_CUDA(b->d_reports.reserve(n_pairs + 1));
-  const LmCfg cfg = make_lm_cfg(h->cfg, want_fitness, fit_max_range);
+  // a VGICP round carries no fitness sums: its scores come from batch_vgicp_fitness after the rounds
+  const LmCfg cfg = make_lm_cfg(h->cfg, want_fitness && !vgicp, fit_max_range);
   b->last_rounds = b->last_pair_rounds = 0;
   for (size_t c0 = 0; c0 < n_pairs; c0 += chunk) {
     const size_t m = std::min(chunk, n_pairs - c0);
@@ -675,6 +760,8 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
     else rc = batch_run_chunk(b, pairs + c0, m, cfg, b->d_reports.p + c0, fit_only);
     if (rc) return rc;
   }
+  if (vgicp && want_fitness) rc = batch_vgicp_fitness(b, pairs, n_pairs, fit_max_range, b->d_reports.p);
+  if (rc) return rc;
   if (ndt && !fit_only)  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
     B2R_CUDA(cudaMemcpyAsync(b->d_reports.p, b->h_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyHostToDevice, h->st));
   if (dbg) {

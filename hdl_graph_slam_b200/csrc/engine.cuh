@@ -96,10 +96,10 @@ struct Stream {
 };
 
 // ---- telemetry: copy byte counters, launch counters and (optional) CUDA-event timing per kernel class
-enum KernelClass { KC_GRID = 0, KC_KNN_COV, KC_GICP_CORR, KC_GICP_LIN, KC_GICP_ERR, KC_FITNESS, KC_NDT_BUILD, KC_NDT_DERIV, KC_NDT_HESS, KC_VOXELGRID, KC_MISC, KC_COUNT };
+enum KernelClass { KC_GRID = 0, KC_KNN_COV, KC_GICP_CORR, KC_GICP_LIN, KC_GICP_ERR, KC_FITNESS, KC_NDT_BUILD, KC_NDT_DERIV, KC_NDT_HESS, KC_VOXELGRID, KC_MISC, KC_VGICP_MAP, KC_VGICP_ROUND, KC_COUNT };
 inline const char* kernel_class_name(int c) {
   static const char* n[KC_COUNT] = {"bvh_build", "knn_covariance", "gicp_correspondences", "gicp_linearize", "gicp_error", "nn_fitness", "ndt_voxel_build",
-                                    "ndt_derivatives", "ndt_hessian", "voxelgrid_downsample", "misc"};
+                                    "ndt_derivatives", "ndt_hessian", "voxelgrid_downsample", "misc", "vgicp_voxel_map", "vgicp_round"};
   return (c >= 0 && c < KC_COUNT) ? n[c] : "?";
 }
 struct Telemetry {
@@ -190,6 +190,7 @@ inline int wait_host_result(const unsigned long long* flag, unsigned long long s
 }
 
 struct NdtVoxelMap;  // ndt.cuh: complete wherever a Cloud is destroyed
+struct VgicpMap;    // vgicp.cuh: likewise
 
 // One point cloud resident on the device with everything derived from it.
 struct Cloud {
@@ -209,7 +210,10 @@ struct Cloud {
   // NDT (target only)
   std::unique_ptr<NdtVoxelMap> ndt;
   bool ndt_ready = false;
-  void invalidate() { bvh_ready = cov_ready = ndt_ready = false; }
+  // VGICP (target only): Gaussian voxel map built from the BVH arrays and the covariances
+  std::unique_ptr<VgicpMap> vgicp;
+  bool vgicp_ready = false;
+  void invalidate() { bvh_ready = cov_ready = ndt_ready = vgicp_ready = false; }
   Bvh bvh() const {
     Bvh b;
     b.sp = sorted.p; b.leaf_lo = leaf_lo.p; b.leaf_hi = leaf_hi.p; b.sup_lo = sup_lo.p; b.sup_hi = sup_hi.p;

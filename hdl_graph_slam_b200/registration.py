@@ -18,7 +18,7 @@ library; nothing here computes.
 import ctypes as C
 import numpy as np
 from . import _capi
-from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL  # noqa: F401
+from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP  # noqa: F401
 
 
 def _cloud(a):
@@ -256,6 +256,34 @@ class Registration:
         check(self._lib.b2r_ndt_neighbors_at(self._h, p.ctypes.data_as(dp), counts.ctypes.data_as(C.POINTER(C.c_uint32)), total.value,
                                              keys.ctypes.data_as(C.POINTER(C.c_int64)), C.byref(total)))
         return counts[:n_source], keys[:total.value]
+
+    def vgicpGetVoxels(self):
+        """(VGICP) the target's Gaussian voxel map, cells ascending: dict(cells (V, 3) int32, counts (V,), mean (V, 3), cov (V, 3, 3))"""
+        nv = C.c_size_t()
+        check(self._lib.b2r_vgicp_get_voxels(self._h, 0, C.byref(nv), None, None, None, None))
+        V = nv.value
+        cells = np.empty((V, 3), np.int32)
+        counts = np.empty(V, np.int32)
+        mean = np.empty((V, 3), np.float64)
+        cov = np.empty((V, 3, 3), np.float64)
+        ip, dp = C.POINTER(C.c_int32), C.POINTER(C.c_double)
+        check(self._lib.b2r_vgicp_get_voxels(self._h, V, C.byref(nv), cells.ctypes.data_as(ip), counts.ctypes.data_as(ip), mean.ctypes.data_as(dp),
+                                             cov.ctypes.data_as(dp)))
+        return dict(cells=cells, counts=counts, mean=mean, cov=cov)
+
+    def vgicpLinearizeAt(self, T, n_source):
+        """(VGICP) one voxel-correspondence update + linearisation at T: (H (6, 6), b (6,), cost, correspondence count, voxel of every
+        source point (n,) int32, -1 = none)"""
+        t = _colmajor(T, np.float64)
+        H = np.empty((6, 6), np.float64)
+        b = np.empty(6, np.float64)
+        cost = C.c_double()
+        nc = C.c_uint64()
+        vox = np.empty(max(n_source, 1), np.int32)
+        dp = C.POINTER(C.c_double)
+        check(self._lib.b2r_vgicp_linearize_at(self._h, t.ctypes.data_as(dp), H.ctypes.data_as(dp), b.ctypes.data_as(dp), C.byref(cost), C.byref(nc),
+                                               vox.ctypes.data_as(C.POINTER(C.c_int32)), n_source))
+        return H, b, cost.value, nc.value, vox[:n_source]
 
     # --- companion / prefilter chain
     def _filter(self, fn, cloud, *args):

@@ -49,6 +49,9 @@ extern "C" {
 #define B2R_METHOD_NDT_PCL 2 /* pcl::NormalDistributionsTransform semantics (registrations.cpp:93-100): radius neighbourhood over the
                                 voxel centroids, float64 derivatives; reads ndt_resolution / ndt_step_size / ndt_outlier_ratio /
                                 ndt_mt_interval_flag / ndt_fixed_iterations, not ndt_search_method */
+#define B2R_METHOD_VGICP 3 /* fast_gicp::FastVGICP semantics (registrations.cpp:48-56): FastGICP's covariances, the target's Gaussian voxel
+                              map at ndt_resolution (reg_resolution), DIRECT1 voxel correspondences, weights sqrt(num_points); reads
+                              max_iterations / k_correspondences / transformation_epsilon, not max_correspondence_distance */
 
 typedef struct b2r_handle b2r_handle;
 
@@ -87,8 +90,9 @@ int b2r_config_default(b2r_config* cfg, int method);
 
 /* replaces select_registration_method(ros::NodeHandle&) (registrations.cpp:22-124): same parameter NAMES and defaults,
  * passed as string key/value pairs (the rosparam namespace of the nodelet).  "FAST_GICP"/"B200_GICP" -> GICP engine,
- * "NDT_OMP"/"B200_NDT" -> NDT engine, "NDT" -> pcl NDT engine (B2R_METHOD_NDT_PCL).  ICP / GICP / GICP_OMP / FAST_VGICP[_CUDA]
- * and unknown names are not re-created: returns B2R_EUNSUPPORTED so the caller keeps the reference's own branch. */
+ * "NDT_OMP"/"B200_NDT" -> NDT engine, "NDT" -> pcl NDT engine (B2R_METHOD_NDT_PCL), "FAST_VGICP"/"B200_VGICP" -> VGICP engine
+ * (B2R_METHOD_VGICP).  ICP / GICP / GICP_OMP / FAST_VGICP_CUDA and unknown names are not re-created: returns B2R_EUNSUPPORTED so
+ * the caller keeps the reference's own branch. */
 int b2r_select_registration_method(const char* const* keys, const char* const* values, int n_params, int device_id,
                                    b2r_handle** out);
 
@@ -161,7 +165,7 @@ int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n);
 int b2r_get_covariances(b2r_handle* h, int which, double* out, size_t n);
 /* one update_correspondences + linearize at pose T (column-major double): H[36] row-major, b[6], *err = sum e^T M e */
 int b2r_gicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* err);
-/* one compute_error at pose T with the correspondences of the last linearisation */
+/* one compute_error at pose T with the correspondences of the last linearisation (GICP handle only: B2R_ESTATE on any other method) */
 int b2r_gicp_error_at(b2r_handle* h, const double T[16], double* err);
 /* NDT voxel table of the target (either NDT method): returns count through *n_voxels; arrays may be NULL.  keys ascending. */
 int b2r_ndt_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int64_t* keys, int32_t* npts, double* mean, double* icov,
@@ -178,6 +182,15 @@ int b2r_ndt_get_centroids(b2r_handle* h, size_t capacity, size_t* n_centroids, i
  * entries, may be NULL) and one flat array of the neighbours' leaf keys, ascending within each point (CSR by counts; the first
  * `capacity` entries are written, keys may be NULL); *total = the number of (point, neighbour) pairs */
 int b2r_ndt_neighbors_at(b2r_handle* h, const double p[6], uint32_t* counts, size_t capacity, int64_t* keys, size_t* total);
+/* B2R_METHOD_VGICP: the target's Gaussian voxel map (GaussianVoxelMap after finalize), cells ascending (x, then y, then z):
+ * cells[3 V] = floor(p / resolution) per axis, counts[V] = num_points, mean[3 V], cov[9 V] (3x3 row-major); *n_voxels = V; the first
+ * `capacity` voxels are written, every array may be NULL.  B2R_EUNSUPPORTED when a finite target point lies 2^20 cells or more from
+ * the origin on an axis (the keys hold 21 bits per axis); points with a non-finite coordinate belong to no voxel. */
+int b2r_vgicp_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int32_t* cells, int32_t* counts, double* mean, double* cov);
+/* B2R_METHOD_VGICP: one update_correspondences (DIRECT1) + linearize at pose T (column-major double): H[36] row-major, b[6],
+ * *cost = sum sqrt(num_points) e^T M e, *n_corr = source points with a voxel, voxel_of (n source entries in the caller's point order,
+ * may be NULL) = the index of the point's voxel in b2r_vgicp_get_voxels' order, or -1 */
+int b2r_vgicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* cost, uint64_t* n_corr, int32_t* voxel_of, size_t n);
 
 /* ---- companion: voxel-grid downsample ---------------------------------------------------------------------------
  * replaces pcl::VoxelGrid<PointXYZI>::filter with setLeafSize(leaf,leaf,leaf) (apps/prefiltering_nodelet.cpp:54-58,138-149;

@@ -1,4 +1,4 @@
-"""torchrun --nproc-per-node N tools/check_multi_gpu.py — the sharded loop-closure batch (b2r_batch_loop_detect: groups dealt to ranks,
+"""torchrun --nproc-per-node N tools/check_multi_gpu.py [groups] [sensor] [registration_method] — the sharded loop-closure batch (b2r_batch_loop_detect: groups dealt to ranks,
 in-library ncclAllGather of 80-byte records) must give EVERY rank the same records, bitwise equal to one GPU aligning all pairs alone
 (SURVEY.md §8e "determinism across G")."""
 import os, sys
@@ -16,6 +16,7 @@ dev = torch.device("cuda", local)
 dist.init_process_group("nccl", device_id=dev)
 n_groups = int(sys.argv[1]) if len(sys.argv) > 1 else 6
 sensor = sys.argv[2] if len(sys.argv) > 2 else "vlp16_16k"
+method = sys.argv[3] if len(sys.argv) > 3 else "FAST_GICP"  # registration_method of both batches (e.g. FAST_VGICP)
 groups, guesses, group_first = batch.loop_workload(n_groups, sensor)
 n_pairs = group_first[-1]
 
@@ -36,7 +37,7 @@ def run(lb, g0, g1):
     return lb.loopDetect(pairs, group_first, 2.5, 0.5, raw=True)
 
 
-lb = pkg.RegistrationBatch(params={"registration_method": "FAST_GICP"}, device_id=local)
+lb = pkg.RegistrationBatch(params={"registration_method": method}, device_id=local)
 idt = torch.zeros(128, dtype=torch.uint8, device=dev)
 if rank == 0:
     idt = torch.frombuffer(bytearray(pkg.RegistrationBatch.ncclUniqueId()), dtype=torch.uint8).to(dev)
@@ -52,7 +53,7 @@ dist.all_gather(allb, t)
 same = all(torch.equal(allb[0], x) for x in allb)
 ok = same
 if rank == 0:
-    solo = pkg.RegistrationBatch(params={"registration_method": "FAST_GICP"}, device_id=local)  # no communicator: one GPU, all pairs
+    solo = pkg.RegistrationBatch(params={"registration_method": method}, device_id=local)  # no communicator: one GPU, all pairs
     b1, r1 = run(solo, 0, n_groups)
     ref = bytes(memoryview(r1)[: n_pairs * 80]) + bytes(np.asarray(b1, np.int32).tobytes())
     ok = same and (ref == mine)
