@@ -5,6 +5,7 @@
 //   b2r_set_target / b2r_set_source <- pcl::Registration::setInputTarget/Source   (call sites in b200reg.h)
 //   b2r_align                       <- pcl::Registration::align -> computeTransformation (fast_gicp LsqRegistration LM loop,
 //                                      ndt_omp Newton + More-Thuente loop; SURVEY.md A.2, A.4)
+//                                      (pcl::GeneralizedIterativeClosestPoint BFGS loop: gicp_pcl.cuh)
 //   b2r_fitness                     <- getFitnessScore
 //   b2r_odometry_matching           <- ScanMatchingOdometryNodelet::matching  apps/scan_matching_odometry_nodelet.cpp:165-262
 //   b2r_loop_matching               <- LoopDetector::matching                include/hdl_graph_slam/loop_detector.hpp:117-171
@@ -25,6 +26,7 @@
 #include "fitness.cuh"
 #include "ndt.cuh"
 #include "vgicp.cuh"
+#include "gicp_pcl.cuh"
 #include "voxelgrid.cuh"
 #include "approx_voxelgrid.cuh"
 #include "prefilter.cuh"
@@ -94,7 +96,7 @@ struct b2r_handle {
   DevBuf<int> pf_total;             // 4 ints
   MappedBuf<int> pf_h_total;        // 4 ints
   BuildCtx bc[2];                   // per-stream build scratch (main stream, prefetch stream)
-  bool knn_smem_attr = false, stat_smem_attr = false;
+  bool knn_smem_attr = false, stat_smem_attr = false, pcl_knn_smem_attr = false;
   int n_sm = 132;
   // last result
   float final_T[16];                // row-major
@@ -103,13 +105,16 @@ struct b2r_handle {
   bool src_promoted = false;        // b2r_promote_source_to_target has taken the source away: no source until the next b2r_set_source*
   NdtWork ndt_work;
   VoxelWork vg_work;
+  GicpPclWork gp_work;              // B2R_METHOD_GICP_PCL: correspondence / cost pass buffers
   Telemetry tel;
 };
 
 static Cloud& SRC(b2r_handle* h) { return h->clouds[h->src]; }
 // the methods whose clouds carry FastGICP's covariances and run the device LM (pair_engine.cuh)
 static bool gicp_family(int method) { return method == B2R_METHOD_GICP || method == B2R_METHOD_VGICP; }
-static bool known_method(int method) { return gicp_family(method) || ndt_family(method); }
+// the methods whose clouds carry k-NN covariances: FastGICP's, or pcl GICP's raw-moment ones (B2R_METHOD_GICP_PCL)
+static bool cov_family(int method) { return gicp_family(method) || method == B2R_METHOD_GICP_PCL; }
+static bool known_method(int method) { return cov_family(method) || ndt_family(method); }
 static Cloud& TGT(b2r_handle* h) { return h->clouds[h->tgt]; }
 
 extern "C" const char* b2r_last_error(void) { return g_last_error.c_str(); }
@@ -132,6 +137,7 @@ extern "C" int b2r_config_default(b2r_config* c, int method) {
   c->ndt_mt_interval_flag = 0;
   c->ndt_fixed_iterations = 0;
   c->grid_cell_min = 0.5f;
+  c->max_optimizer_iterations = 20;   // :75
   if (!known_method(method)) return fail(B2R_EINVAL, "unknown method");
   return B2R_OK;
 }
@@ -181,6 +187,16 @@ extern "C" int b2r_select_registration_method(const char* const* keys, const cha
     c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
     c.max_iterations = iparam("reg_maximum_iterations", 64);
     c.k_correspondences = iparam("reg_correspondence_randomness", 20);
+  } else if (method.find("GICP") != std::string::npos && method.find("OMP") == std::string::npos && method != "FAST_VGICP_CUDA") {
+    // registrations.cpp:66-76 (every name containing GICP but not OMP that no branch above takes): pcl::GeneralizedIterativeClosestPoint.
+    // reg_use_reciprocal_correspondences is read upstream and has no effect on GICP; FAST_VGICP_CUDA stays refused (the reference only
+    // reaches this branch with it when built without USE_VGICP_CUDA)
+    b2r_config_default(&c, B2R_METHOD_GICP_PCL);
+    c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
+    c.max_iterations = iparam("reg_maximum_iterations", 64);
+    c.max_correspondence_distance = dparam("reg_max_correspondence_distance", 2.5);
+    c.k_correspondences = iparam("reg_correspondence_randomness", 20);
+    c.max_optimizer_iterations = iparam("reg_max_optimizer_iterations", 20);
   } else {
     return fail(B2R_EUNSUPPORTED, "registration_method '" + method + "' is not re-created by b200reg; keep the reference branch");
   }
@@ -200,6 +216,7 @@ extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
   if (cfg->method == B2R_METHOD_VGICP && !(cfg->ndt_resolution > 0.0 && std::isfinite(cfg->ndt_resolution)))
     return fail(B2R_EINVAL, "VGICP: ndt_resolution (reg_resolution) must be finite and positive");
   if (cfg->k_correspondences < 1 || cfg->k_correspondences > 64) return fail(B2R_EINVAL, "k_correspondences must be in [1,64]");
+  if (cfg->method == B2R_METHOD_GICP_PCL && cfg->max_optimizer_iterations < 1) return fail(B2R_EINVAL, "max_optimizer_iterations must be >= 1");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev <= 0) return fail(B2R_ENODEVICE, std::string("no CUDA device: ") + cudaGetErrorString(e));
@@ -467,7 +484,17 @@ static int build_cov(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
     prof = d_prof;
 #endif
     TEL_BEGIN(&h->tel, st);
-    if (k == kKnnRegK) {  // the reference's default reg_correspondence_randomness: lists live in registers
+    if (h->cfg.method == B2R_METHOD_GICP_PCL) {  // pcl GICP's raw-moment covariances (gicp_pcl.cuh)
+      if (k == kKnnRegK) {
+        k_pcl_cov_reg<kKnnRegK><<<(unsigned)(padded / kKnnThreads), kKnnThreads, 0, st>>>(c.bvh(), c.raw_view, c.stride_f, c.cov.p);
+      } else {
+        if (smem > 48 * 1024 && !h->pcl_knn_smem_attr) {  // the attribute belongs to the handle's device
+          B2R_CUDA(cudaFuncSetAttribute(k_pcl_cov, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * kKnnThreads * 8));
+          h->pcl_knn_smem_attr = true;
+        }
+        k_pcl_cov<<<(unsigned)(padded / kKnnThreads), kKnnThreads, smem, st>>>(c.bvh(), k, c.raw_view, c.stride_f, c.cov.p);
+      }
+    } else if (k == kKnnRegK) {  // the reference's default reg_correspondence_randomness: lists live in registers
       // On the PREFETCH stream the kernel works for the NEXT frame while the align chain of the current one runs beside it.  All of its
       // 512 blocks become resident at once (104 registers x 128 threads x ~3.9 blocks per SM on 132 SMs = 80 % of the register file) and
       // stay for the kernel's whole run — stream priorities only order PENDING blocks, so the chain's search kernels then run in what is left of each SM.
@@ -530,7 +557,7 @@ static int vgicp_ensure_map(b2r_handle* h, Cloud& c) {
 static int preprocess(b2r_handle* h, int which, bool is_target) {
   Cloud& c = h->clouds[which];
   if (h->cfg.method == B2R_METHOD_VGICP && is_target) return vgicp_ensure_map(h, c);
-  if (gicp_family(h->cfg.method)) {
+  if (cov_family(h->cfg.method)) {
     // a target gets its covariances now; a SOURCE only its search structure: its k-NN covariance kernel is launched by the align,
     // beside the first correspondence search, which does not read it (run_single_pair) — unless the cloud arrives through the
     // prefetch path, where both have been built ahead on the second stream
@@ -602,7 +629,7 @@ static int prefetch_source(b2r_handle* h, const void* pts, size_t n, size_t stri
   // align that has completed: b2r_align synchronises), so they are free to be overwritten here
   int rc = upload(h, h->nxt, pts, n, stride, dev, h->st2);
   if (rc) return rc;
-  if (gicp_family(h->cfg.method)) {
+  if (cov_family(h->cfg.method)) {
     rc = ensure_cov(h, h->clouds[h->nxt], 1);
     if (rc) return rc;
   }
@@ -936,6 +963,77 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out, const 
   return B2R_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ pcl GICP align (gicp_pcl.cuh)
+// the two device passes of B2R_METHOD_GICP_PCL over the handle's current source and target (covariances built)
+struct HandleGicpPclPasses {
+  b2r_handle* h;
+  explicit HandleGicpPclPasses(b2r_handle* h_) : h(h_) {}
+  int corr(const float* G, const float* T, const double* R, uint64_t* m) {
+    GicpPclWork& W = h->gp_work;
+    Cloud& s = SRC(h);
+    Cloud& t = TGT(h);
+    int rc = gicp_pcl_ensure_ws(W, (size_t)s.nsup * 1024, h->st);
+    if (rc) return rc;
+    gicp_pcl_fill_args(h->cfg, s, t, G, T, R, W.corr.p, W.M.p, W.A);
+    double cnt = 0.0;
+    W.corr_valid = false;
+    rc = gicp_pcl_run<1>(W, true, &h->tel, h->st, &cnt);
+    if (rc) return rc;
+    W.m = (uint64_t)cnt;
+    W.corr_valid = true;
+    h->corr_valid = true;
+    *m = W.m;
+    return B2R_OK;
+  }
+  int cost(const float* T, double* sums) {
+    GicpPclArgs& A = h->gp_work.A;
+    for (int i = 0; i < 12; i++) A.T[i] = T[i];
+    return gicp_pcl_run<kGicpPclSums>(h->gp_work, false, &h->tel, h->st, sums);
+  }
+};
+
+static void colmajor_to_row_f(const float* c, float* r) {
+  for (int i = 0; i < 4; i++)
+    for (int j = 0; j < 4; j++) r[i * 4 + j] = c[j * 4 + i];
+}
+
+// pcl::GeneralizedIterativeClosestPoint::align: the pair's GicpPclPairState (computeTransformation and PCL's BFGS on the host) asks for
+// one device pass at a time; every correspondence update and every functor evaluation is one pass whose sums come back through a
+// mapped message.  The batch runs the same state machine (batch_run_gicp_pcl_chunk).
+static int gicp_pcl_align(b2r_handle* h, const float* guess, b2r_result* out) {
+  Cloud& s = SRC(h);
+  Cloud& t = TGT(h);
+  float G[16];
+  colmajor_to_row_f(guess, G);
+  if (s.n == 0 || t.n == 0) {  // pcl::Registration::initCompute fails: converged_ = false
+    store_result(h, G, false, 0, out);
+    return B2R_OK;
+  }
+  int rc = ensure_cov(h, s);
+  if (!rc) rc = ensure_cov(h, t);
+  if (rc) return rc;
+  HandleGicpPclPasses P(h);
+  GicpPclPairState S;
+  S.start(h->cfg, G);
+  while (S.next() != GicpPclPairState::DONE) {
+    if (S.next() == GicpPclPairState::CORR) {
+      double R[9];
+      S.rel_rotation(R);
+      uint64_t m = 0;
+      rc = P.corr(G, S.T(), R, &m);
+      if (rc) return rc;
+      S.consume_corr(m);
+    } else {
+      double sums[kGicpPclSums];
+      rc = P.cost(S.T(), sums);
+      if (rc) return rc;
+      S.consume_cost(sums);
+    }
+  }
+  store_result(h, S.Tfinal, S.converged, S.nr_iterations, out);
+  return B2R_OK;
+}
+
 // b2r_align; `between` as in run_single_pair (GICP only: the NDT Newton loop is host-driven and has no single enqueue point)
 static int align_impl(b2r_handle* h, const float guess[16], b2r_result* out, const std::function<int()>* between) {
   if (!h || !guess) return fail(B2R_EINVAL, "NULL argument");
@@ -943,6 +1041,7 @@ static int align_impl(b2r_handle* h, const float guess[16], b2r_result* out, con
   int rc = need_source(h);
   if (rc != B2R_OK) {}  // reported below like every failed align
   else if (gicp_family(h->cfg.method)) rc = gicp_align(h, guess, out, between);
+  else if (h->cfg.method == B2R_METHOD_GICP_PCL) rc = gicp_pcl_align(h, guess, out);
   else {
     float Tfinal[16];
     bool conv = false;
@@ -1065,12 +1164,15 @@ extern "C" int b2r_target_nearest(b2r_handle* h, const void* queries, size_t n, 
   return B2R_OK;
 }
 
+static int gicp_pcl_fetch_correspondences(b2r_handle* h, int32_t* corr, double* M, size_t n);
+
 extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
   if (!h || !out) return fail(B2R_EINVAL, "NULL argument");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (need_source(h)) return B2R_ESTATE;
   if (!h->corr_valid) return fail(B2R_ESTATE, "no linearisation has run since the clouds were set");
   if (n != SRC(h).n) return fail(B2R_EINVAL, "n does not match the source cloud");
+  if (h->cfg.method == B2R_METHOD_GICP_PCL) return gicp_pcl_fetch_correspondences(h, out, nullptr, n);
   // a non-finite source point is not in the source's search structure (pos_of = -1): no search writes its entry, and like a PCL
   // query that finds nothing it has no correspondence
   std::vector<int> pos(n);
@@ -1084,7 +1186,7 @@ extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
 
 extern "C" int b2r_get_covariances(b2r_handle* h, int which, double* out, size_t n) {
   if (!h || !out) return fail(B2R_EINVAL, "NULL argument");
-  if (!gicp_family(h->cfg.method)) return fail(B2R_ESTATE, "covariances exist only for the GICP and VGICP engines");
+  if (!cov_family(h->cfg.method)) return fail(B2R_ESTATE, "covariances exist only for the GICP, VGICP and pcl GICP engines");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (!which && need_source(h)) return B2R_ESTATE;
   Cloud& c = which ? TGT(h) : SRC(h);
@@ -1148,6 +1250,74 @@ extern "C" int b2r_gicp_error_at(b2r_handle* h, const double T[16], double* err)
   if (rc) return rc;
   B2R_CUDA(cudaStreamSynchronize(h->st));
   *err = h->h_tap[28];
+  return B2R_OK;
+}
+
+// the last correspondence pass of a pcl GICP handle in the caller's point order: target index (-1 = none) and M (NaN where none)
+static int gicp_pcl_fetch_correspondences(b2r_handle* h, int32_t* corr, double* M, size_t n) {
+  Cloud& s = SRC(h);
+  GicpPclWork& W = h->gp_work;
+  const size_t padded = (size_t)s.nsup * 1024;
+  Cloud& t = TGT(h);
+  const size_t tpadded = (size_t)t.nsup * 1024;
+  std::vector<int> cs(padded + 1), pos(n + 1);
+  std::vector<float4> tsp(tpadded + 1);  // the target's sorted points: w carries the original index
+  std::vector<double> ms(M ? padded * 9 + 9 : 0);
+  if (n) {
+    B2R_CUDA(cudaMemcpyAsync(cs.data(), W.corr.p, padded * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    if (tpadded) B2R_CUDA(cudaMemcpyAsync(tsp.data(), t.sorted.p, tpadded * sizeof(float4), cudaMemcpyDeviceToHost, h->st));
+    B2R_CUDA(cudaMemcpyAsync(pos.data(), s.pos_of.p, n * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    if (M) B2R_CUDA(cudaMemcpyAsync(ms.data(), W.M.p, padded * 9 * sizeof(double), cudaMemcpyDeviceToHost, h->st));
+  }
+  B2R_CUDA(cudaStreamSynchronize(h->st));
+  for (size_t i = 0; i < n; i++) {
+    const int c = pos[i] >= 0 ? cs[pos[i]] : -1;  // a non-finite point is not in the source's structure: no correspondence
+    if (corr) corr[i] = c >= 0 ? idx_bits(tsp[c].w) : -1;
+    if (M)
+      for (int k = 0; k < 9; k++) M[i * 9 + k] = c >= 0 ? ms[(size_t)pos[i] * 9 + k] : NAN;
+  }
+  return B2R_OK;
+}
+
+extern "C" int b2r_gicp_pcl_correspondences_at(b2r_handle* h, const float guess[16], const float T_rel[16], int32_t* corr, double* M, uint64_t* n_corr) {
+  if (!h || !guess || !T_rel || !n_corr) return fail(B2R_EINVAL, "NULL argument");
+  if (h->cfg.method != B2R_METHOD_GICP_PCL) return fail(B2R_ESTATE, "pcl GICP engine (B2R_METHOD_GICP_PCL) required");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (need_source(h)) return B2R_ESTATE;
+  Cloud& s = SRC(h);
+  Cloud& t = TGT(h);
+  if (s.n == 0 || t.n == 0) return fail(B2R_ESTATE, "source/target not set");
+  int rc = ensure_cov(h, s);
+  if (!rc) rc = ensure_cov(h, t);
+  if (rc) return rc;
+  float G[16], T[16];
+  colmajor_to_row_f(guess, G);
+  colmajor_to_row_f(T_rel, T);
+  double R[9];
+  gicp_pcl_rel_rotation(T, G, R);
+  HandleGicpPclPasses P(h);
+  uint64_t m = 0;
+  rc = P.corr(G, T, R, &m);
+  if (rc) return rc;
+  *n_corr = m;
+  return (corr || M) ? gicp_pcl_fetch_correspondences(h, corr, M, s.n) : B2R_OK;
+}
+
+extern "C" int b2r_gicp_pcl_cost_at(b2r_handle* h, const float T[16], double* f_sum, double* g_sum, double* dR_sum) {
+  if (!h || !T || !f_sum || !g_sum || !dR_sum) return fail(B2R_EINVAL, "NULL argument");
+  if (h->cfg.method != B2R_METHOD_GICP_PCL) return fail(B2R_ESTATE, "pcl GICP engine (B2R_METHOD_GICP_PCL) required");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (need_source(h)) return B2R_ESTATE;
+  if (!h->corr_valid || !h->gp_work.corr_valid) return fail(B2R_ESTATE, "no correspondence pass has run since the clouds were set");
+  float Tr[16];
+  colmajor_to_row_f(T, Tr);
+  double sums[kGicpPclSums];
+  HandleGicpPclPasses P(h);
+  int rc = P.cost(Tr, sums);
+  if (rc) return rc;
+  *f_sum = sums[0];
+  for (int i = 0; i < 3; i++) g_sum[i] = sums[1 + i];
+  for (int i = 0; i < 9; i++) dR_sum[i] = sums[4 + i];
   return B2R_OK;
 }
 

@@ -75,6 +75,10 @@ struct b2r_batch {
   MappedBuf<double> h_ndt_msg;      // one result message per record of the round, then the round's flag (8 doubles)
   DevBuf<unsigned int> d_ndt_round; // messages of the current round (the last one publishes the flag and re-arms it)
   unsigned long long ndt_seq = 0;
+  // pcl GICP batch (batch_run_gicp_pcl_chunk): its rounds publish through h_ndt_msg / d_ndt_round / ndt_seq like the NDT rounds
+  DevBuf<char> gp_ws;               // per pair in flight: correspondences, M, reduction partials and counter; fitness partials
+  DevBuf<GicpPclArgs> d_gp_args;    // the round's pass records: correspondence passes first, then cost passes
+  PinnedBuf<GicpPclArgs> h_gp_args; // staging
   // telemetry of the last b2r_batch_align
   unsigned long long last_rounds = 0, last_pair_rounds = 0;
   ~b2r_batch() {  // what is not a plain free; the members then go in reverse order, the engine last
@@ -278,7 +282,10 @@ static int batch_build_structures(b2r_batch* b, const int32_t* ids, size_t n_ids
   }
   B2R_CUDA(cudaMemcpyAsync(b->d_knn.p, b->h_knn.p, todo.size() * sizeof(KnnBatchItem), cudaMemcpyHostToDevice, st));
   { TEL_BEGIN(&h->tel, st);
-    k_knn_cov_reg_batch<kKnnRegK><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
+    if (h->cfg.method == B2R_METHOD_GICP_PCL)  // pcl GICP's raw-moment covariances (gicp_pcl.cuh)
+      k_pcl_cov_reg_batch<kKnnRegK><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
+    else
+      k_knn_cov_reg_batch<kKnnRegK><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
     TEL_END(&h->tel, KC_KNN_COV, 1, st); }
   B2R_CUDA(cudaGetLastError());
   for (Cloud* c : todo) c->cov_ready = true;
@@ -531,6 +538,37 @@ static int batch_ndt_maps(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, b
   return B2R_OK;
 }
 
+// getFitnessScore at each pair's final pose (T[i]: row-major, the first 12 floats are read): the kernel and reduction of b2r_fitness,
+// one launch per pair, one wait for all.  base + fit_off[i]: the pair's k_fitness partials, then its counter (zeroed); base + fit_out:
+// 3 doubles per pair.  fit[3 i ..] = sum d2, count, inliers.
+static int batch_fitness_at(b2r_batch* b, const b2r_pair* pairs, size_t m, const std::vector<const float*>& T, char* base,
+                            const std::vector<size_t>& fit_off, size_t fit_out, double fit_max_range, std::vector<double>& fit) {
+  b2r_handle* h = b->eng.get();
+  cudaStream_t st = h->st;
+  double* d_fit = reinterpret_cast<double*>(base + fit_out);
+  for (size_t i = 0; i < m; i++) {
+    Cloud& s = *b->clouds[pairs[i].source];
+    Cloud& t = *b->clouds[pairs[i].target];
+    if (s.n == 0 || t.n == 0) continue;
+    const size_t nb = (size_t)s.nsup * 1024 / kLinThreads;
+    FitArgs A;
+    A.src = s.bvh(); A.tgt = t.bvh();
+    for (int k = 0; k < 12; k++) A.Tf[k] = T[i][k];
+    A.max_range = fit_max_range; A.inlier_thresh_sq = 0.25f;
+    A.partials = reinterpret_cast<double*>(base + fit_off[i]);
+    A.counter = reinterpret_cast<unsigned int*>(base + fit_off[i] + align_up(nb * 3 * sizeof(double), 256));
+    A.out = d_fit + 3 * i;
+    TEL_BEGIN(&h->tel, st);
+    k_fitness<<<(unsigned)nb, kLinThreads, 0, st>>>(A);
+    TEL_END(&h->tel, KC_FITNESS, 1, st);
+    B2R_CUDA(cudaGetLastError());
+  }
+  B2R_CUDA(cudaMemcpyAsync(fit.data(), d_fit, m * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
+  B2R_CUDA(cudaStreamSynchronize(st));
+  h->tel.d2h += m * 3 * sizeof(double);
+  return B2R_OK;
+}
+
 constexpr int kNdtMsg = 48;  // doubles per result message: kNdtAcc sums (or 36 Hessian entries), pair count, checksum
 
 // per pair in flight: [chunks + 1][kNdtAcc] chunk rows (also the Hessian pass's [blocks][36]), [groups][kNdtAcc] group rows,
@@ -673,30 +711,12 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       if (S[i].next() != NDT_PASS_DONE) active[keep++] = i;
     active.resize(keep);
   }
-  // getFitnessScore at each final pose: the kernel and reduction of b2r_fitness, one launch per pair, one wait for all
   std::vector<double> fit(m * 3, 0.0);
   if (want_fitness) {
-    double* d_fit = reinterpret_cast<double*>(base + fit_out);
-    for (size_t i = 0; i < m; i++) {
-      Cloud& s = *b->clouds[pairs[i].source];
-      Cloud& t = *b->clouds[pairs[i].target];
-      if (s.n == 0 || t.n == 0) continue;
-      const size_t nb = (size_t)s.nsup * 1024 / kLinThreads;
-      FitArgs A;
-      A.src = s.bvh(); A.tgt = t.bvh();
-      for (int k = 0; k < 12; k++) A.Tf[k] = S[i].Tfinal[k];
-      A.max_range = fit_max_range; A.inlier_thresh_sq = 0.25f;
-      A.partials = reinterpret_cast<double*>(base + fit_off[i]);
-      A.counter = reinterpret_cast<unsigned int*>(base + fit_off[i] + align_up(nb * 3 * sizeof(double), 256));
-      A.out = d_fit + 3 * i;
-      TEL_BEGIN(&h->tel, st);
-      k_fitness<<<(unsigned)nb, kLinThreads, 0, st>>>(A);
-      TEL_END(&h->tel, KC_FITNESS, 1, st);
-      B2R_CUDA(cudaGetLastError());
-    }
-    B2R_CUDA(cudaMemcpyAsync(fit.data(), d_fit, m * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    B2R_CUDA(cudaStreamSynchronize(st));
-    h->tel.d2h += m * 3 * sizeof(double);
+    std::vector<const float*> T(m);
+    for (size_t i = 0; i < m; i++) T[i] = S[i].Tfinal;
+    int rc = batch_fitness_at(b, pairs, m, T, base, fit_off, fit_out, fit_max_range, fit);
+    if (rc) return rc;
   }
   for (size_t i = 0; i < m; i++) {
     PairReport& R = rep[i];
@@ -708,6 +728,146 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
     R.r.converged = S[i].converged ? 1 : 0;
     R.r.iterations = S[i].nr_iterations;
     R.rounds = S[i].passes;
+  }
+  return B2R_OK;
+}
+
+// per pair in flight: correspondences [n_pad] ints, M [n_pad][9], reduction partials [blocks][13], then the counter — zero at the start
+struct GicpPclPairWs { size_t corr, M, partials, counter, bytes; };
+static GicpPclPairWs gicp_pcl_pair_ws(const Cloud& s) {
+  const size_t n = (size_t)s.nsup * 1024, nb = n / kGicpPclThreads;
+  GicpPclPairWs w;
+  w.corr = 0;
+  w.M = align_up(n * sizeof(int), 256);
+  w.partials = w.M + align_up(n * 9 * sizeof(double), 256);
+  w.counter = w.partials + align_up(nb * kGicpPclSums * sizeof(double), 256);
+  w.bytes = w.counter + 256;
+  return w;
+}
+
+// pairs[0..m) of a pcl GICP batch -> rep[0..m) (host).  Every pair runs the single handle's GicpPclPairState; a round gathers the
+// pass each active pair asks for into at most two launches (correspondence passes, cost passes; blockIdx.y = pair), waits once for
+// the round's flag and hands every pair its result.  A pair reduces through its own partials and counter, exactly as alone.
+static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, double fit_max_range, PairReport* rep) {
+  b2r_handle* h = b->eng.get();
+  cudaStream_t st = h->st;
+  const b2r_config& cfg = h->cfg;
+  std::vector<GicpPclPairState> S(m);
+  std::vector<char> started(m, 0);
+  std::vector<float> G(m * 16);
+  std::vector<size_t> active, off(m, 0), fit_off(m, 0);
+  size_t ws = 0;
+  for (size_t i = 0; i < m; i++) {
+    for (int r = 0; r < 4; r++)
+      for (int c = 0; c < 4; c++) G[i * 16 + r * 4 + c] = pairs[i].guess[c * 4 + r];
+    Cloud& s = *b->clouds[pairs[i].source];
+    Cloud& t = *b->clouds[pairs[i].target];
+    if (s.n == 0 || t.n == 0) continue;  // initCompute fails: the guess, not converged, no iteration (as gicp_pcl_align)
+    fit_off[i] = ws;
+    ws += align_up((size_t)s.nsup * 1024 / kLinThreads * 3 * sizeof(double), 256) + 256;
+    S[i].start(cfg, &G[i * 16]);
+    started[i] = 1;
+    active.push_back(i);
+    off[i] = ws;
+    ws += gicp_pcl_pair_ws(s).bytes;
+  }
+  const size_t fit_out = ws;
+  ws += align_up(m * 3 * sizeof(double), 256);
+  B2R_CUDA(b->gp_ws.reserve(ws + 256));
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->gp_ws.p), 256));
+  B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
+  B2R_CUDA(b->d_gp_args.reserve(m));
+  if (b->h_gp_args.cap < m) B2R_CUDA(b->h_gp_args.alloc(m));
+  if (b->h_ndt_msg.cap < m * kNdtMsg + 8) {
+    B2R_CUDA(b->h_ndt_msg.alloc(m * kNdtMsg + 8));
+    std::memset(b->h_ndt_msg.p, 0, b->h_ndt_msg.cap * sizeof(double));
+  }
+  const size_t flag_at = b->h_ndt_msg.cap - 8;
+  unsigned long long* flag = reinterpret_cast<unsigned long long*>(b->h_ndt_msg.p + flag_at);
+  unsigned long long* flag_dev = reinterpret_cast<unsigned long long*>(b->h_ndt_msg.d + flag_at);
+  std::vector<size_t> order;
+  std::vector<int> kind_of;
+  while (!active.empty()) {
+    order.clear(); kind_of.clear();
+    size_t cnt[2] = {0, 0};
+    unsigned max_nb[2] = {0, 0};
+    for (int k = 0; k < 2; k++)
+      for (size_t i : active)
+        if ((S[i].next() == GicpPclPairState::CORR) == (k == 0)) {
+          order.push_back(i); kind_of.push_back(k); cnt[k]++;
+          max_nb[k] = std::max(max_nb[k], (unsigned)((size_t)b->clouds[pairs[i].source]->nsup * 1024 / kGicpPclThreads));
+        }
+    const unsigned long long seq = ++b->ndt_seq;
+    for (size_t r = 0; r < order.size(); r++) {
+      const size_t i = order[r];
+      Cloud& s = *b->clouds[pairs[i].source];
+      Cloud& t = *b->clouds[pairs[i].target];
+      const GicpPclPairWs w = gicp_pcl_pair_ws(s);
+      char* p = base + off[i];
+      double R[9];
+      S[i].rel_rotation(R);
+      GicpPclArgs& A = b->h_gp_args.p[r];
+      gicp_pcl_fill_args(cfg, s, t, S[i].guess(), S[i].T(), R, reinterpret_cast<int*>(p + w.corr), reinterpret_cast<double*>(p + w.M), A);
+      A.partials = reinterpret_cast<double*>(p + w.partials);
+      A.counter = reinterpret_cast<unsigned int*>(p + w.counter);
+      A.out = b->h_ndt_msg.d + r * kNdtMsg;
+      A.flag = flag_dev;
+      A.seq = seq;
+      A.round = b->d_ndt_round.p;
+      A.round_n = (unsigned)order.size();
+      A.nrow = (unsigned)((size_t)s.nsup * 1024 / kGicpPclThreads);
+    }
+    B2R_CUDA(cudaMemcpyAsync(b->d_gp_args.p, b->h_gp_args.p, order.size() * sizeof(GicpPclArgs), cudaMemcpyHostToDevice, st));
+    h->tel.h2d += order.size() * sizeof(GicpPclArgs);
+    if (cnt[0]) {
+      TEL_BEGIN(&h->tel, st);
+      k_gicp_pcl_corr_batch<<<dim3(max_nb[0], (unsigned)cnt[0]), kGicpPclThreads, 0, st>>>(b->d_gp_args.p);
+      TEL_END(&h->tel, KC_GICP_PCL_CORR, 1, st);
+      B2R_CUDA(cudaGetLastError());
+    }
+    if (cnt[1]) {
+      TEL_BEGIN(&h->tel, st);
+      k_gicp_pcl_cost_batch<<<dim3(max_nb[1], (unsigned)cnt[1]), kGicpPclThreads, 0, st>>>(b->d_gp_args.p + cnt[0]);
+      TEL_END(&h->tel, KC_GICP_PCL_COST, 1, st);
+      B2R_CUDA(cudaGetLastError());
+    }
+    h->tel.d2h += order.size() * (kGicpPclSums + 2) * sizeof(double);
+    b->last_rounds++;
+    for (size_t r = 0; r < order.size(); r++) {  // the first wait covers the round; the rest only check each message
+      const double* msg = b->h_ndt_msg.p + r * kNdtMsg;
+      GicpPclPairState& P = S[order[r]];
+      if (kind_of[r] == 0) {
+        int rc = wait_host_result(flag, seq, msg, 1, false, st);
+        if (rc) return rc;
+        P.consume_corr((uint64_t)msg[0]);
+      } else {
+        int rc = wait_host_result(flag, seq, msg, kGicpPclSums, false, st);
+        if (rc) return rc;
+        P.consume_cost(msg);
+      }
+    }
+    size_t keep = 0;
+    for (size_t i : active)
+      if (S[i].next() != GicpPclPairState::DONE) active[keep++] = i;
+    active.resize(keep);
+  }
+  std::vector<const float*> T(m);
+  for (size_t i = 0; i < m; i++) T[i] = started[i] ? S[i].Tfinal : &G[i * 16];
+  std::vector<double> fit(m * 3, 0.0);
+  if (want_fitness) {
+    int rc = batch_fitness_at(b, pairs, m, T, base, fit_off, fit_out, fit_max_range, fit);
+    if (rc) return rc;
+  }
+  for (size_t i = 0; i < m; i++) {
+    PairReport& R = rep[i];
+    std::memset(&R, 0, sizeof(R));
+    for (int r = 0; r < 4; r++)
+      for (int c = 0; c < 4; c++) R.r.T[c * 4 + r] = T[i][r * 4 + c];
+    const double nr = fit[3 * i + 1];
+    R.r.fitness = !want_fitness ? NAN : (nr > 0 ? fit[3 * i] / nr : DBL_MAX);
+    R.r.converged = (started[i] && S[i].converged) ? 1 : 0;
+    R.r.iterations = started[i] ? S[i].nr_iterations : 0;
+    R.rounds = started[i] ? S[i].corr_passes + S[i].cost_passes : 0;
   }
   return B2R_OK;
 }
@@ -743,6 +903,7 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   if (ndt) rc = batch_ndt_maps(b, pairs, n_pairs, fit_only);
   if (rc) return rc;
   const bool vgicp = h->cfg.method == B2R_METHOD_VGICP && !fit_only;
+  const bool gpcl = h->cfg.method == B2R_METHOD_GICP_PCL && !fit_only;  // host-driven rounds, like NDT
   if (vgicp) rc = batch_vgicp_maps(b, pairs, n_pairs);
   if (rc) return rc;
   const auto t_b = std::chrono::steady_clock::now();
@@ -757,12 +918,13 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
     const size_t m = std::min(chunk, n_pairs - c0);
     // an NDT align runs its own rounds; a stand-alone fitness evaluation is the same search on either engine
     if (ndt && !fit_only) rc = batch_run_ndt_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
+    else if (gpcl) rc = batch_run_gicp_pcl_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
     else rc = batch_run_chunk(b, pairs + c0, m, cfg, b->d_reports.p + c0, fit_only);
     if (rc) return rc;
   }
   if (vgicp && want_fitness) rc = batch_vgicp_fitness(b, pairs, n_pairs, fit_max_range, b->d_reports.p);
   if (rc) return rc;
-  if (ndt && !fit_only)  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
+  if ((ndt && !fit_only) || gpcl)  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
     B2R_CUDA(cudaMemcpyAsync(b->d_reports.p, b->h_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyHostToDevice, h->st));
   if (dbg) {
     const auto t_c = std::chrono::steady_clock::now();

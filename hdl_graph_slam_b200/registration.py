@@ -18,7 +18,7 @@ library; nothing here computes.
 import ctypes as C
 import numpy as np
 from . import _capi
-from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP  # noqa: F401
+from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL  # noqa: F401
 
 
 def _cloud(a):
@@ -284,6 +284,29 @@ class Registration:
         check(self._lib.b2r_vgicp_linearize_at(self._h, t.ctypes.data_as(dp), H.ctypes.data_as(dp), b.ctypes.data_as(dp), C.byref(cost), C.byref(nc),
                                                vox.ctypes.data_as(C.POINTER(C.c_int32)), n_source))
         return H, b, cost.value, nc.value, vox[:n_source]
+
+    def gicpPclCorrespondencesAt(self, guess, T_rel, n_source):
+        """(pcl GICP) one correspondence pass at (guess, T_rel): (target index of every source point (n,) int32, -1 = none,
+        Mahalanobis matrices (n, 3, 3), NaN where there is none, accepted count)"""
+        g = _colmajor(guess, np.float32)
+        t = _colmajor(T_rel, np.float32)
+        corr = np.empty(max(n_source, 1), np.int32)
+        M = np.empty((max(n_source, 1), 3, 3), np.float64)
+        nc = C.c_uint64()
+        fp = C.POINTER(C.c_float)
+        check(self._lib.b2r_gicp_pcl_correspondences_at(self._h, g.ctypes.data_as(fp), t.ctypes.data_as(fp), corr.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                        M.ctypes.data_as(C.POINTER(C.c_double)), C.byref(nc)))
+        return corr[:n_source], M[:n_source], nc.value
+
+    def gicpPclCostAt(self, T):
+        """(pcl GICP) one cost pass at T over the last correspondences: (sum res^T M res, sum M res (3,), sum p (M res)^T (3, 3))"""
+        t = _colmajor(T, np.float32)
+        f = C.c_double()
+        g = np.empty(3, np.float64)
+        dR = np.empty((3, 3), np.float64)
+        dp = C.POINTER(C.c_double)
+        check(self._lib.b2r_gicp_pcl_cost_at(self._h, t.ctypes.data_as(C.POINTER(C.c_float)), C.byref(f), g.ctypes.data_as(dp), dR.ctypes.data_as(dp)))
+        return f.value, g, dR
 
     # --- companion / prefilter chain
     def _filter(self, fn, cloud, *args):

@@ -52,6 +52,11 @@ extern "C" {
 #define B2R_METHOD_VGICP 3 /* fast_gicp::FastVGICP semantics (registrations.cpp:48-56): FastGICP's covariances, the target's Gaussian voxel
                               map at ndt_resolution (reg_resolution), DIRECT1 voxel correspondences, weights sqrt(num_points); reads
                               max_iterations / k_correspondences / transformation_epsilon, not max_correspondence_distance */
+#define B2R_METHOD_GICP_PCL 4 /* pcl::GeneralizedIterativeClosestPoint semantics (PCL 1.10, registrations.cpp:66-76): raw-moment k-NN
+                                 covariances, exact 1-NN Mahalanobis correspondences, PCL's BFGS over (t, euler ZYX); reads
+                                 max_iterations / k_correspondences / transformation_epsilon / max_correspondence_distance /
+                                 max_optimizer_iterations; rotation_epsilon stays 2e-3.  The BFGS runs on the host (one device pass per correspondence
+                                 update and per functor evaluation); a batch gathers every pair's pass of a round into shared launches */
 
 typedef struct b2r_handle b2r_handle;
 
@@ -71,6 +76,8 @@ typedef struct b2r_config {
   int32_t ndt_mt_interval_flag;       /* 0 = ndt_omp polarity (More-Thuente loop never entered), 1 = active line search */
   int32_t ndt_fixed_iterations;       /* >0: exactly this many iterations (BASELINE config 3), convergence test off */
   float grid_cell_min;                /* engine tuning: smallest search-grid cell, power of two (default 0.5 m) */
+  int32_t max_optimizer_iterations;   /* reg_max_optimizer_iterations      (20)   pcl GICP max_inner_iterations_ (B2R_METHOD_GICP_PCL) */
+  int32_t reserved;                   /* explicit padding to a multiple of 8 bytes */
 } b2r_config;
 
 /* What the callers read back after align(): getFinalTransformation(), hasConverged(), and (loop closure)
@@ -91,8 +98,10 @@ int b2r_config_default(b2r_config* cfg, int method);
 /* replaces select_registration_method(ros::NodeHandle&) (registrations.cpp:22-124): same parameter NAMES and defaults,
  * passed as string key/value pairs (the rosparam namespace of the nodelet).  "FAST_GICP"/"B200_GICP" -> GICP engine,
  * "NDT_OMP"/"B200_NDT" -> NDT engine, "NDT" -> pcl NDT engine (B2R_METHOD_NDT_PCL), "FAST_VGICP"/"B200_VGICP" -> VGICP engine
- * (B2R_METHOD_VGICP).  ICP / GICP / GICP_OMP / FAST_VGICP_CUDA and unknown names are not re-created: returns B2R_EUNSUPPORTED so
- * the caller keeps the reference's own branch. */
+ * (B2R_METHOD_VGICP), "GICP"/"B200_GICP_PCL" and every other name that reaches the reference's GICP branch (contains "GICP" but not
+ * "OMP") -> pcl GICP engine (B2R_METHOD_GICP_PCL).  ICP / GICP_OMP / FAST_VGICP_CUDA and unknown names are not re-created: returns
+ * B2R_EUNSUPPORTED so the caller keeps the reference's own branch.  (Built without USE_VGICP_CUDA the reference sends FAST_VGICP_CUDA to
+ * its GICP branch; this factory refuses it all the same, so the caller decides.) */
 int b2r_select_registration_method(const char* const* keys, const char* const* values, int n_params, int device_id,
                                    b2r_handle** out);
 
@@ -191,6 +200,16 @@ int b2r_vgicp_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int32
  * *cost = sum sqrt(num_points) e^T M e, *n_corr = source points with a voxel, voxel_of (n source entries in the caller's point order,
  * may be NULL) = the index of the point's voxel in b2r_vgicp_get_voxels' order, or -1 */
 int b2r_vgicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* cost, uint64_t* n_corr, int32_t* voxel_of, size_t n);
+
+/* B2R_METHOD_GICP_PCL: one correspondence pass of pcl GICP's computeTransformation at the guess (applied to the source first,
+ * transformPointCloud) and T_rel (transformation_), both column-major float: corr[n] (caller's point order, may be NULL) = the target
+ * index of the exact 1-NN when its squared distance < max_correspondence_distance^2, else -1; M[9 n] (may be NULL) = the Mahalanobis
+ * matrix (R C1 R^T + C2)^-1, 3x3 row-major, of every accepted point (NaN elsewhere); *n_corr = the accepted count.  The cost tap below
+ * reads these correspondences. */
+int b2r_gicp_pcl_correspondences_at(b2r_handle* h, const float guess[16], const float T_rel[16], int32_t* corr, double* M, uint64_t* n_corr);
+/* B2R_METHOD_GICP_PCL: one cost pass (OptimizationFunctorWithIndices) at the column-major float pose T over the last correspondences:
+ * *f_sum = sum res^T M res, g_sum[3] = sum M res, dR_sum[9] = sum p_src (M res)^T (row-major), unscaled (the functor divides by m) */
+int b2r_gicp_pcl_cost_at(b2r_handle* h, const float T[16], double* f_sum, double* g_sum, double* dR_sum);
 
 /* ---- companion: voxel-grid downsample ---------------------------------------------------------------------------
  * replaces pcl::VoxelGrid<PointXYZI>::filter with setLeafSize(leaf,leaf,leaf) (apps/prefiltering_nodelet.cpp:54-58,138-149;
@@ -379,6 +398,9 @@ int b2r_loop_matching(b2r_handle* h, const void* new_keyframe, size_t n_new, siz
  * Newton / More-Thuente driver and each round of derivative passes covers every pair in flight (one host wait per round).
  * Pose, flag, iteration count and fitness are bitwise those of b2r_set_target / b2r_set_source / b2r_align / b2r_fitness on
  * one NDT handle; b2r_batch_last_rounds counts batched rounds and, per pair, derivative / Hessian passes.
+ * pcl GICP config (B2R_METHOD_GICP_PCL): every pair runs the single handle's computeTransformation / BFGS driver and each round has at
+ * most one batched correspondence launch and one batched cost launch (one host wait per round); the records are bitwise the single
+ * handle's, and b2r_batch_last_rounds counts, per pair, correspondence and cost passes.
  *
  * Host buffers passed to b2r_batch_add_cloud may be pageable (copied before the call returns) or pinned (DMA'd in place:
  * keep them unmodified until the next b2r_batch_align / b2r_batch_loop_detect / b2r_batch_synchronize returns). */
