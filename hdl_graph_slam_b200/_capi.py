@@ -8,7 +8,7 @@ LIB_PATH = os.environ.get("B2R_LIB") or os.path.join(_HERE, "_lib", "libb200reg.
 
 B2R_OK = 0
 B2R_EINVAL, B2R_ENODEVICE, B2R_ECUDA, B2R_ESTATE, B2R_EUNSUPPORTED, B2R_ENCCL = -1, -2, -3, -4, -5, -6
-B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL = 0, 1, 2, 3, 4
+B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL = 0, 1, 2, 3, 4, 5
 B2R_DOWNSAMPLE_NONE, B2R_DOWNSAMPLE_VOXELGRID, B2R_DOWNSAMPLE_APPROX_VOXELGRID = 0, 1, 2
 
 
@@ -18,7 +18,7 @@ class Config(C.Structure):
         ("transformation_epsilon", C.c_double), ("rotation_epsilon", C.c_double), ("max_correspondence_distance", C.c_double),
         ("ndt_resolution", C.c_double), ("ndt_step_size", C.c_double), ("ndt_outlier_ratio", C.c_double),
         ("ndt_search_method", C.c_int32), ("ndt_mt_interval_flag", C.c_int32), ("ndt_fixed_iterations", C.c_int32),
-        ("grid_cell_min", C.c_float), ("max_optimizer_iterations", C.c_int32), ("reserved", C.c_int32),
+        ("grid_cell_min", C.c_float), ("max_optimizer_iterations", C.c_int32), ("use_reciprocal_correspondences", C.c_int32),
     ]
 
 
@@ -123,6 +123,8 @@ SYMBOLS = [
     ("b2r_vgicp_linearize_at", C.c_int, [_VP, _F64P, _F64P, _F64P, _F64P, C.POINTER(C.c_uint64), C.POINTER(C.c_int32), _SZ]),
     ("b2r_gicp_pcl_correspondences_at", C.c_int, [_VP, _F32P, _F32P, C.POINTER(C.c_int32), _F64P, C.POINTER(C.c_uint64)]),
     ("b2r_gicp_pcl_cost_at", C.c_int, [_VP, _F32P, _F64P, _F64P, _F64P]),
+    ("b2r_icp_pcl_correspondences_at", C.c_int, [_VP, _F32P, _I32P, _F32P, C.POINTER(C.c_uint64)]),
+    ("b2r_icp_pcl_estimate_at", C.c_int, [_VP, _F32P, _F32P, _F64P]),
     ("b2r_voxelgrid", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_float, _VP, C.POINTER(_SZ), _I32P, _I32P]),
     ("b2r_voxelgrid_device", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_float, C.POINTER(_VP), C.POINTER(_SZ)]),
     ("b2r_approximate_voxelgrid", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_float, _VP, C.POINTER(_SZ), _I32P]),

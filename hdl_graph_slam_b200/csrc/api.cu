@@ -6,6 +6,7 @@
 //   b2r_align                       <- pcl::Registration::align -> computeTransformation (fast_gicp LsqRegistration LM loop,
 //                                      ndt_omp Newton + More-Thuente loop; SURVEY.md A.2, A.4)
 //                                      (pcl::GeneralizedIterativeClosestPoint BFGS loop: gicp_pcl.cuh)
+//                                      (pcl::IterativeClosestPoint loop: icp_pcl.cuh)
 //   b2r_fitness                     <- getFitnessScore
 //   b2r_odometry_matching           <- ScanMatchingOdometryNodelet::matching  apps/scan_matching_odometry_nodelet.cpp:165-262
 //   b2r_loop_matching               <- LoopDetector::matching                include/hdl_graph_slam/loop_detector.hpp:117-171
@@ -27,6 +28,7 @@
 #include "ndt.cuh"
 #include "vgicp.cuh"
 #include "gicp_pcl.cuh"
+#include "icp_pcl.cuh"
 #include "voxelgrid.cuh"
 #include "approx_voxelgrid.cuh"
 #include "prefilter.cuh"
@@ -106,6 +108,9 @@ struct b2r_handle {
   NdtWork ndt_work;
   VoxelWork vg_work;
   GicpPclWork gp_work;              // B2R_METHOD_GICP_PCL: correspondence / cost pass buffers
+  DevBuf<char> icp_ws;              // B2R_METHOD_ICP_PCL: the pair's workspace (icp_pair_ws)
+  DevBuf<IcpPairDev> icp_pair;      // B2R_METHOD_ICP_PCL: the pair's record
+  PinnedBuf<IcpPairDev> icp_h;      // its host copy
   Telemetry tel;
 };
 
@@ -114,7 +119,7 @@ static Cloud& SRC(b2r_handle* h) { return h->clouds[h->src]; }
 static bool gicp_family(int method) { return method == B2R_METHOD_GICP || method == B2R_METHOD_VGICP; }
 // the methods whose clouds carry k-NN covariances: FastGICP's, or pcl GICP's raw-moment ones (B2R_METHOD_GICP_PCL)
 static bool cov_family(int method) { return gicp_family(method) || method == B2R_METHOD_GICP_PCL; }
-static bool known_method(int method) { return cov_family(method) || ndt_family(method); }
+static bool known_method(int method) { return cov_family(method) || ndt_family(method) || method == B2R_METHOD_ICP_PCL; }
 static Cloud& TGT(b2r_handle* h) { return h->clouds[h->tgt]; }
 
 extern "C" const char* b2r_last_error(void) { return g_last_error.c_str(); }
@@ -138,6 +143,7 @@ extern "C" int b2r_config_default(b2r_config* c, int method) {
   c->ndt_fixed_iterations = 0;
   c->grid_cell_min = 0.5f;
   c->max_optimizer_iterations = 20;   // :75
+  c->use_reciprocal_correspondences = 0;  // :64 (false)
   if (!known_method(method)) return fail(B2R_EINVAL, "unknown method");
   return B2R_OK;
 }
@@ -197,6 +203,18 @@ extern "C" int b2r_select_registration_method(const char* const* keys, const cha
     c.max_correspondence_distance = dparam("reg_max_correspondence_distance", 2.5);
     c.k_correspondences = iparam("reg_correspondence_randomness", 20);
     c.max_optimizer_iterations = iparam("reg_max_optimizer_iterations", 20);
+  } else if (method == "B200_ICP") {
+    // registrations.cpp:57-65: pcl::IterativeClosestPoint with transformation epsilon, maximum iterations, correspondence distance and
+    // the reciprocal check.  The plain name ICP stays with the reference's own branch until integrators have moved to this one
+    b2r_config_default(&c, B2R_METHOD_ICP_PCL);
+    c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
+    c.max_iterations = iparam("reg_maximum_iterations", 64);
+    c.max_correspondence_distance = dparam("reg_max_correspondence_distance", 2.5);
+    const char* r = find_param(keys, values, n, "reg_use_reciprocal_correspondences");
+    const std::string rs = r ? r : "false";
+    if (rs == "true" || rs == "1") c.use_reciprocal_correspondences = 1;
+    else if (rs == "false" || rs == "0") c.use_reciprocal_correspondences = 0;
+    else return fail(B2R_EINVAL, "reg_use_reciprocal_correspondences must be true, false, 1 or 0");
   } else {
     return fail(B2R_EUNSUPPORTED, "registration_method '" + method + "' is not re-created by b200reg; keep the reference branch");
   }
@@ -217,6 +235,8 @@ extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
     return fail(B2R_EINVAL, "VGICP: ndt_resolution (reg_resolution) must be finite and positive");
   if (cfg->k_correspondences < 1 || cfg->k_correspondences > 64) return fail(B2R_EINVAL, "k_correspondences must be in [1,64]");
   if (cfg->method == B2R_METHOD_GICP_PCL && cfg->max_optimizer_iterations < 1) return fail(B2R_EINVAL, "max_optimizer_iterations must be >= 1");
+  if (cfg->method == B2R_METHOD_ICP_PCL && cfg->use_reciprocal_correspondences != 0 && cfg->use_reciprocal_correspondences != 1)
+    return fail(B2R_EINVAL, "use_reciprocal_correspondences must be 0 or 1");
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev <= 0) return fail(B2R_ENODEVICE, std::string("no CUDA device: ") + cudaGetErrorString(e));
@@ -557,6 +577,7 @@ static int vgicp_ensure_map(b2r_handle* h, Cloud& c) {
 static int preprocess(b2r_handle* h, int which, bool is_target) {
   Cloud& c = h->clouds[which];
   if (h->cfg.method == B2R_METHOD_VGICP && is_target) return vgicp_ensure_map(h, c);
+  if (h->cfg.method == B2R_METHOD_ICP_PCL) return ensure_grid(h, c);  // ICP reads the search structures only
   if (cov_family(h->cfg.method)) {
     // a target gets its covariances now; a SOURCE only its search structure: its k-NN covariance kernel is launched by the align,
     // beside the first correspondence search, which does not read it (run_single_pair) — unless the cloud arrives through the
@@ -631,6 +652,9 @@ static int prefetch_source(b2r_handle* h, const void* pts, size_t n, size_t stri
   if (rc) return rc;
   if (cov_family(h->cfg.method)) {
     rc = ensure_cov(h, h->clouds[h->nxt], 1);
+    if (rc) return rc;
+  } else if (h->cfg.method == B2R_METHOD_ICP_PCL) {
+    rc = ensure_grid(h, h->clouds[h->nxt], 1);
     if (rc) return rc;
   }
   B2R_CUDA(cudaEventRecord(h->ev_prefetch, h->st2));
@@ -1034,6 +1058,48 @@ static int gicp_pcl_align(b2r_handle* h, const float* guess, b2r_result* out) {
   return B2R_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ pcl ICP align (icp_pcl.cuh)
+// the handle's pair record at the column-major guess, uploaded: both structures built, the workspace's counter zeroed
+static int icp_prepare(b2r_handle* h, const float* guess_col) {
+  Cloud& s = SRC(h);
+  Cloud& t = TGT(h);
+  int rc = ensure_grid(h, s);
+  if (!rc) rc = ensure_grid(h, t);
+  if (rc) return rc;
+  const IcpPairWs w = icp_pair_ws(s);
+  B2R_CUDA(h->icp_ws.reserve(w.bytes + 256));
+  B2R_CUDA(h->icp_pair.reserve(1));
+  if (!h->icp_h.p) B2R_CUDA(h->icp_h.alloc(1));
+  IcpPairDev& P = *h->icp_h.p;
+  icp_fill_pair(h->cfg, s, t, guess_col, h->icp_ws.p, P);
+  B2R_CUDA(cudaMemsetAsync(h->icp_ws.p + w.counter, 0, 256, h->st));
+  B2R_CUDA(cudaMemcpyAsync(h->icp_pair.p, &P, sizeof(IcpPairDev), cudaMemcpyHostToDevice, h->st));
+  h->tel.h2d += sizeof(IcpPairDev);
+  return B2R_OK;
+}
+
+// pcl::IterativeClosestPoint::align: every iteration runs on the device (icp_run); the host looks at the record once the predicted
+// rounds have run
+static int icp_align(b2r_handle* h, const float* guess, b2r_result* out) {
+  Cloud& s = SRC(h);
+  Cloud& t = TGT(h);
+  float G[16];
+  colmajor_to_row_f(guess, G);
+  if (s.n == 0 || t.n == 0) {  // pcl::Registration::initCompute fails: converged_ = false
+    store_result(h, G, false, 0, out);
+    return B2R_OK;
+  }
+  int rc = icp_prepare(h, guess);
+  if (rc) return rc;
+  int rounds = 0;
+  rc = icp_run(h->icp_pair.p, h->icp_h.p, 1, h->last_rounds > 0 ? h->last_rounds : 8, &h->tel, h->st, &rounds);
+  if (rc) return rc;
+  const IcpPairDev& P = *h->icp_h.p;
+  h->last_rounds = P.rounds;
+  store_result(h, P.T, P.converged != 0, P.iterations, out);
+  return B2R_OK;
+}
+
 // b2r_align; `between` as in run_single_pair (GICP only: the NDT Newton loop is host-driven and has no single enqueue point)
 static int align_impl(b2r_handle* h, const float guess[16], b2r_result* out, const std::function<int()>* between) {
   if (!h || !guess) return fail(B2R_EINVAL, "NULL argument");
@@ -1042,6 +1108,7 @@ static int align_impl(b2r_handle* h, const float guess[16], b2r_result* out, con
   if (rc != B2R_OK) {}  // reported below like every failed align
   else if (gicp_family(h->cfg.method)) rc = gicp_align(h, guess, out, between);
   else if (h->cfg.method == B2R_METHOD_GICP_PCL) rc = gicp_pcl_align(h, guess, out);
+  else if (h->cfg.method == B2R_METHOD_ICP_PCL) rc = icp_align(h, guess, out);
   else {
     float Tfinal[16];
     bool conv = false;
@@ -1173,6 +1240,7 @@ extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
   if (!h->corr_valid) return fail(B2R_ESTATE, "no linearisation has run since the clouds were set");
   if (n != SRC(h).n) return fail(B2R_EINVAL, "n does not match the source cloud");
   if (h->cfg.method == B2R_METHOD_GICP_PCL) return gicp_pcl_fetch_correspondences(h, out, nullptr, n);
+  if (h->cfg.method == B2R_METHOD_ICP_PCL) return fail(B2R_ESTATE, "pcl ICP handle: use b2r_icp_pcl_correspondences_at");
   // a non-finite source point is not in the source's search structure (pos_of = -1): no search writes its entry, and like a PCL
   // query that finds nothing it has no correspondence
   std::vector<int> pos(n);
@@ -1318,6 +1386,61 @@ extern "C" int b2r_gicp_pcl_cost_at(b2r_handle* h, const float T[16], double* f_
   *f_sum = sums[0];
   for (int i = 0; i < 3; i++) g_sum[i] = sums[1 + i];
   for (int i = 0; i < 9; i++) dR_sum[i] = sums[4 + i];
+  return B2R_OK;
+}
+
+// one correspondence pass (forward or reciprocal) of a pcl ICP handle with the source transformed once by T; step = true also runs the
+// estimation step.  The record comes back in h->icp_h.
+static int icp_tap(b2r_handle* h, const float* T, bool step) {
+  if (h->cfg.method != B2R_METHOD_ICP_PCL) return fail(B2R_ESTATE, "pcl ICP engine (B2R_METHOD_ICP_PCL) required");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  if (need_source(h)) return B2R_ESTATE;
+  if (SRC(h).n == 0 || TGT(h).n == 0) return fail(B2R_ESTATE, "source/target not set");
+  int rc = icp_prepare(h, T);
+  if (rc) return rc;
+  const IcpPairDev& P = *h->icp_h.p;
+  rc = icp_enqueue_round(h->icp_pair.p, 1, (unsigned)P.nrow, (unsigned)P.src.nsup, P.reciprocal != 0, step, &h->tel, h->st);
+  if (rc) return rc;
+  B2R_CUDA(cudaMemcpyAsync(h->icp_h.p, h->icp_pair.p, sizeof(IcpPairDev), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaStreamSynchronize(h->st));
+  return B2R_OK;
+}
+
+extern "C" int b2r_icp_pcl_correspondences_at(b2r_handle* h, const float T[16], int32_t* corr, float* d2, uint64_t* count) {
+  if (!h || !T || !count) return fail(B2R_EINVAL, "NULL argument");
+  int rc = icp_tap(h, T, false);
+  if (rc) return rc;
+  const IcpPairDev& P = *h->icp_h.p;
+  *count = (uint64_t)P.n_corr;
+  if (!corr && !d2) return B2R_OK;
+  Cloud& s = SRC(h);
+  Cloud& t = TGT(h);
+  const size_t n = s.n, padded = (size_t)s.nsup * 1024, tpadded = (size_t)t.nsup * 1024;
+  std::vector<int> cs(padded + 1), pos(n + 1);
+  std::vector<float> ds(padded + 1);
+  std::vector<float4> tsp(tpadded + 1);  // the target's sorted points: w carries the original index
+  B2R_CUDA(cudaMemcpyAsync(cs.data(), P.corr, padded * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaMemcpyAsync(ds.data(), P.d2, padded * sizeof(float), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaMemcpyAsync(tsp.data(), t.sorted.p, tpadded * sizeof(float4), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaMemcpyAsync(pos.data(), s.pos_of.p, n * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaStreamSynchronize(h->st));
+  for (size_t i = 0; i < n; i++) {
+    const int c = pos[i] >= 0 ? cs[pos[i]] : -1;  // a non-finite point is not in the source's structure: no correspondence
+    if (corr) corr[i] = c >= 0 ? idx_bits(tsp[c].w) : -1;
+    if (d2) d2[i] = c >= 0 ? ds[pos[i]] : NAN;
+  }
+  return B2R_OK;
+}
+
+extern "C" int b2r_icp_pcl_estimate_at(b2r_handle* h, const float T[16], float* transformation, double* sums) {
+  if (!h || !T || !transformation || !sums) return fail(B2R_EINVAL, "NULL argument");
+  int rc = icp_tap(h, T, true);
+  if (rc) return rc;
+  const IcpPairDev& P = *h->icp_h.p;
+  if (P.n_corr < 3) return fail(B2R_ESTATE, "fewer than 3 correspondences: no transformation is estimated");
+  for (int r = 0; r < 4; r++)
+    for (int c = 0; c < 4; c++) transformation[c * 4 + r] = P.inc[r * 4 + c];
+  for (int i = 0; i < kIcpStats + kIcpCross; i++) sums[i] = P.sums[i];
   return B2R_OK;
 }
 

@@ -79,6 +79,10 @@ struct b2r_batch {
   DevBuf<char> gp_ws;               // per pair in flight: correspondences, M, reduction partials and counter; fitness partials
   DevBuf<GicpPclArgs> d_gp_args;    // the round's pass records: correspondence passes first, then cost passes
   PinnedBuf<GicpPclArgs> h_gp_args; // staging
+  // pcl ICP batch (batch_run_icp_chunk)
+  DevBuf<char> icp_ws;              // per pair in flight: icp_pair_ws, then its k_fitness partials and counter
+  DevBuf<IcpPairDev> d_icp;         // the pair records
+  PinnedBuf<IcpPairDev> h_icp;      // their host copies
   // telemetry of the last b2r_batch_align
   unsigned long long last_rounds = 0, last_pair_rounds = 0;
   ~b2r_batch() {  // what is not a plain free; the members then go in reverse order, the engine last
@@ -872,6 +876,70 @@ static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t 
   return B2R_OK;
 }
 
+// pairs[0..m) of a pcl ICP batch -> rep[0..m) (host).  Every pair runs the single handle's device loop; one launch per pass covers
+// every pair (blockIdx.y = pair), so a round is 2 launches (4 with the reciprocal check) whatever the number of pairs.
+static int batch_run_icp_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, double fit_max_range, PairReport* rep) {
+  b2r_handle* h = b->eng.get();
+  cudaStream_t st = h->st;
+  std::vector<size_t> active, off(m, 0), fit_off(m, 0);
+  std::vector<float> G(m * 16);
+  size_t ws = 0;
+  for (size_t i = 0; i < m; i++) {
+    for (int r = 0; r < 4; r++)
+      for (int c = 0; c < 4; c++) G[i * 16 + r * 4 + c] = pairs[i].guess[c * 4 + r];
+    Cloud& s = *b->clouds[pairs[i].source];
+    Cloud& t = *b->clouds[pairs[i].target];
+    if (s.n == 0 || t.n == 0) continue;  // initCompute fails: the guess, not converged, no iteration (as icp_align)
+    fit_off[i] = ws;
+    ws += align_up((size_t)s.nsup * 1024 / kLinThreads * 3 * sizeof(double), 256) + 256;
+    off[i] = ws;
+    ws += icp_pair_ws(s).bytes;
+    active.push_back(i);
+  }
+  const size_t fit_out = ws;
+  ws += align_up(m * 3 * sizeof(double), 256);
+  B2R_CUDA(b->icp_ws.reserve(ws + 256));
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->icp_ws.p), 256));
+  B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
+  const size_t na = active.size();
+  if (na) {
+    B2R_CUDA(b->d_icp.reserve(na));
+    if (b->h_icp.cap < na) B2R_CUDA(b->h_icp.alloc(na + 16));
+    for (size_t k = 0; k < na; k++) {
+      const size_t i = active[k];
+      icp_fill_pair(h->cfg, *b->clouds[pairs[i].source], *b->clouds[pairs[i].target], pairs[i].guess, base + off[i], b->h_icp.p[k]);
+    }
+    B2R_CUDA(cudaMemcpyAsync(b->d_icp.p, b->h_icp.p, na * sizeof(IcpPairDev), cudaMemcpyHostToDevice, st));
+    h->tel.h2d += na * sizeof(IcpPairDev);
+    int rounds = 0;
+    int rc = icp_run(b->d_icp.p, b->h_icp.p, (unsigned)na, 8, &h->tel, st, &rounds);
+    if (rc) return rc;
+    b->last_rounds += (unsigned long long)rounds;
+  }
+  std::vector<const float*> T(m);
+  std::vector<int> slot(m, -1);
+  for (size_t k = 0; k < na; k++) slot[active[k]] = (int)k;
+  for (size_t i = 0; i < m; i++) T[i] = slot[i] >= 0 ? b->h_icp.p[slot[i]].T : &G[i * 16];
+  std::vector<double> fit(m * 3, 0.0);
+  if (want_fitness) {
+    int rc = batch_fitness_at(b, pairs, m, T, base, fit_off, fit_out, fit_max_range, fit);
+    if (rc) return rc;
+  }
+  for (size_t i = 0; i < m; i++) {
+    PairReport& R = rep[i];
+    std::memset(&R, 0, sizeof(R));
+    for (int r = 0; r < 4; r++)
+      for (int c = 0; c < 4; c++) R.r.T[c * 4 + r] = T[i][r * 4 + c];
+    const double nr = fit[3 * i + 1];
+    R.r.fitness = !want_fitness ? NAN : (nr > 0 ? fit[3 * i] / nr : DBL_MAX);
+    const IcpPairDev* P = slot[i] >= 0 ? &b->h_icp.p[slot[i]] : nullptr;
+    R.r.converged = (P && P->converged) ? 1 : 0;
+    R.r.iterations = P ? P->iterations : 0;
+    R.rounds = P ? P->rounds : 0;
+  }
+  return B2R_OK;
+}
+
 __global__ void k_pack_results(const PairReport* rep, int n, b2r_result* out, int n_out, unsigned long long* round_sum) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_out) return;
@@ -898,7 +966,8 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   std::vector<int32_t> named(2 * n_pairs);
   for (size_t i = 0; i < n_pairs; i++) { named[2 * i] = pairs[i].source; named[2 * i + 1] = pairs[i].target; }
   const bool ndt = ndt_family(h->cfg.method);
-  rc = batch_build_structures(b, named.data(), named.size(), !fit_only && !ndt);
+  const bool icp = h->cfg.method == B2R_METHOD_ICP_PCL;  // ICP reads the search structures only
+  rc = batch_build_structures(b, named.data(), named.size(), !fit_only && !ndt && !icp);
   if (rc) return rc;
   if (ndt) rc = batch_ndt_maps(b, pairs, n_pairs, fit_only);
   if (rc) return rc;
@@ -919,12 +988,13 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
     // an NDT align runs its own rounds; a stand-alone fitness evaluation is the same search on either engine
     if (ndt && !fit_only) rc = batch_run_ndt_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
     else if (gpcl) rc = batch_run_gicp_pcl_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
+    else if (icp && !fit_only) rc = batch_run_icp_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
     else rc = batch_run_chunk(b, pairs + c0, m, cfg, b->d_reports.p + c0, fit_only);
     if (rc) return rc;
   }
   if (vgicp && want_fitness) rc = batch_vgicp_fitness(b, pairs, n_pairs, fit_max_range, b->d_reports.p);
   if (rc) return rc;
-  if ((ndt && !fit_only) || gpcl)  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
+  if ((ndt && !fit_only) || gpcl || (icp && !fit_only))  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
     B2R_CUDA(cudaMemcpyAsync(b->d_reports.p, b->h_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyHostToDevice, h->st));
   if (dbg) {
     const auto t_c = std::chrono::steady_clock::now();

@@ -96,11 +96,11 @@ struct Stream {
 };
 
 // ---- telemetry: copy byte counters, launch counters and (optional) CUDA-event timing per kernel class
-enum KernelClass { KC_GRID = 0, KC_KNN_COV, KC_GICP_CORR, KC_GICP_LIN, KC_GICP_ERR, KC_FITNESS, KC_NDT_BUILD, KC_NDT_DERIV, KC_NDT_HESS, KC_VOXELGRID, KC_MISC, KC_VGICP_MAP, KC_VGICP_ROUND, KC_GICP_PCL_CORR, KC_GICP_PCL_COST, KC_COUNT };
+enum KernelClass { KC_GRID = 0, KC_KNN_COV, KC_GICP_CORR, KC_GICP_LIN, KC_GICP_ERR, KC_FITNESS, KC_NDT_BUILD, KC_NDT_DERIV, KC_NDT_HESS, KC_VOXELGRID, KC_MISC, KC_VGICP_MAP, KC_VGICP_ROUND, KC_GICP_PCL_CORR, KC_GICP_PCL_COST, KC_ICP_PCL, KC_COUNT };
 inline const char* kernel_class_name(int c) {
   static const char* n[KC_COUNT] = {"bvh_build", "knn_covariance", "gicp_correspondences", "gicp_linearize", "gicp_error", "nn_fitness", "ndt_voxel_build",
                                     "ndt_derivatives", "ndt_hessian", "voxelgrid_downsample", "misc", "vgicp_voxel_map", "vgicp_round",
-                                    "gicp_pcl_correspondences", "gicp_pcl_cost"};
+                                    "gicp_pcl_correspondences", "gicp_pcl_cost", "icp_pcl_round"};
   return (c >= 0 && c < KC_COUNT) ? n[c] : "?";
 }
 struct Telemetry {

@@ -318,7 +318,7 @@ inline int gicp_pcl_run(GicpPclWork& W, bool corr_pass, Telemetry* tel, cudaStre
 }
 
 // row-major float 4x4 product ((a0 b0 + a1 b1) + a2 b2) + a3 b3, unfused (Eigen's Matrix4f product)
-inline void gicp_pcl_mul4f(const float* A, const float* B, float* O) {
+B2R_HD void gicp_pcl_mul4f(const float* A, const float* B, float* O) {
   for (int i = 0; i < 4; i++)
     for (int j = 0; j < 4; j++) O[i * 4 + j] = fadd(fadd(fadd(fmul(A[i * 4], B[j]), fmul(A[i * 4 + 1], B[4 + j])), fmul(A[i * 4 + 2], B[8 + j])), fmul(A[i * 4 + 3], B[12 + j]));
 }

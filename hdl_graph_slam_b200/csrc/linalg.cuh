@@ -336,6 +336,159 @@ B2R_HD void mul_iso(const double* A, const double* B, double* O) {
   for (int i = 0; i < 16; i++) O[i] = T[i];
 }
 
+// ---- pcl::IterativeClosestPoint (B2R_METHOD_ICP_PCL): Eigen 3.3.7's JacobiSVD<Matrix3f>, pcl::umeyama and DefaultConvergenceCriteria
+// in float32 / float64 exactly as upstream types them, every operation unfused (tests/icp_pcl_ref.cpp states each choice; the host
+// build in tests/icp_pcl_harness.cu must agree with it bit for bit)
+B2R_HD float fdiv_rn(float a, float b) {
+#ifdef __CUDA_ARCH__
+  return __fdiv_rn(a, b);
+#else
+  volatile float r = a / b; return r;
+#endif
+}
+B2R_HD float fsqrt_rn(float a) {
+#ifdef __CUDA_ARCH__
+  return __fsqrt_rn(a);
+#else
+  return sqrtf(a);
+#endif
+}
+// apply_rotation_in_the_plane over rows p, q (stride 1) or columns p, q (stride 3) of a row-major 3x3: x' = c x + s y, y' = -s x + c y
+B2R_HD void icp_rotate(float* M, int p, int q, int along, int step, float c, float s) {
+  if (c == 1.0f && s == 0.0f) return;
+#pragma unroll
+  for (int k = 0; k < 3; k++) {
+    const float xi = M[p * along + k * step], yi = M[q * along + k * step];
+    M[p * along + k * step] = fadd(fmul(c, xi), fmul(s, yi));
+    M[q * along + k * step] = fadd(fmul(-s, xi), fmul(c, yi));
+  }
+}
+// JacobiSVD<Matrix3f>(A, ComputeFullU | ComputeFullV): A, U, V row-major; d descending (two-sided Jacobi sweeps of real_2x2_jacobi_svd,
+// then |diagonal| with the sign moved into U, times the scale, then the selection sort of step 4)
+B2R_HD void icp_jacobi_svd3(const float* A, float* U, float* d, float* V) {
+  const float kMin = 1.17549435e-38f, kPrec = 2.0f * 1.1920929e-07f;
+  float scale = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 9; i++) scale = fabsf(A[i]) > scale ? fabsf(A[i]) : scale;
+  if (scale == 0.0f) scale = 1.0f;
+  float W[9];
+#pragma unroll
+  for (int i = 0; i < 9; i++) { W[i] = fdiv_rn(A[i], scale); U[i] = (i % 4 == 0) ? 1.0f : 0.0f; V[i] = U[i]; }
+  float maxd = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 3; i++) maxd = fabsf(W[i * 4]) > maxd ? fabsf(W[i * 4]) : maxd;
+  bool finished = false;
+  while (!finished) {
+    finished = true;
+    for (int p = 1; p < 3; p++)
+      for (int q = 0; q < p; q++) {
+        const float pm = fmul(kPrec, maxd);
+        const float thr = kMin > pm ? kMin : pm;
+        if (fabsf(W[p * 3 + q]) > thr || fabsf(W[q * 3 + p]) > thr) {
+          finished = false;
+          // real_2x2_jacobi_svd
+          float m00 = W[p * 4], m01 = W[p * 3 + q], m10 = W[q * 3 + p], m11 = W[q * 4];
+          const float t = fadd(m00, m11), dd = fsub(m10, m01);
+          float c1 = 1.0f, s1 = 0.0f;
+          if (!(fabsf(dd) < kMin)) {
+            const float u = fdiv_rn(t, dd);
+            const float tmp = fsqrt_rn(fadd(1.0f, fmul(u, u)));
+            s1 = fdiv_rn(1.0f, tmp);
+            c1 = fdiv_rn(u, tmp);
+          }
+          if (!(c1 == 1.0f && s1 == 0.0f)) {
+            const float a0 = m00, a1 = m01, b0 = m10, b1 = m11;
+            m00 = fadd(fmul(c1, a0), fmul(s1, b0)); m01 = fadd(fmul(c1, a1), fmul(s1, b1));
+            m10 = fadd(fmul(-s1, a0), fmul(c1, b0)); m11 = fadd(fmul(-s1, a1), fmul(c1, b1));
+          }
+          (void)m10;
+          // j_right.makeJacobi(m, 0, 1)
+          float cr = 1.0f, sr = 0.0f;
+          const float deno = fmul(2.0f, fabsf(m01));
+          if (!(deno < kMin)) {
+            const float tau = fdiv_rn(fsub(m00, m11), deno);
+            const float w = fsqrt_rn(fadd(fmul(tau, tau), 1.0f));
+            const float tt = tau > 0.0f ? fdiv_rn(1.0f, fadd(tau, w)) : fdiv_rn(1.0f, fsub(tau, w));
+            const float sign_t = tt > 0.0f ? 1.0f : -1.0f;
+            const float n = fdiv_rn(1.0f, fsqrt_rn(fadd(fmul(tt, tt), 1.0f)));
+            sr = fmul(fmul(fmul(-sign_t, fdiv_rn(m01, fabsf(m01))), fabsf(tt)), n);
+            cr = n;
+          }
+          // j_left = rot1 * j_right.transpose()
+          const float cl = fsub(fmul(c1, cr), fmul(s1, -sr)), sl = fadd(fmul(c1, -sr), fmul(s1, cr));
+          icp_rotate(W, p, q, 3, 1, cl, sl);   // W.applyOnTheLeft(p, q, j_left)
+          icp_rotate(U, p, q, 1, 3, cl, sl);   // U.applyOnTheRight(p, q, j_left.transpose())
+          icp_rotate(W, p, q, 1, 3, cr, -sr);  // W.applyOnTheRight(p, q, j_right)
+          icp_rotate(V, p, q, 1, 3, cr, -sr);  // V.applyOnTheRight(p, q, j_right)
+          const float ap = fabsf(W[p * 4]), aq = fabsf(W[q * 4]);
+          const float mpq = ap < aq ? aq : ap;
+          maxd = maxd < mpq ? mpq : maxd;
+        }
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < 3; i++) {
+    const float a = W[i * 4];
+    d[i] = fabsf(a);
+    if (a < 0.0f)
+      for (int k = 0; k < 3; k++) U[k * 3 + i] = -U[k * 3 + i];
+  }
+#pragma unroll
+  for (int i = 0; i < 3; i++) d[i] = fmul(d[i], scale);
+  for (int i = 0; i < 3; i++) {
+    int pos = i;
+    float mx = d[i];
+    for (int j = i + 1; j < 3; j++)
+      if (d[j] > mx) { mx = d[j]; pos = j; }
+    if (mx == 0.0f) break;
+    if (pos != i) {
+      float t = d[i]; d[i] = d[pos]; d[pos] = t;
+      for (int k = 0; k < 3; k++) {
+        t = U[k * 3 + i]; U[k * 3 + i] = U[k * 3 + pos]; U[k * 3 + pos] = t;
+        t = V[k * 3 + i]; V[k * 3 + i] = V[k * 3 + pos]; V[k * 3 + pos] = t;
+      }
+    }
+  }
+}
+// Eigen's 3x3 determinant: (m00 (m11 m22 - m12 m21) - m01 (m10 m22 - m12 m20)) + m02 (m10 m21 - m11 m20), float32
+B2R_HD float icp_det3f(const float* m) {
+  const float h0 = fmul(m[0], fsub(fmul(m[4], m[8]), fmul(m[5], m[7])));
+  const float h1 = fmul(m[1], fsub(fmul(m[3], m[8]), fmul(m[5], m[6])));
+  const float h2 = fmul(m[2], fsub(fmul(m[3], m[7]), fmul(m[4], m[6])));
+  return fadd(fsub(h0, h1), h2);
+}
+// a 3-term coefficient of a small fixed-size Eigen product: x0 + (x1 + x2) (redux_novec_unroller splits 3 as 1 + 2)
+B2R_HD float icp_dot3f(float a0, float b0, float a1, float b1, float a2, float b2) { return fadd(fmul(a0, b0), fadd(fmul(a1, b1), fmul(a2, b2))); }
+// pcl::umeyama(src, dst, false) from sigma = (1/n) dst_demean src_demean^T and the means (PCL's copy with the rank-deficient branch):
+// Rt row-major 4x4 float
+B2R_HD void icp_umeyama(const float* sigma, const float* src_mean, const float* dst_mean, float* Rt) {
+  float U[9], d[3], V[9];
+  icp_jacobi_svd3(sigma, U, d, V);
+  float S[3] = {1.0f, 1.0f, icp_det3f(sigma) < 0.0f ? -1.0f : 1.0f};
+  int rank = 0;
+  for (int i = 0; i < 3; i++)
+    if (!(fabsf(d[i]) <= fmul(fabsf(d[0]), 1e-5f))) rank++;  // !isMuchSmallerThan(d_i, d_0), float dummy_precision
+  if (rank == 2) S[2] = fmul(icp_det3f(U), icp_det3f(V)) > 0.0f ? 1.0f : -1.0f;
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++)
+      Rt[i * 4 + j] = icp_dot3f(fmul(U[i * 3], S[0]), V[j * 3], fmul(U[i * 3 + 1], S[1]), V[j * 3 + 1], fmul(U[i * 3 + 2], S[2]), V[j * 3 + 2]);
+  for (int i = 0; i < 3; i++)
+    Rt[i * 4 + 3] = fsub(dst_mean[i], icp_dot3f(Rt[i * 4], src_mean[0], Rt[i * 4 + 1], src_mean[1], Rt[i * 4 + 2], src_mean[2]));
+  Rt[12] = Rt[13] = Rt[14] = 0.0f; Rt[15] = 1.0f;
+}
+// DefaultConvergenceCriteria::hasConverged after ++nr_iterations_ (failure_after_max_iter_ false, max_iterations_similar_transforms_ 0,
+// mse_threshold_relative_ = euclidean_fitness_epsilon_ = -DBL_MAX, which never fires): T = transformation_ row-major 4x4, mse = this
+// iteration's correspondence MSE, *prev_mse updated as upstream does.  rot_thr = 1 - transformation_epsilon, trans_thr = transformation_epsilon
+B2R_HD bool icp_has_converged(const float* T, int iterations, int max_iterations, double rot_thr, double trans_thr, double mse, double* prev_mse) {
+  if (iterations >= max_iterations) return true;
+  const double cos_angle = 0.5 * (double)fsub(fadd(fadd(T[0], T[5]), T[10]), 1.0f);
+  const double tsq = (double)fadd(fadd(fmul(T[3], T[3]), fmul(T[7], T[7])), fmul(T[11], T[11]));
+  if (cos_angle >= rot_thr && tsq <= trans_thr) return true;
+  if (fabs(mse - *prev_mse) < 1e-12) return true;
+  *prev_mse = mse;
+  return false;
+}
+
 B2R_HD bool gicp_is_converged(const double* D, double rot_eps, double trans_eps) {
   double mr = 0, mt = 0;
 #pragma unroll

@@ -18,7 +18,7 @@ library; nothing here computes.
 import ctypes as C
 import numpy as np
 from . import _capi
-from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL  # noqa: F401
+from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL  # noqa: F401
 
 
 def _cloud(a):
@@ -307,6 +307,27 @@ class Registration:
         dp = C.POINTER(C.c_double)
         check(self._lib.b2r_gicp_pcl_cost_at(self._h, t.ctypes.data_as(C.POINTER(C.c_float)), C.byref(f), g.ctypes.data_as(dp), dR.ctypes.data_as(dp)))
         return f.value, g, dR
+
+    def icpPclCorrespondencesAt(self, T, n_source):
+        """(pcl ICP) one correspondence pass with the source transformed once by T, forward or reciprocal as configured: (target index of
+        every source point (n,) int32, -1 = none, squared distance (n,) float32, NaN where there is none, accepted count)"""
+        t = _colmajor(T, np.float32)
+        corr = np.empty(max(n_source, 1), np.int32)
+        d2 = np.empty(max(n_source, 1), np.float32)
+        nc = C.c_uint64()
+        check(self._lib.b2r_icp_pcl_correspondences_at(self._h, t.ctypes.data_as(C.POINTER(C.c_float)), corr.ctypes.data_as(C.POINTER(C.c_int32)),
+                                                       d2.ctypes.data_as(C.POINTER(C.c_float)), C.byref(nc)))
+        return corr[:n_source], d2[:n_source], nc.value
+
+    def icpPclEstimateAt(self, T):
+        """(pcl ICP) the same pass, then pcl::umeyama on it: (transformation_ (4, 4) float32, sums (17,): count, sum d2, sum src (3),
+        sum tgt (3), demeaned cross products (9))"""
+        t = _colmajor(T, np.float32)
+        out = np.empty(16, np.float32)
+        sums = np.empty(17, np.float64)
+        check(self._lib.b2r_icp_pcl_estimate_at(self._h, t.ctypes.data_as(C.POINTER(C.c_float)), out.ctypes.data_as(C.POINTER(C.c_float)),
+                                                sums.ctypes.data_as(C.POINTER(C.c_double))))
+        return _from_colmajor(out), sums
 
     # --- companion / prefilter chain
     def _filter(self, fn, cloud, *args):

@@ -57,6 +57,10 @@ extern "C" {
                                  max_iterations / k_correspondences / transformation_epsilon / max_correspondence_distance /
                                  max_optimizer_iterations; rotation_epsilon stays 2e-3.  The BFGS runs on the host (one device pass per correspondence
                                  update and per functor evaluation); a batch gathers every pair's pass of a round into shared launches */
+#define B2R_METHOD_ICP_PCL 5 /* pcl::IterativeClosestPoint semantics (PCL 1.10, registrations.cpp:57-65): exact 1-NN correspondences accepted at
+                                d2 <= max_correspondence_distance^2 (optionally reciprocal), pcl::umeyama's SVD step, DefaultConvergenceCriteria;
+                                reads max_iterations / transformation_epsilon / max_correspondence_distance / use_reciprocal_correspondences.
+                                The whole loop runs on the device: 2 launches per iteration, 4 with the reciprocal check */
 
 typedef struct b2r_handle b2r_handle;
 
@@ -77,7 +81,7 @@ typedef struct b2r_config {
   int32_t ndt_fixed_iterations;       /* >0: exactly this many iterations (BASELINE config 3), convergence test off */
   float grid_cell_min;                /* engine tuning: smallest search-grid cell, power of two (default 0.5 m) */
   int32_t max_optimizer_iterations;   /* reg_max_optimizer_iterations      (20)   pcl GICP max_inner_iterations_ (B2R_METHOD_GICP_PCL) */
-  int32_t reserved;                   /* explicit padding to a multiple of 8 bytes */
+  int32_t use_reciprocal_correspondences; /* reg_use_reciprocal_correspondences (false): 0 or 1, read by B2R_METHOD_ICP_PCL only */
 } b2r_config;
 
 /* What the callers read back after align(): getFinalTransformation(), hasConverged(), and (loop closure)
@@ -99,7 +103,8 @@ int b2r_config_default(b2r_config* cfg, int method);
  * passed as string key/value pairs (the rosparam namespace of the nodelet).  "FAST_GICP"/"B200_GICP" -> GICP engine,
  * "NDT_OMP"/"B200_NDT" -> NDT engine, "NDT" -> pcl NDT engine (B2R_METHOD_NDT_PCL), "FAST_VGICP"/"B200_VGICP" -> VGICP engine
  * (B2R_METHOD_VGICP), "GICP"/"B200_GICP_PCL" and every other name that reaches the reference's GICP branch (contains "GICP" but not
- * "OMP") -> pcl GICP engine (B2R_METHOD_GICP_PCL).  ICP / GICP_OMP / FAST_VGICP_CUDA and unknown names are not re-created: returns
+ * "OMP") -> pcl GICP engine (B2R_METHOD_GICP_PCL), "B200_ICP" -> pcl ICP engine (B2R_METHOD_ICP_PCL; reg_use_reciprocal_correspondences
+ * must be true / false / 1 / 0, else B2R_EINVAL).  ICP / GICP_OMP / FAST_VGICP_CUDA and unknown names are not re-created: returns
  * B2R_EUNSUPPORTED so the caller keeps the reference's own branch.  (Built without USE_VGICP_CUDA the reference sends FAST_VGICP_CUDA to
  * its GICP branch; this factory refuses it all the same, so the caller decides.) */
 int b2r_select_registration_method(const char* const* keys, const char* const* values, int n_params, int device_id,
@@ -210,6 +215,15 @@ int b2r_gicp_pcl_correspondences_at(b2r_handle* h, const float guess[16], const 
 /* B2R_METHOD_GICP_PCL: one cost pass (OptimizationFunctorWithIndices) at the column-major float pose T over the last correspondences:
  * *f_sum = sum res^T M res, g_sum[3] = sum M res, dR_sum[9] = sum p_src (M res)^T (row-major), unscaled (the functor divides by m) */
 int b2r_gicp_pcl_cost_at(b2r_handle* h, const float T[16], double* f_sum, double* g_sum, double* dR_sum);
+
+/* B2R_METHOD_ICP_PCL: one correspondence pass with the source transformed once by the column-major float T (transformPointCloud),
+ * forward or reciprocal as configured: corr[n] (caller's point order, may be NULL) = the target index of the accepted correspondence or
+ * -1, d2[n] (may be NULL) = its squared distance (NaN where there is none), *count = the accepted number */
+int b2r_icp_pcl_correspondences_at(b2r_handle* h, const float T[16], int32_t* corr, float* d2, uint64_t* count);
+/* B2R_METHOD_ICP_PCL: the same pass, then TransformationEstimationSVD (pcl::umeyama) on it: transformation[16] column-major float and
+ * sums[17] = count, sum d2, sum src (3), sum tgt (3) of the accepted pairs, then sum (tgt - tgt_mean)_i (src - src_mean)_j row-major (9).
+ * B2R_ESTATE below 3 correspondences (the align stops there unconverged) */
+int b2r_icp_pcl_estimate_at(b2r_handle* h, const float T[16], float* transformation, double* sums);
 
 /* ---- companion: voxel-grid downsample ---------------------------------------------------------------------------
  * replaces pcl::VoxelGrid<PointXYZI>::filter with setLeafSize(leaf,leaf,leaf) (apps/prefiltering_nodelet.cpp:54-58,138-149;
