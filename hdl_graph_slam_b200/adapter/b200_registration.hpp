@@ -97,7 +97,8 @@ public:
                       : cfg.method == B2R_METHOD_NDT_PCL ? "B200_NDT_PCL"
                       : cfg.method == B2R_METHOD_VGICP ? "B200_VGICP"
                       : cfg.method == B2R_METHOD_GICP_PCL ? "B200_GICP_PCL"
-                      : cfg.method == B2R_METHOD_ICP_PCL ? "B200_ICP" : "B200_NDT";
+                      : cfg.method == B2R_METHOD_ICP_PCL ? "B200_ICP"
+                      : cfg.method == B2R_METHOD_VGICP_CUDA ? "B200_VGICP_CUDA" : "B200_NDT";
     this->max_iterations_ = cfg.max_iterations;
     this->transformation_epsilon_ = cfg.transformation_epsilon;
     this->corr_dist_threshold_ = cfg.max_correspondence_distance;
@@ -215,6 +216,16 @@ private:
 //       cfg.max_iterations = pnh.param<int>("reg_maximum_iterations", 64);
 //       cfg.max_correspondence_distance = pnh.param<double>("reg_max_correspondence_distance", 2.5);
 //       cfg.use_reciprocal_correspondences = pnh.param<bool>("reg_use_reciprocal_correspondences", false) ? 1 : 0;
+//       cfg.device_id = pnh.param<int>("reg_device_id", 0);
+//       return pcl::Registration<PointT, PointT>::Ptr(new B200Registration<PointT>(cfg));
+//     }
+//     else if(registration_method == "B200_VGICP_CUDA") {  // in place of the FAST_VGICP_CUDA branch (registrations.cpp:37-47)
+//       b2r_config cfg;
+//       b2r_config_default(&cfg, B2R_METHOD_VGICP_CUDA);  // fast_gicp::FastVGICPCuda: k-NN exact, PLANE, DIRECT1, float32 terms
+//       cfg.ndt_resolution = pnh.param<double>("reg_resolution", 1.0);
+//       cfg.transformation_epsilon = pnh.param<double>("reg_transformation_epsilon", 0.01);
+//       cfg.max_iterations = pnh.param<int>("reg_maximum_iterations", 64);
+//       cfg.k_correspondences = pnh.param<int>("reg_correspondence_randomness", 20);
 //       cfg.device_id = pnh.param<int>("reg_device_id", 0);
 //       return pcl::Registration<PointT, PointT>::Ptr(new B200Registration<PointT>(cfg));
 //     }

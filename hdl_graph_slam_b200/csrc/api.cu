@@ -27,6 +27,7 @@
 #include "fitness.cuh"
 #include "ndt.cuh"
 #include "vgicp.cuh"
+#include "vgicp_cuda.cuh"
 #include "gicp_pcl.cuh"
 #include "icp_pcl.cuh"
 #include "voxelgrid.cuh"
@@ -115,8 +116,10 @@ struct b2r_handle {
 };
 
 static Cloud& SRC(b2r_handle* h) { return h->clouds[h->src]; }
-// the methods whose clouds carry FastGICP's covariances and run the device LM (pair_engine.cuh)
-static bool gicp_family(int method) { return method == B2R_METHOD_GICP || method == B2R_METHOD_VGICP; }
+// the methods that run the device LM (pair_engine.cuh); their clouds carry FastGICP's covariances, or FastVGICPCuda's float32 ones
+static bool gicp_family(int method) { return method == B2R_METHOD_GICP || method == B2R_METHOD_VGICP || method == B2R_METHOD_VGICP_CUDA; }
+// the methods that align to a Gaussian voxel map of the target (vgicp.cuh): FastVGICP's, or FastVGICPCuda's float32 one
+static bool vgicp_family(int method) { return method == B2R_METHOD_VGICP || method == B2R_METHOD_VGICP_CUDA; }
 // the methods whose clouds carry k-NN covariances: FastGICP's, or pcl GICP's raw-moment ones (B2R_METHOD_GICP_PCL)
 static bool cov_family(int method) { return gicp_family(method) || method == B2R_METHOD_GICP_PCL; }
 static bool known_method(int method) { return cov_family(method) || ndt_family(method) || method == B2R_METHOD_ICP_PCL; }
@@ -135,7 +138,7 @@ extern "C" int b2r_config_default(b2r_config* c, int method) {
   c->transformation_epsilon = 0.01;   // :31,109
   c->rotation_epsilon = 2e-3;         // fast_gicp default
   c->max_correspondence_distance = 2.5;  // :33
-  c->ndt_resolution = method == B2R_METHOD_VGICP ? 1.0 : 0.5;  // :93; FAST_VGICP's reg_resolution default (:51)
+  c->ndt_resolution = vgicp_family(method) ? 1.0 : 0.5;  // :93; FAST_VGICP[_CUDA]'s reg_resolution default (:43, :51)
   c->ndt_step_size = 0.1;             // ndt_omp default (never overridden by the factory)
   c->ndt_outlier_ratio = 0.55;
   c->ndt_search_method = 7;           // :103 DIRECT7
@@ -193,6 +196,15 @@ extern "C" int b2r_select_registration_method(const char* const* keys, const cha
     c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
     c.max_iterations = iparam("reg_maximum_iterations", 64);
     c.k_correspondences = iparam("reg_correspondence_randomness", 20);
+  } else if (method == "B200_VGICP_CUDA") {
+    // registrations.cpp:37-47: fast_gicp::FastVGICPCuda with resolution, transformation epsilon, maximum iterations and correspondence
+    // randomness; reg_max_correspondence_distance and reg_num_threads are not read.  The plain name FAST_VGICP_CUDA stays with the
+    // reference's own branch, which also depends on how the reference was built (USE_VGICP_CUDA)
+    b2r_config_default(&c, B2R_METHOD_VGICP_CUDA);
+    c.ndt_resolution = dparam("reg_resolution", 1.0);
+    c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
+    c.max_iterations = iparam("reg_maximum_iterations", 64);
+    c.k_correspondences = iparam("reg_correspondence_randomness", 20);
   } else if (method.find("GICP") != std::string::npos && method.find("OMP") == std::string::npos && method != "FAST_VGICP_CUDA") {
     // registrations.cpp:66-76 (every name containing GICP but not OMP that no branch above takes): pcl::GeneralizedIterativeClosestPoint.
     // reg_use_reciprocal_correspondences is read upstream and has no effect on GICP; FAST_VGICP_CUDA stays refused (the reference only
@@ -231,7 +243,7 @@ extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
   if (!cfg || !out) return fail(B2R_EINVAL, "NULL argument");
   *out = nullptr;
   if (!known_method(cfg->method)) return fail(B2R_EINVAL, "unknown method");
-  if (cfg->method == B2R_METHOD_VGICP && !(cfg->ndt_resolution > 0.0 && std::isfinite(cfg->ndt_resolution)))
+  if (vgicp_family(cfg->method) && !(cfg->ndt_resolution > 0.0 && std::isfinite(cfg->ndt_resolution)))
     return fail(B2R_EINVAL, "VGICP: ndt_resolution (reg_resolution) must be finite and positive");
   if (cfg->k_correspondences < 1 || cfg->k_correspondences > 64) return fail(B2R_EINVAL, "k_correspondences must be in [1,64]");
   if (cfg->method == B2R_METHOD_GICP_PCL && cfg->max_optimizer_iterations < 1) return fail(B2R_EINVAL, "max_optimizer_iterations must be >= 1");
@@ -487,6 +499,22 @@ static int build_bvh(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
 
 static int ensure_grid(b2r_handle* h, Cloud& c, int ctx = 0) { return build_bvh(h, c, h->bc[ctx], ctx ? h->st2 : h->st); }
 
+// the raw-moment k-NN covariance kernels (gicp_pcl.cuh) under the moment rule `Rule`
+template <class Rule>
+static int launch_raw_cov(b2r_handle* h, Cloud& c, int k, size_t smem, cudaStream_t st) {
+  const size_t padded = (size_t)c.nsup * 1024;
+  if (k == kKnnRegK) {
+    k_pcl_cov_reg<kKnnRegK, Rule><<<(unsigned)(padded / kKnnThreads), kKnnThreads, 0, st>>>(c.bvh(), c.raw_view, c.stride_f, c.cov.p);
+  } else {
+    if (smem > 48 * 1024 && !h->pcl_knn_smem_attr) {  // the attribute belongs to the handle's device (a handle runs one rule)
+      B2R_CUDA(cudaFuncSetAttribute(k_pcl_cov<Rule>, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * kKnnThreads * 8));
+      h->pcl_knn_smem_attr = true;
+    }
+    k_pcl_cov<Rule><<<(unsigned)(padded / kKnnThreads), kKnnThreads, smem, st>>>(c.bvh(), k, c.raw_view, c.stride_f, c.cov.p);
+  }
+  return B2R_OK;
+}
+
 static int build_cov(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
   int rc = build_bvh(h, c, B, st);
   if (rc) return rc;
@@ -505,15 +533,11 @@ static int build_cov(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
 #endif
     TEL_BEGIN(&h->tel, st);
     if (h->cfg.method == B2R_METHOD_GICP_PCL) {  // pcl GICP's raw-moment covariances (gicp_pcl.cuh)
-      if (k == kKnnRegK) {
-        k_pcl_cov_reg<kKnnRegK><<<(unsigned)(padded / kKnnThreads), kKnnThreads, 0, st>>>(c.bvh(), c.raw_view, c.stride_f, c.cov.p);
-      } else {
-        if (smem > 48 * 1024 && !h->pcl_knn_smem_attr) {  // the attribute belongs to the handle's device
-          B2R_CUDA(cudaFuncSetAttribute(k_pcl_cov, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * kKnnThreads * 8));
-          h->pcl_knn_smem_attr = true;
-        }
-        k_pcl_cov<<<(unsigned)(padded / kKnnThreads), kKnnThreads, smem, st>>>(c.bvh(), k, c.raw_view, c.stride_f, c.cov.p);
-      }
+      rc = launch_raw_cov<PclCov>(h, c, k, smem, st);
+      if (rc) return rc;
+    } else if (h->cfg.method == B2R_METHOD_VGICP_CUDA) {  // FastVGICPCuda's float32 raw-moment covariances (vgicp_cuda.cuh)
+      rc = launch_raw_cov<VcudaCov>(h, c, k, smem, st);
+      if (rc) return rc;
     } else if (k == kKnnRegK) {  // the reference's default reg_correspondence_randomness: lists live in registers
       // On the PREFETCH stream the kernel works for the NEXT frame while the align chain of the current one runs beside it.  All of its
       // 512 blocks become resident at once (104 registers x 128 threads x ~3.9 blocks per SM on 132 SMs = 80 % of the register file) and
@@ -566,17 +590,23 @@ static int build_cov(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
 
 static int ensure_cov(b2r_handle* h, Cloud& c, int ctx = 0) { return build_cov(h, c, h->bc[ctx], ctx ? h->st2 : h->st); }
 
-// VGICP: the Gaussian voxel map of a target (after its covariances), built once per cloud
+// the Gaussian voxel map of cloud c (covariances built) under the method's cell and accumulation rule
+static int vgicp_map_of(b2r_handle* h, Cloud& c) {
+  return h->cfg.method == B2R_METHOD_VGICP_CUDA ? vgicp_build_map<VcudaMapRule>(c, h->cfg.ndt_resolution, &h->tel, h->st)
+                                                : vgicp_build_map<VgicpMapRule>(c, h->cfg.ndt_resolution, &h->tel, h->st);
+}
+
+// VGICP / VGICP_CUDA: the Gaussian voxel map of a target (after its covariances), built once per cloud
 static int vgicp_ensure_map(b2r_handle* h, Cloud& c) {
   if (c.vgicp_ready) return B2R_OK;
   int rc = ensure_cov(h, c);
   if (rc) return rc;
-  return vgicp_build_map(c, h->cfg.ndt_resolution, &h->tel, h->st);
+  return vgicp_map_of(h, c);
 }
 
 static int preprocess(b2r_handle* h, int which, bool is_target) {
   Cloud& c = h->clouds[which];
-  if (h->cfg.method == B2R_METHOD_VGICP && is_target) return vgicp_ensure_map(h, c);
+  if (vgicp_family(h->cfg.method) && is_target) return vgicp_ensure_map(h, c);
   if (h->cfg.method == B2R_METHOD_ICP_PCL) return ensure_grid(h, c);  // ICP reads the search structures only
   if (cov_family(h->cfg.method)) {
     // a target gets its covariances now; a SOURCE only its search structure: its k-NN covariance kernel is launched by the align,
@@ -786,9 +816,10 @@ static cudaError_t launch_search(PairDev* d_pairs, const int* d_active, unsigned
 }
 
 // one round (update_correspondences + linearize/compute_error + LM step) over n_slots pair slots
-// vmaps != nullptr: a VGICP round (k_vgicp_round + k_pair_lm; vmaps[k] is the voxel map of pair k's target)
+// vmaps != nullptr: a VGICP round (k_vgicp_round + k_pair_lm; vmaps[k] is the voxel map of pair k's target), or with vcuda the
+// FastVGICPCuda round (k_vgicp_cuda_round + k_pair_lm)
 static int launch_round(PairDev* d_pairs, const int* d_active, unsigned n_slots, unsigned max_sorted, int copies, const LmCfg& cfg, cudaStream_t st,
-                        Telemetry* tel, bool search = true, const VgicpMapDev* vmaps = nullptr) {
+                        Telemetry* tel, bool search = true, const VgicpMapDev* vmaps = nullptr, bool vcuda = false) {
   static const bool pdl = !getenv("B2R_NO_PDL");
   if (vmaps) {
     TEL_BEGIN(tel, st);
@@ -798,7 +829,7 @@ static int launch_round(PairDev* d_pairs, const int* d_active, unsigned n_slots,
     la[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     la[0].val.programmaticStreamSerializationAllowed = 1;
     lc.attrs = la; lc.numAttrs = pdl ? 1 : 0;
-    B2R_CUDA(cudaLaunchKernelEx(&lc, k_vgicp_round, d_pairs, d_active, vmaps));
+    B2R_CUDA(cudaLaunchKernelEx(&lc, vcuda ? k_vgicp_cuda_round : k_vgicp_round, d_pairs, d_active, vmaps));
     lc.gridDim = dim3(n_slots); lc.blockDim = dim3(kLmThreads);
     B2R_CUDA(cudaLaunchKernelEx(&lc, k_pair_lm, d_pairs, d_active, cfg));
     TEL_END(tel, KC_VGICP_ROUND, 2, st);
@@ -895,7 +926,8 @@ static int run_single_pair(b2r_handle* h, const double* x, int mode, int tap, co
   }
   auto enqueue = [&](int n) -> int {
     for (int i = 0; i < n; i++) {
-      int rc = launch_round(h->d_pair.p, nullptr, 1, max_sorted, copies, cfg, h->st, &h->tel, true, vmaps);
+      int rc = launch_round(h->d_pair.p, nullptr, 1, max_sorted, copies, cfg, h->st, &h->tel, true, vmaps,
+                            h->cfg.method == B2R_METHOD_VGICP_CUDA);
       if (rc) return rc;
       enq++;
     }
@@ -958,7 +990,7 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out, const 
     return between ? (*between)() : B2R_OK;
   }
   static const bool overlap = !getenv("B2R_NO_COV_OVERLAP");
-  const bool vgicp = h->cfg.method == B2R_METHOD_VGICP;
+  const bool vgicp = vgicp_family(h->cfg.method);
   const bool cov_beside = overlap && !s.cov_ready && !vgicp;  // see run_single_pair (a VGICP round reads the source covariances at once)
   int rc = cov_beside ? ensure_grid(h, s) : ensure_cov(h, s);
   if (rc) return rc;
@@ -1254,7 +1286,7 @@ extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
 
 extern "C" int b2r_get_covariances(b2r_handle* h, int which, double* out, size_t n) {
   if (!h || !out) return fail(B2R_EINVAL, "NULL argument");
-  if (!cov_family(h->cfg.method)) return fail(B2R_ESTATE, "covariances exist only for the GICP, VGICP and pcl GICP engines");
+  if (!cov_family(h->cfg.method)) return fail(B2R_ESTATE, "covariances exist only for the GICP, VGICP, VGICP_CUDA and pcl GICP engines");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (!which && need_source(h)) return B2R_ESTATE;
   Cloud& c = which ? TGT(h) : SRC(h);
@@ -1447,7 +1479,7 @@ extern "C" int b2r_icp_pcl_estimate_at(b2r_handle* h, const float T[16], float* 
 extern "C" int b2r_vgicp_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int32_t* cells, int32_t* counts, double* mean, double* cov) {
   if (!h || !n_voxels) return fail(B2R_EINVAL, "NULL argument");
   *n_voxels = 0;
-  if (h->cfg.method != B2R_METHOD_VGICP) return fail(B2R_ESTATE, "VGICP engine (B2R_METHOD_VGICP) required");
+  if (!vgicp_family(h->cfg.method)) return fail(B2R_ESTATE, "VGICP engine (B2R_METHOD_VGICP or B2R_METHOD_VGICP_CUDA) required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   int rc = vgicp_ensure_map(h, TGT(h));
   if (rc) return rc;
@@ -1457,7 +1489,7 @@ extern "C" int b2r_vgicp_get_voxels(b2r_handle* h, size_t capacity, size_t* n_vo
 extern "C" int b2r_vgicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* cost, uint64_t* n_corr, int32_t* voxel_of,
                                       size_t n) {
   if (!h || !T || !H || !b || !cost) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_VGICP) return fail(B2R_ESTATE, "VGICP engine (B2R_METHOD_VGICP) required");
+  if (!vgicp_family(h->cfg.method)) return fail(B2R_ESTATE, "VGICP engine (B2R_METHOD_VGICP or B2R_METHOD_VGICP_CUDA) required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (need_source(h)) return B2R_ESTATE;
   Cloud& s = SRC(h);

@@ -287,7 +287,9 @@ static int batch_build_structures(b2r_batch* b, const int32_t* ids, size_t n_ids
   B2R_CUDA(cudaMemcpyAsync(b->d_knn.p, b->h_knn.p, todo.size() * sizeof(KnnBatchItem), cudaMemcpyHostToDevice, st));
   { TEL_BEGIN(&h->tel, st);
     if (h->cfg.method == B2R_METHOD_GICP_PCL)  // pcl GICP's raw-moment covariances (gicp_pcl.cuh)
-      k_pcl_cov_reg_batch<kKnnRegK><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
+      k_pcl_cov_reg_batch<kKnnRegK, PclCov><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
+    else if (h->cfg.method == B2R_METHOD_VGICP_CUDA)  // FastVGICPCuda's float32 raw-moment covariances (vgicp_cuda.cuh)
+      k_pcl_cov_reg_batch<kKnnRegK, VcudaCov><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
     else
       k_knn_cov_reg_batch<kKnnRegK><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
     TEL_END(&h->tel, KC_KNN_COV, 1, st); }
@@ -350,7 +352,7 @@ static int wait_word(const b2r_batch::Lane& L, unsigned long long need_seq, size
 static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const LmCfg& cfg, PairReport* d_rep, bool fit_only) {
   b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
-  const bool vgicp = h->cfg.method == B2R_METHOD_VGICP && !fit_only;  // a stand-alone fitness evaluation runs the GICP search
+  const bool vgicp = vgicp_family(h->cfg.method) && !fit_only;  // a stand-alone fitness evaluation runs the GICP search
   // per-launch kernel timing (b2r_set_profiling) wants every kernel alone on the device; tiny chunks are not worth a second stream
   const int n_lanes = (h->tel.on || m < 16) ? 1 : b->n_lanes;
   size_t ws_total = 0;
@@ -428,7 +430,7 @@ static int batch_run_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, const 
       if (R.known == 0) continue;
       any = true;
       int rc = launch_round(L.d_pairs.p, L.d_active.p, (unsigned)R.known, (unsigned)R.max_pad, b->copies, cfg, L.st, &h->tel, true,
-                            vgicp ? L.d_vmaps.p : nullptr);
+                            vgicp ? L.d_vmaps.p : nullptr, h->cfg.method == B2R_METHOD_VGICP_CUDA);
       if (rc) return rc;
       b->last_rounds++;
       sq[l] = ++L.seq;
@@ -465,7 +467,7 @@ static int batch_vgicp_maps(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs)
   for (size_t i = 0; i < n_pairs; i++) {
     Cloud& t = *b->clouds[pairs[i].target];
     if (t.n == 0 || t.vgicp_ready) continue;
-    int rc = vgicp_build_map(t, h->cfg.ndt_resolution, &h->tel, h->st);
+    int rc = vgicp_map_of(h, t);
     if (rc) return rc;
   }
   return B2R_OK;
@@ -971,7 +973,7 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   if (rc) return rc;
   if (ndt) rc = batch_ndt_maps(b, pairs, n_pairs, fit_only);
   if (rc) return rc;
-  const bool vgicp = h->cfg.method == B2R_METHOD_VGICP && !fit_only;
+  const bool vgicp = vgicp_family(h->cfg.method) && !fit_only;
   const bool gpcl = h->cfg.method == B2R_METHOD_GICP_PCL && !fit_only;  // host-driven rounds, like NDT
   if (vgicp) rc = batch_vgicp_maps(b, pairs, n_pairs);
   if (rc) return rc;

@@ -1,7 +1,7 @@
 // gicp_pcl.cuh — the factory's `GICP` branch: pcl::GeneralizedIterativeClosestPoint (PCL 1.10) on the device (B2R_METHOD_GICP_PCL).
 //
 // Re-creates, GPU-first, what registrations.cpp:66-76 selects (semantics pinned by tests/gicp_pcl_ref.cpp, see its header):
-//   k_pcl_cov_reg<20> / k_pcl_cov  <- computeCovariances: k-NN (the point itself included) in ascending (d2, index) order, raw
+//   k_pcl_cov_reg<20, PclCov> / k_pcl_cov<PclCov>  <- computeCovariances: k-NN (the point itself included) in ascending (d2, index) order, raw
 //                                     moments in float64 with float32 products, cov -= mean mean^T, singular values (1, 1, gicp_epsilon)
 //   k_gicp_pcl_corr                <- the correspondence loop of computeTransformation: q = transformation_ (guess p), exact 1-NN,
 //                                     d2 < corr_dist^2 in float64, M = (R C1 R^T + C2)^-1 with Eigen's 3x3 inverse
@@ -58,8 +58,14 @@ __device__ __forceinline__ void pcl_cov_store(int kk, PtAt pt_at, double* __rest
   o[5] = dsub(1.0, dmul(dmul(w, n[2]), n[2]));
 }
 
+// the moment rule of the kernels below: pcl GICP's (this file); FastVGICPCuda's float32 one is VcudaCov (vgicp_cuda.cuh)
+struct PclCov {
+  template <class PtAt>
+  __device__ __forceinline__ static void store(int kk, PtAt pt_at, double* __restrict__ o) { pcl_cov_store(kk, pt_at, o); }
+};
+
 // k = 20 (reg_correspondence_randomness' default): register lists, one warp per leaf, as k_knn_cov_reg
-template <int K>
+template <int K, class Rule>
 __device__ __forceinline__ void pcl_cov_reg_body(const Bvh& b, const float* __restrict__ raw, int stride_f, double* __restrict__ cov, int block_x) {
   __shared__ int nbr[K][kKnnThreads];
   const int s = block_x * blockDim.x + threadIdx.x;
@@ -74,25 +80,26 @@ __device__ __forceinline__ void pcl_cov_reg_body(const Bvh& b, const float* __re
 #pragma unroll
   for (int j = 0; j < K; j++) nbr[j][threadIdx.x] = (int)(unsigned int)(L.key[j] & 0xffffffffull);
   const int tx = threadIdx.x;
-  pcl_cov_store(L.count(), [&](int j) {
+  Rule::store(L.count(), [&](int j) {
     const float* p = raw + (size_t)nbr[j][tx] * stride_f;
     return make_float3(p[0], p[1], p[2]);
   }, cov + (size_t)s * 6);
 }
 
-template <int K>
+template <int K, class Rule>
 __global__ void __launch_bounds__(kKnnThreads, B2R_KNN_MINBLOCKS) k_pcl_cov_reg(Bvh b, const float* __restrict__ raw, int stride_f, double* __restrict__ cov) {
-  pcl_cov_reg_body<K>(b, raw, stride_f, cov, blockIdx.x);
+  pcl_cov_reg_body<K, Rule>(b, raw, stride_f, cov, blockIdx.x);
 }
 
 // the same for MANY clouds in one launch (blockIdx.y = cloud), as k_knn_cov_reg_batch
-template <int K>
+template <int K, class Rule>
 __global__ void __launch_bounds__(kKnnThreads, B2R_KNN_BATCH_MINBLOCKS) k_pcl_cov_reg_batch(const KnnBatchItem* __restrict__ items) {
   const KnnBatchItem it = items[blockIdx.y];
-  pcl_cov_reg_body<K>(it.b, it.raw, it.stride_f, it.cov, blockIdx.x);
+  pcl_cov_reg_body<K, Rule>(it.b, it.raw, it.stride_f, it.cov, blockIdx.x);
 }
 
 // any k: per-lane lists in shared memory, as k_knn_cov
+template <class Rule>
 __global__ void __launch_bounds__(kKnnThreads, 4) k_pcl_cov(Bvh b, int k, const float* __restrict__ raw, int stride_f, double* __restrict__ cov) {
   extern __shared__ unsigned long long pcl_knn_keys[];  // [k][blockDim]
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -110,7 +117,7 @@ __global__ void __launch_bounds__(kKnnThreads, 4) k_pcl_cov(Bvh b, int k, const 
   if (!active) return;
   const int stride = L.stride;
   const unsigned long long* keyp = L.key;
-  pcl_cov_store(L.cnt, [=](int j) {
+  Rule::store(L.cnt, [=](int j) {
     const int idx = (int)(unsigned int)(keyp[j * stride] & 0xffffffffull);
     const float* p = raw + (size_t)idx * stride_f;
     return make_float3(p[0], p[1], p[2]);

@@ -12,7 +12,8 @@
 //     J = [skew(T mean_A) | -I].  compute_error reuses the correspondences and M of the linearisation point.
 //
 // Device layout: the map is built from the cloud's BVH arrays (sorted points + pos_of) and its covariances, so it needs neither the
-// caller's records nor a copy of them: a promoted source (odometry keyframe) gets its map from what it already holds.
+// caller's records nor a copy of them: a promoted source (odometry keyframe) gets its map from what it already holds.  The build is
+// templated on the cell and accumulation rule: FastVGICP's VgicpMapRule below, FastVGICPCuda's float32 VcudaMapRule (vgicp_cuda.cuh).
 // One VGICP round = k_vgicp_round (probe, M, trial cost of the previous set, weighted linearisation; the 29 block partials of
 // k_pair_accumulate's layout) + the unchanged k_pair_lm.  Pair records (PairDev) are the GICP engine's; the map travels beside them.
 #pragma once
@@ -53,8 +54,8 @@ struct VgicpMap {
   int nvox = 0;
 };
 
-__device__ __forceinline__ bool vgicp_cell(double x, double y, double z, double res, unsigned long long* key) {
-  const double fx = floor(x / res), fy = floor(y / res), fz = floor(z / res);
+// the key of the cell (fx, fy, fz) (whole numbers), false outside the 21-bit range per axis or for a NaN
+__device__ __forceinline__ bool vgicp_key(double fx, double fy, double fz, unsigned long long* key) {
   const double lo = -(double)kVgicpBias, hi = (double)kVgicpBias;
   if (!(fx >= lo && fx < hi && fy >= lo && fy < hi && fz >= lo && fz < hi)) return false;  // also every NaN
   *key = ((unsigned long long)((long long)fx + kVgicpBias) << (2 * kVgicpAxisBits)) |
@@ -62,12 +63,28 @@ __device__ __forceinline__ bool vgicp_cell(double x, double y, double z, double 
   return true;
 }
 
+__device__ __forceinline__ bool vgicp_cell(double x, double y, double z, double res, unsigned long long* key) {
+  return vgicp_key(floor(x / res), floor(y / res), floor(z / res), key);
+}
+
+// The map's cell and accumulation rule.  This one is FastVGICP's: float64 cells floor(p / res) and float64 sums; FastVGICPCuda's
+// float32 rule is VcudaMapRule (vgicp_cuda.cuh).  Both store the finalised means and covariances as doubles.
+struct VgicpMapRule {
+  using Acc = double;
+  __device__ __forceinline__ static bool cell(float x, float y, float z, double res, unsigned long long* key) {
+    return vgicp_cell((double)x, (double)y, (double)z, res, key);
+  }
+  __device__ __forceinline__ static double add(double a, double b) { return dadd(a, b); }
+  __device__ __forceinline__ static double div(double a, int n) { return __ddiv_rn(a, (double)n); }
+};
+
 __device__ __forceinline__ unsigned int vgicp_hash(unsigned long long k) {
   k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
   return (unsigned int)k;
 }
 
 // one key per point in ascending point index (the radix sort below is stable, so a voxel's points stay in index order)
+template <class Rule>
 __global__ void k_vgicp_keys(const float4* __restrict__ sorted, const int* __restrict__ pos_of, int n, double res, unsigned long long* keys,
                              int* vals, int* misc) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -77,7 +94,7 @@ __global__ void k_vgicp_keys(const float4* __restrict__ sorted, const int* __res
   const int j = pos_of[i];
   if (j >= 0) {  // in the search structure = a finite point
     const float4 p = sorted[j];
-    if (!vgicp_cell((double)p.x, (double)p.y, (double)p.z, res, &key)) { key = kVgicpNone; atomicAdd(misc + 0, 1); }
+    if (!Rule::cell(p.x, p.y, p.z, res, &key)) { key = kVgicpNone; atomicAdd(misc + 0, 1); }
   } else {
     atomicAdd(misc + 1, 1);
   }
@@ -85,6 +102,7 @@ __global__ void k_vgicp_keys(const float4* __restrict__ sorted, const int* __res
 }
 
 // one thread per voxel: sums in point-index order, finalize, table insert
+template <class Rule>
 __global__ void k_vgicp_voxels(const float4* __restrict__ sorted, const int* __restrict__ pos_of, const double* __restrict__ pcov,
                                const unsigned long long* __restrict__ ukeys, const int* __restrict__ counts, const int* __restrict__ offs,
                                const int* __restrict__ idx, int nvox, double* mean, double* cov, int* count, unsigned long long* tkeys,
@@ -92,20 +110,20 @@ __global__ void k_vgicp_voxels(const float4* __restrict__ sorted, const int* __r
   const int v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= nvox) return;
   const int c = counts[v], o = offs[v];
-  double m[3] = {0.0, 0.0, 0.0}, s[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  using Acc = typename Rule::Acc;
+  Acc m[3] = {0, 0, 0}, s[6] = {0, 0, 0, 0, 0, 0};
   for (int k = 0; k < c; k++) {
     const int j = pos_of[idx[o + k]];
     const float4 p = sorted[j];
-    m[0] = dadd(m[0], (double)p.x); m[1] = dadd(m[1], (double)p.y); m[2] = dadd(m[2], (double)p.z);
+    m[0] = Rule::add(m[0], (Acc)p.x); m[1] = Rule::add(m[1], (Acc)p.y); m[2] = Rule::add(m[2], (Acc)p.z);
     const double* ci = pcov + (size_t)j * 6;
 #pragma unroll
-    for (int q = 0; q < 6; q++) s[q] = dadd(s[q], ci[q]);
+    for (int q = 0; q < 6; q++) s[q] = Rule::add(s[q], (Acc)ci[q]);
   }
-  const double dn = (double)c;
 #pragma unroll
-  for (int q = 0; q < 3; q++) mean[(size_t)v * 3 + q] = __ddiv_rn(m[q], dn);
+  for (int q = 0; q < 3; q++) mean[(size_t)v * 3 + q] = (double)Rule::div(m[q], c);
 #pragma unroll
-  for (int q = 0; q < 6; q++) cov[(size_t)v * 6 + q] = __ddiv_rn(s[q], dn);
+  for (int q = 0; q < 6; q++) cov[(size_t)v * 6 + q] = (double)Rule::div(s[q], c);
   count[v] = c;
   const unsigned long long key = ukeys[v];
   unsigned int h = vgicp_hash(key) & mask;
@@ -126,8 +144,9 @@ __device__ __forceinline__ int vgicp_probe(const VgicpMapDev& M, unsigned long l
   }
 }
 
-// Builds (or keeps) the voxel map of cloud `c` at `res`: needs c's BVH and covariances.  Synchronises `st` once (extent check, voxel
-// count).  B2R_EUNSUPPORTED when a finite point lies beyond the 21-bit key range.
+// Builds (or keeps) the voxel map of cloud `c` at `res` under `Rule`: needs c's BVH and covariances.  Synchronises `st` once (extent
+// check, voxel count).  B2R_EUNSUPPORTED when a finite point lies beyond the 21-bit key range.
+template <class Rule>
 inline int vgicp_build_map(Cloud& c, double res, Telemetry* tel, cudaStream_t st) {
   if (!c.vgicp) c.vgicp.reset(new VgicpMap());
   VgicpMap& M = *c.vgicp;
@@ -146,7 +165,7 @@ inline int vgicp_build_map(Cloud& c, double res, Telemetry* tel, cudaStream_t st
     B2R_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b_scan, M.counts.p, M.offs.p, n, st));
     B2R_CUDA(M.tmp.reserve(std::max(b_sort, std::max(b_rle, b_scan)) + 256));
     TEL_BEGIN(tel, st);
-    k_vgicp_keys<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c.sorted.p, c.pos_of.p, n, res, M.keys_a.p, M.vals_a.p, M.misc.p);
+    k_vgicp_keys<Rule><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(c.sorted.p, c.pos_of.p, n, res, M.keys_a.p, M.vals_a.p, M.misc.p);
     size_t tb = M.tmp.cap;
     B2R_CUDA(cub::DeviceRadixSort::SortPairs(M.tmp.p, tb, M.keys_a.p, M.keys_b.p, M.vals_a.p, M.vals_b.p, n, 0, 64, st));
     tb = M.tmp.cap;
@@ -171,7 +190,7 @@ inline int vgicp_build_map(Cloud& c, double res, Telemetry* tel, cudaStream_t st
   B2R_CUDA(cudaMemsetAsync(M.tkeys.p, 0xff, cap * sizeof(unsigned long long), st));
   if (M.nvox > 0) {
     TEL_BEGIN(tel, st);
-    k_vgicp_voxels<<<(unsigned)((M.nvox + 127) / 128), 128, 0, st>>>(c.sorted.p, c.pos_of.p, c.cov.p, M.ukeys.p, M.counts.p, M.offs.p, M.vals_b.p,
+    k_vgicp_voxels<Rule><<<(unsigned)((M.nvox + 127) / 128), 128, 0, st>>>(c.sorted.p, c.pos_of.p, c.cov.p, M.ukeys.p, M.counts.p, M.offs.p, M.vals_b.p,
                                                                      M.nvox, M.mean.p, M.cov.p, M.count.p, M.tkeys.p, M.tvals.p, cap - 1);
     TEL_END(tel, KC_VGICP_MAP, 1, st);
     B2R_CUDA(cudaGetLastError());

@@ -18,7 +18,7 @@ library; nothing here computes.
 import ctypes as C
 import numpy as np
 from . import _capi
-from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL  # noqa: F401
+from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL, B2R_METHOD_VGICP_CUDA  # noqa: F401
 
 
 def _cloud(a):
@@ -258,7 +258,7 @@ class Registration:
         return counts[:n_source], keys[:total.value]
 
     def vgicpGetVoxels(self):
-        """(VGICP) the target's Gaussian voxel map, cells ascending: dict(cells (V, 3) int32, counts (V,), mean (V, 3), cov (V, 3, 3))"""
+        """(VGICP, VGICP_CUDA) the target's Gaussian voxel map, cells ascending: dict(cells (V, 3) int32, counts (V,), mean (V, 3), cov (V, 3, 3))"""
         nv = C.c_size_t()
         check(self._lib.b2r_vgicp_get_voxels(self._h, 0, C.byref(nv), None, None, None, None))
         V = nv.value
@@ -272,7 +272,7 @@ class Registration:
         return dict(cells=cells, counts=counts, mean=mean, cov=cov)
 
     def vgicpLinearizeAt(self, T, n_source):
-        """(VGICP) one voxel-correspondence update + linearisation at T: (H (6, 6), b (6,), cost, correspondence count, voxel of every
+        """(VGICP, VGICP_CUDA) one voxel-correspondence update + linearisation at T: (H (6, 6), b (6,), cost, correspondence count, voxel of every
         source point (n,) int32, -1 = none)"""
         t = _colmajor(T, np.float64)
         H = np.empty((6, 6), np.float64)

@@ -61,6 +61,11 @@ extern "C" {
                                 d2 <= max_correspondence_distance^2 (optionally reciprocal), pcl::umeyama's SVD step, DefaultConvergenceCriteria;
                                 reads max_iterations / transformation_epsilon / max_correspondence_distance / use_reciprocal_correspondences.
                                 The whole loop runs on the device: 2 launches per iteration, 4 with the reciprocal check */
+#define B2R_METHOD_VGICP_CUDA 6 /* fast_gicp::FastVGICPCuda semantics (registrations.cpp:37-47, opted into as B200_VGICP_CUDA):
+                                   float32 raw-moment k-NN covariances with float32 PLANE, the target's float32 Gaussian voxel map at
+                                   ndt_resolution (reg_resolution) with cells floor(p / res - 0.5), DIRECT1 voxel correspondences and
+                                   float32 terms weighted sqrt(num_points), summed in float64; reads max_iterations / k_correspondences /
+                                   transformation_epsilon, not max_correspondence_distance */
 
 typedef struct b2r_handle b2r_handle;
 
@@ -104,7 +109,8 @@ int b2r_config_default(b2r_config* cfg, int method);
  * "NDT_OMP"/"B200_NDT" -> NDT engine, "NDT" -> pcl NDT engine (B2R_METHOD_NDT_PCL), "FAST_VGICP"/"B200_VGICP" -> VGICP engine
  * (B2R_METHOD_VGICP), "GICP"/"B200_GICP_PCL" and every other name that reaches the reference's GICP branch (contains "GICP" but not
  * "OMP") -> pcl GICP engine (B2R_METHOD_GICP_PCL), "B200_ICP" -> pcl ICP engine (B2R_METHOD_ICP_PCL; reg_use_reciprocal_correspondences
- * must be true / false / 1 / 0, else B2R_EINVAL).  ICP / GICP_OMP / FAST_VGICP_CUDA and unknown names are not re-created: returns
+ * must be true / false / 1 / 0, else B2R_EINVAL), "B200_VGICP_CUDA" -> FastVGICPCuda engine (B2R_METHOD_VGICP_CUDA).
+ * ICP / GICP_OMP / FAST_VGICP_CUDA and unknown names are not re-created: returns
  * B2R_EUNSUPPORTED so the caller keeps the reference's own branch.  (Built without USE_VGICP_CUDA the reference sends FAST_VGICP_CUDA to
  * its GICP branch; this factory refuses it all the same, so the caller decides.) */
 int b2r_select_registration_method(const char* const* keys, const char* const* values, int n_params, int device_id,
@@ -196,13 +202,13 @@ int b2r_ndt_get_centroids(b2r_handle* h, size_t capacity, size_t* n_centroids, i
  * entries, may be NULL) and one flat array of the neighbours' leaf keys, ascending within each point (CSR by counts; the first
  * `capacity` entries are written, keys may be NULL); *total = the number of (point, neighbour) pairs */
 int b2r_ndt_neighbors_at(b2r_handle* h, const double p[6], uint32_t* counts, size_t capacity, int64_t* keys, size_t* total);
-/* B2R_METHOD_VGICP: the target's Gaussian voxel map (GaussianVoxelMap after finalize), cells ascending (x, then y, then z):
- * cells[3 V] = floor(p / resolution) per axis, counts[V] = num_points, mean[3 V], cov[9 V] (3x3 row-major); *n_voxels = V; the first
+/* B2R_METHOD_VGICP / B2R_METHOD_VGICP_CUDA: the target's Gaussian voxel map (GaussianVoxelMap after finalize), cells ascending (x,
+ * then y, then z): cells[3 V] = floor(p / resolution) per axis (VGICP_CUDA: floorf(p / resolution - 0.5f) in float32), counts[V] = num_points, mean[3 V], cov[9 V] (3x3 row-major); *n_voxels = V; the first
  * `capacity` voxels are written, every array may be NULL.  B2R_EUNSUPPORTED when a finite target point lies 2^20 cells or more from
  * the origin on an axis (the keys hold 21 bits per axis); points with a non-finite coordinate belong to no voxel. */
 int b2r_vgicp_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int32_t* cells, int32_t* counts, double* mean, double* cov);
-/* B2R_METHOD_VGICP: one update_correspondences (DIRECT1) + linearize at pose T (column-major double): H[36] row-major, b[6],
- * *cost = sum sqrt(num_points) e^T M e, *n_corr = source points with a voxel, voxel_of (n source entries in the caller's point order,
+/* B2R_METHOD_VGICP / B2R_METHOD_VGICP_CUDA: one update_correspondences (DIRECT1) + linearize at pose T (column-major double): H[36]
+ * row-major, b[6], *cost = sum sqrt(num_points) e^T M e (VGICP_CUDA: float32 terms at T rounded to float32, summed in float64), *n_corr = source points with a voxel, voxel_of (n source entries in the caller's point order,
  * may be NULL) = the index of the point's voxel in b2r_vgicp_get_voxels' order, or -1 */
 int b2r_vgicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* cost, uint64_t* n_corr, int32_t* voxel_of, size_t n);
 
