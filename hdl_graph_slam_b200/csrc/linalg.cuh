@@ -89,8 +89,24 @@ B2R_HD void sym_cross_eigvec3(double a00, double a01, double a02, double a11, do
   v[0] = x * inv; v[1] = y * inv; v[2] = z * inv;
 }
 
+// An exactly diagonal A (an axis-aligned line or a single point) has tied eigenvalues, so "the smallest eigenvector" is not
+// unique there; it returns the axis upstream's JacobiSVD leaves in U's last column.  JacobiSVD does no rotation on a diagonal
+// matrix; its step-4 sort walks i = 0, 1, swapping column i with the FIRST maximum of the remaining |a_jj| only when that is not
+// at i, and stops at a zero maximum.  After i = 0 (first maximum p) the remaining columns are (u, w) = (1, 2), (0, 2) or (1, 0);
+// i = 1 swaps them only if |a_ww| > |a_uu|.  So the zero matrix and multiples of I give e_z, diag(0, 0, a) gives e_x.
 B2R_HD void sym_min_eigvec3(const double* A, double* v) {
   const double a00 = A[0], a01 = A[1], a02 = A[2], a11 = A[4], a12 = A[5], a22 = A[8];
+  if (a01 == 0.0 && a02 == 0.0 && a12 == 0.0) {
+    const double s0 = fabs(a00), s1 = fabs(a11), s2 = fabs(a22);
+    int u = 1, w = 2;
+    double su = s1, sw = s2;
+    if (!(s0 >= s1 && s0 >= s2)) {
+      if (s1 >= s2) { u = 0; su = s0; } else { w = 0; sw = s0; }
+    }
+    const int axis = sw > su ? u : w;
+    v[0] = axis == 0 ? 1.0 : 0.0; v[1] = axis == 1 ? 1.0 : 0.0; v[2] = axis == 2 ? 1.0 : 0.0;
+    return;
+  }
   const double q = (a00 + a11 + a22) / 3.0;
   const double b00 = a00 - q, b11 = a11 - q, b22 = a22 - q;
   const double p2 = b00 * b00 + b11 * b11 + b22 * b22 + 2.0 * (a01 * a01 + a02 * a02 + a12 * a12);

@@ -55,13 +55,9 @@ static void covariances(const KdTree& tree, const float* pts, size_t n, size_t s
     // PLANE: JacobiSVD(cov) -> U diag(1,1,1e-3) V^T; for a symmetric PSD matrix U = V = eigenvectors, values descending.
     double w[3], V[9];
     sym_eigen<3>(c, w, V);  // ascending: V col 2 = largest
-    if (c[1] == 0.0 && c[2] == 0.0 && c[5] == 0.0 && c[0] == c[4] && c[4] == c[8]) {
-      // a multiple of I (all k neighbours one point: the zero matrix): every direction is an eigenvector.  JacobiSVD leaves U = I
-      // and keeps the equal singular values in place, so its smallest-value column is e_z: diag(1, 1, 1e-3), not the e_x the
-      // ascending Jacobi above would pick.
-      for (int a = 0; a < 9; a++) V[a] = 0.0;
-      V[0 * 3 + 1] = 1.0; V[1 * 3 + 2] = 1.0; V[2 * 3 + 0] = 1.0;  // column 0 (-> 1e-3) = e_z, columns 1, 2 = e_x, e_y
-    }
+    // exactly diagonal (an axis-aligned line, or all k neighbours one point): the eigenvalues tie and the ascending Jacobi above
+    // would pick its own column; JacobiSVD's is the one its step-4 sort leaves last (linalg.hpp diagonal_normal).  UPSTREAM-RECALL
+    if (c[1] == 0.0 && c[2] == 0.0 && c[5] == 0.0) diagonal_normal(c, V);
     const double vals[3] = {1e-3, 1.0, 1.0};  // smallest eigenvalue -> 1e-3
     double* o = cov_out + (size_t)i * 9;
     for (int a = 0; a < 3; a++)

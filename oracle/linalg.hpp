@@ -72,6 +72,25 @@ inline void sym_eigen(const double* A_in, double* w, double* V, bool stop_conver
   }
 }
 
+// The PLANE normal of an exactly diagonal 3x3 C (row-major), where tied eigenvalues leave the smallest eigenvector undefined:
+// the column JacobiSVD<Matrix3d> puts last in U.  On a diagonal matrix JacobiSVD does no rotation, moves negative signs into U
+// and then runs its step-4 sort: for each i, the FIRST maximum of the remaining |values| is swapped into place only when it is
+// not already at i, and the sort stops once that maximum is 0.  UPSTREAM-RECALL.  V gets column 0 = the normal (the eigenvector
+// that PLANE scales by epsilon) and columns 1, 2 = the other two axes, in the layout sym_eigen<3> returns.
+inline void diagonal_normal(const double* C, double* V) {
+  double s[3] = {std::fabs(C[0]), std::fabs(C[4]), std::fabs(C[8])};
+  int col[3] = {0, 1, 2};
+  for (int i = 0; i < 3; i++) {
+    int pos = i;
+    for (int j = i + 1; j < 3; j++)
+      if (s[j] > s[pos]) pos = j;
+    if (s[pos] == 0.0) break;
+    if (pos != i) { std::swap(s[i], s[pos]); std::swap(col[i], col[pos]); }
+  }
+  for (int a = 0; a < 9; a++) V[a] = 0.0;
+  V[col[2] * 3 + 0] = 1.0; V[col[0] * 3 + 1] = 1.0; V[col[1] * 3 + 2] = 1.0;
+}
+
 // 3x3 inverse by cofactors (what Eigen's fixed-size inverse() does). returns false if det == 0.
 inline bool inv3(const double* m, double* o) {
   double c00 = m[4] * m[8] - m[5] * m[7];

@@ -75,3 +75,48 @@ def relrel(a, b):
     a = np.asarray(a, np.float64)
     b = np.asarray(b, np.float64)
     return float(np.max(np.abs(a - b)) / max(np.max(np.abs(b)), 1e-300))
+
+
+def jacobisvd_diagonal_normal(C):
+    """The PLANE normal of an exactly diagonal 3x3 C, whose tied eigenvalues leave the smallest eigenvector undefined: the column
+    Eigen's JacobiSVD leaves last in U.  It does no rotation on a diagonal matrix; its step-4 sort swaps the FIRST maximum of the
+    remaining |values| into place when it is not already there and stops at a zero maximum.  None for a matrix that is not diagonal."""
+    C = np.asarray(C, np.float64)
+    if C[0, 1] != 0.0 or C[0, 2] != 0.0 or C[1, 2] != 0.0:
+        return None
+    s = list(np.abs(np.diag(C)))
+    col = [0, 1, 2]
+    for i in range(3):
+        pos = i + int(np.argmax(s[i:]))  # argmax returns the first maximum
+        if s[pos] == 0.0:
+            break
+        s[i], s[pos] = s[pos], s[i]
+        col[i], col[pos] = col[pos], col[i]
+    return np.eye(3)[col[2]]
+
+
+def axis_lines(n_per_axis=40, seed=0, length=(24, 40)):
+    """(n, 4) float32 records: separated straight segments along x, y and z, points on a 0.25 grid, every coordinate off the
+    segment's axis 0 or a power of two (so PCL's float32 raw moments are exact and the off-diagonals cancel to exactly 0) and
+    every segment more than 50 m from any other (so the k nearest neighbours of each point, k < length[0], lie on its own
+    segment).  The first segment of each axis lies on the axis itself.  Each neighbourhood's covariance is exactly diagonal."""
+    rng = np.random.default_rng(seed)
+    vals = np.array([0.0, 64.0, -64.0, 128.0, -128.0, 256.0, -256.0, 512.0])
+    on_axis = [tuple(float(128 * axis) if a == axis else 0.0 for a in range(3)) for axis in range(3)]
+    used = set(on_axis)
+    segs = []
+    for axis in range(3):
+        for s in range(n_per_axis):
+            c = on_axis[axis]
+            while s > 0:
+                c = tuple(float(v) for v in rng.choice(vals, 3))
+                if c not in used:
+                    used.add(c)
+                    break
+            m = int(rng.integers(length[0], length[1] + 1))
+            p = np.tile(np.asarray(c), (m, 1))
+            p[:, axis] += 0.25 * np.arange(m) - 4.0
+            segs.append(p)
+    p = np.concatenate(segs)
+    p = p[rng.permutation(len(p))]
+    return np.c_[p, np.ones(len(p))].astype(np.float32)

@@ -14,8 +14,12 @@
  *     cov(k, l) -= mean_k mean_l; JacobiSVD, rebuilt with singular values (1, 1, gicp_epsilon).                  UPSTREAM-RECALL
  *     For the PSD matrices met here the rebuild is I - (1 - eps) n n^T with n the eigenvector of the SMALLEST eigenvalue (this
  *     reference: orc::sym_eigen, the engine: a closed form; they agree within 1e-8).  An indefinite matrix from cancellation would
- *     order SVD's singular values by magnitude instead; the engine keeps the smallest eigenvalue.                   ENGINE
- *     A zero matrix (all neighbours one point) gives n = e_z, JacobiSVD's untouched identity.                       UPSTREAM-RECALL
+ *     order SVD's singular values by magnitude instead; the engine keeps the smallest eigenvalue, except on an exactly diagonal
+ *     matrix, where the rule below orders by magnitude as JacobiSVD does.                                           ENGINE
+ *     An exactly diagonal matrix (a line along an axis whose products are exact, or all neighbours one point) has tied
+ *     eigenvalues; n is the column JacobiSVD leaves last: no rotation, then its step-4 sort (first maximum of the remaining
+ *     |values| swapped in only when not already in place, stop at a zero maximum).  diag(a, 0, 0) and diag(0, a, 0) give e_z,
+ *     diag(0, 0, a) gives e_x, the zero matrix and multiples of I give e_z (orc::diagonal_normal).               UPSTREAM-RECALL
  *   non-finite points are in no search structure: they are nobody's neighbour, have no covariance and no correspondence.  ENGINE
  *   a cloud with fewer than k (finite) points: upstream indexes past the neighbour list (undefined); here the moments run over
  *     the neighbours found and divide by their count.                                                                ENGINE
@@ -109,10 +113,7 @@ void covariances(const float* pts, size_t n, size_t stride, int k, double* out) 
       }
     double w[3], V[9];
     orc::sym_eigen<3>(c, w, V);  // ascending: column 0 = the smallest eigenvalue's vector
-    if (c[1] == 0.0 && c[2] == 0.0 && c[5] == 0.0 && c[0] == c[4] && c[4] == c[8]) {
-      for (int a = 0; a < 9; a++) V[a] = 0.0;
-      V[0 * 3 + 1] = 1.0; V[1 * 3 + 2] = 1.0; V[2 * 3 + 0] = 1.0;  // column 0 = e_z
-    }
+    if (c[1] == 0.0 && c[2] == 0.0 && c[5] == 0.0) orc::diagonal_normal(c, V);  // column 0 = JacobiSVD's last column
     const double vals[3] = {1e-3, 1.0, 1.0};
     for (int a = 0; a < 9; a++) o[a] = 0.0;
     for (int e = 2; e >= 0; e--)  // U's columns in descending singular value

@@ -138,3 +138,14 @@ def transform(pts, T):
     out = pts.copy()
     out[:, :3] = p.astype(np.float32)
     return out
+
+
+
+def end_point_is_as_good(T, T_ref):
+    """an engine align's end pose T against the reference's T_ref after the same outer iterations: equal to 1e-5, or, where the two
+    BFGS line searches part in the last bits (fixed-tree against index-order sums), within 2e-3 in translation and rotation.  The
+    outer loop only stops once a whole iteration moves the pose by less than transformation_epsilon (0.01 m) and rotation_epsilon
+    (2e-3), so end points that far apart are the same answer to the stopping rule's resolution; a wrong optimiser step is larger."""
+    dt = float(np.max(np.abs(np.asarray(T)[:3, 3] - np.asarray(T_ref)[:3, 3])))
+    dr = float(np.max(np.abs(np.asarray(T)[:3, :3] - np.asarray(T_ref)[:3, :3])))
+    assert (dt <= 1e-5 and dr <= 1e-5) or (dt <= 2e-3 and dr <= 2e-3), (dt, dr)

@@ -7,6 +7,7 @@ import pytest
 from scipy.spatial.transform import Rotation
 
 import gicp_pcl_ref as gr
+from common import axis_lines, jacobisvd_diagonal_normal
 from oracle import oracle as orc
 
 EPS = 1e-3
@@ -40,8 +41,9 @@ def np_covariances(pts, k=20):
             raw += np.outer(v, v).astype(np.float32).astype(np.float64)  # each product rounded to float32
         mean /= len(p)
         C = raw / len(p) - np.outer(mean, mean)
-        w, V = np.linalg.eigh(C)
-        n = V[:, 0]
+        n = jacobisvd_diagonal_normal(C)  # tied eigenvalues of an exactly diagonal C: JacobiSVD's column, not eigh's
+        if n is None:
+            n = np.linalg.eigh(C)[1][:, 0]
         out[i] = np.eye(3) - (1 - EPS) * np.outer(n, n)
     return out
 
@@ -107,6 +109,15 @@ def test_covariances_match_numpy(ref):
     for k in (20, 7):
         got = ref.covariances(tgt, k)
         assert np.max(np.abs(got - np_covariances(tgt, k))) <= 1e-8
+
+
+@pytest.mark.parametrize("k", [2, 20])
+def test_axis_lines_take_the_jacobisvd_normal(ref, k):
+    """exactly diagonal raw-moment covariances (common.axis_lines): the restatement's diagonal branch against the reference"""
+    p = axis_lines(n_per_axis=4, seed=k)
+    want = np_covariances(p, k)
+    assert np.max(np.abs(ref.covariances(p, k) - want)) <= 1e-12
+    assert (np.abs(np.diagonal(want, axis1=1, axis2=2) - 1e-3) < 1e-12).any(axis=1).all()
 
 
 def test_planar_patch_gives_the_plane_covariance(ref):

@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 from scipy.spatial import cKDTree
 from scipy.linalg import expm
-from common import perturb, relrel
+from common import axis_lines, jacobisvd_diagonal_normal, perturb, relrel
 
 
 def skew(v):
@@ -34,6 +34,10 @@ def indep_covariances(pts, k=20):
     cov = np.einsum("nki,nkj->nij", c, c) / k
     U, S, Vt = np.linalg.svd(cov)
     reg = np.einsum("nij,j,njk->nik", U, np.array([1.0, 1.0, 1e-3]), Vt)
+    # an exactly diagonal covariance (an axis-aligned line) ties singular values, which LAPACK orders its own way: JacobiSVD's rule
+    for i in np.flatnonzero((cov[:, 0, 1] == 0) & (cov[:, 0, 2] == 0) & (cov[:, 1, 2] == 0)):
+        n = jacobisvd_diagonal_normal(cov[i])
+        reg[i] = np.eye(3) - (1.0 - 1e-3) * np.outer(n, n)
     return reg, ambiguous
 
 
@@ -71,6 +75,14 @@ def test_gicp_covariances_independent(pair, oracle):
     ok = ~amb
     assert ok.mean() > 0.99
     assert np.max(np.abs(got[ok] - want[ok])) < 1e-6  # the smallest singular vector of a near-isotropic patch is ill-conditioned: 1e-6, not 1e-9
+
+
+def test_gicp_covariances_of_axis_lines_independent(oracle):
+    """exactly diagonal covariances (common.axis_lines): the diagonal branch against the oracle, every point (the regularised matrix
+    depends on the normal alone, so the tie-ambiguous neighbour sets do not matter here)"""
+    p = axis_lines(n_per_axis=4, seed=2)
+    want, _ = indep_covariances(p, 20)
+    assert np.max(np.abs(oracle.gicp_covariances(p, 20) - want)) <= 1e-12
 
 
 def test_gicp_linearize_and_one_lm_step_independent(pair, oracle):

@@ -7,6 +7,7 @@ import pytest
 from scipy.spatial import cKDTree
 
 import vgicp_ref as vr
+from common import axis_lines, jacobisvd_diagonal_normal
 
 
 @pytest.fixture(scope="module")
@@ -23,6 +24,10 @@ def np_covariances(pts, k=20):
         nb = p[idx[i]]
         d = nb - nb.mean(axis=0)
         C = d.T @ d / k
+        n = jacobisvd_diagonal_normal(C)  # tied singular values of an exactly diagonal C: JacobiSVD's column, not LAPACK's
+        if n is not None:
+            out[i] = np.eye(3) - (1.0 - 1e-3) * np.outer(n, n)
+            continue
         U, _, Vt = np.linalg.svd(C)
         out[i] = U @ np.diag([1.0, 1.0, 1e-3]) @ Vt
     return out
@@ -71,6 +76,13 @@ def test_covariances_match_the_independent_restatement():
     got = vr.covariances(tgt)
     want = np_covariances(tgt)
     assert np.max(np.abs(got - want)) < 1e-8
+
+
+def test_axis_line_covariances_match_the_independent_restatement():
+    """exactly diagonal covariances (common.axis_lines): the restatement's diagonal branch against the oracle; the regularised matrix
+    depends on the normal alone, so the tie order of the k-NN lists does not matter"""
+    p = axis_lines(n_per_axis=4, seed=1)
+    assert np.max(np.abs(vr.covariances(p, 20) - np_covariances(p, 20))) <= 1e-12
 
 
 @pytest.mark.parametrize("res", [0.25, 0.5, 1.0, 2.0])

@@ -19,6 +19,8 @@
  *     ascending, v = (1e-3, 1, 1), each entry (a <= b, mirrored) ((1e-3 u0_a) u0_b + u1_a u1_b) + u2_a u2_b.  svd3's iterations are not
  *     reproduced: its U and V agree with these eigenvectors only to float32 rounding, and for an indefinite matrix (cancellation far
  *     from the origin) svd3 orders by |eigenvalue| where this keeps the smallest eigenvalue.                         ENGINE
+ *     An exactly diagonal matrix (an axis-aligned line) has tied eigenvalues: the normal is whichever column this Jacobi's selection
+ *     sort leaves first, not the JacobiSVD rule of the float64 engines (svd3 is not JacobiSVD).                          ENGINE
  *   a cloud with fewer than k finite points: the moments run over the neighbours found and divide by their count.    ENGINE
  *   non-finite points are nobody's neighbour, have no covariance, belong to no voxel and have no correspondence.      ENGINE
  *   voxel map of the target: cell = floorf(x / res - 0.5f) per axis in float32, the division and the subtraction rounded separately
