@@ -98,7 +98,8 @@ public:
                       : cfg.method == B2R_METHOD_VGICP ? "B200_VGICP"
                       : cfg.method == B2R_METHOD_GICP_PCL ? "B200_GICP_PCL"
                       : cfg.method == B2R_METHOD_ICP_PCL ? "B200_ICP"
-                      : cfg.method == B2R_METHOD_VGICP_CUDA ? "B200_VGICP_CUDA" : "B200_NDT";
+                      : cfg.method == B2R_METHOD_VGICP_CUDA ? "B200_VGICP_CUDA"
+                      : cfg.method == B2R_METHOD_GICP_OMP ? "B200_GICP_OMP" : "B200_NDT";
     this->max_iterations_ = cfg.max_iterations;
     this->transformation_epsilon_ = cfg.transformation_epsilon;
     this->corr_dist_threshold_ = cfg.max_correspondence_distance;
@@ -226,6 +227,17 @@ private:
 //       cfg.transformation_epsilon = pnh.param<double>("reg_transformation_epsilon", 0.01);
 //       cfg.max_iterations = pnh.param<int>("reg_maximum_iterations", 64);
 //       cfg.k_correspondences = pnh.param<int>("reg_correspondence_randomness", 20);
+//       cfg.device_id = pnh.param<int>("reg_device_id", 0);
+//       return pcl::Registration<PointT, PointT>::Ptr(new B200Registration<PointT>(cfg));
+//     }
+//     else if(registration_method == "B200_GICP_OMP") {  // in place of the GICP_OMP branch (registrations.cpp:76-86)
+//       b2r_config cfg;
+//       b2r_config_default(&cfg, B2R_METHOD_GICP_OMP);  // pclomp::GeneralizedIterativeClosestPoint: cost poses applyState(guess, x)
+//       cfg.transformation_epsilon = pnh.param<double>("reg_transformation_epsilon", 0.01);
+//       cfg.max_iterations = pnh.param<int>("reg_maximum_iterations", 64);
+//       cfg.max_correspondence_distance = pnh.param<double>("reg_max_correspondence_distance", 2.5);
+//       cfg.k_correspondences = pnh.param<int>("reg_correspondence_randomness", 20);
+//       cfg.max_optimizer_iterations = pnh.param<int>("reg_max_optimizer_iterations", 20);
 //       cfg.device_id = pnh.param<int>("reg_device_id", 0);
 //       return pcl::Registration<PointT, PointT>::Ptr(new B200Registration<PointT>(cfg));
 //     }

@@ -108,7 +108,7 @@ struct b2r_handle {
   bool src_promoted = false;        // b2r_promote_source_to_target has taken the source away: no source until the next b2r_set_source*
   NdtWork ndt_work;
   VoxelWork vg_work;
-  GicpPclWork gp_work;              // B2R_METHOD_GICP_PCL: correspondence / cost pass buffers
+  GicpPclWork gp_work;              // B2R_METHOD_GICP_PCL / _GICP_OMP: correspondence / cost pass buffers
   DevBuf<char> icp_ws;              // B2R_METHOD_ICP_PCL: the pair's workspace (icp_pair_ws)
   DevBuf<IcpPairDev> icp_pair;      // B2R_METHOD_ICP_PCL: the pair's record
   PinnedBuf<IcpPairDev> icp_h;      // its host copy
@@ -120,8 +120,10 @@ static Cloud& SRC(b2r_handle* h) { return h->clouds[h->src]; }
 static bool gicp_family(int method) { return method == B2R_METHOD_GICP || method == B2R_METHOD_VGICP || method == B2R_METHOD_VGICP_CUDA; }
 // the methods that align to a Gaussian voxel map of the target (vgicp.cuh): FastVGICP's, or FastVGICPCuda's float32 one
 static bool vgicp_family(int method) { return method == B2R_METHOD_VGICP || method == B2R_METHOD_VGICP_CUDA; }
-// the methods whose clouds carry k-NN covariances: FastGICP's, or pcl GICP's raw-moment ones (B2R_METHOD_GICP_PCL)
-static bool cov_family(int method) { return gicp_family(method) || method == B2R_METHOD_GICP_PCL; }
+// the methods that run pcl GICP's computeTransformation / BFGS driver (gicp_pcl.cuh): PCL's GICP, or pclomp's copy of it
+static bool gicp_pcl_family(int method) { return method == B2R_METHOD_GICP_PCL || method == B2R_METHOD_GICP_OMP; }
+// the methods whose clouds carry k-NN covariances: FastGICP's, or pcl GICP's raw-moment ones (B2R_METHOD_GICP_PCL, _GICP_OMP)
+static bool cov_family(int method) { return gicp_family(method) || gicp_pcl_family(method); }
 static bool known_method(int method) { return cov_family(method) || ndt_family(method) || method == B2R_METHOD_ICP_PCL; }
 static Cloud& TGT(b2r_handle* h) { return h->clouds[h->tgt]; }
 
@@ -205,6 +207,15 @@ extern "C" int b2r_select_registration_method(const char* const* keys, const cha
     c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
     c.max_iterations = iparam("reg_maximum_iterations", 64);
     c.k_correspondences = iparam("reg_correspondence_randomness", 20);
+  } else if (method == "B200_GICP_OMP") {
+    // registrations.cpp:76-86: pclomp::GeneralizedIterativeClosestPoint with the GICP branch's six setters (reg_num_threads is not
+    // read).  The plain name GICP_OMP stays with the reference's own branch until integrators have moved to this one
+    b2r_config_default(&c, B2R_METHOD_GICP_OMP);
+    c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
+    c.max_iterations = iparam("reg_maximum_iterations", 64);
+    c.max_correspondence_distance = dparam("reg_max_correspondence_distance", 2.5);
+    c.k_correspondences = iparam("reg_correspondence_randomness", 20);
+    c.max_optimizer_iterations = iparam("reg_max_optimizer_iterations", 20);
   } else if (method.find("GICP") != std::string::npos && method.find("OMP") == std::string::npos && method != "FAST_VGICP_CUDA") {
     // registrations.cpp:66-76 (every name containing GICP but not OMP that no branch above takes): pcl::GeneralizedIterativeClosestPoint.
     // reg_use_reciprocal_correspondences is read upstream and has no effect on GICP; FAST_VGICP_CUDA stays refused (the reference only
@@ -246,7 +257,7 @@ extern "C" int b2r_create(const b2r_config* cfg, b2r_handle** out) {
   if (vgicp_family(cfg->method) && !(cfg->ndt_resolution > 0.0 && std::isfinite(cfg->ndt_resolution)))
     return fail(B2R_EINVAL, "VGICP: ndt_resolution (reg_resolution) must be finite and positive");
   if (cfg->k_correspondences < 1 || cfg->k_correspondences > 64) return fail(B2R_EINVAL, "k_correspondences must be in [1,64]");
-  if (cfg->method == B2R_METHOD_GICP_PCL && cfg->max_optimizer_iterations < 1) return fail(B2R_EINVAL, "max_optimizer_iterations must be >= 1");
+  if (gicp_pcl_family(cfg->method) && cfg->max_optimizer_iterations < 1) return fail(B2R_EINVAL, "max_optimizer_iterations must be >= 1");
   if (cfg->method == B2R_METHOD_ICP_PCL && cfg->use_reciprocal_correspondences != 0 && cfg->use_reciprocal_correspondences != 1)
     return fail(B2R_EINVAL, "use_reciprocal_correspondences must be 0 or 1");
   int ndev = 0;
@@ -532,7 +543,7 @@ static int build_cov(b2r_handle* h, Cloud& c, BuildCtx& B, cudaStream_t st) {
     prof = d_prof;
 #endif
     TEL_BEGIN(&h->tel, st);
-    if (h->cfg.method == B2R_METHOD_GICP_PCL) {  // pcl GICP's raw-moment covariances (gicp_pcl.cuh)
+    if (gicp_pcl_family(h->cfg.method)) {  // pcl GICP's raw-moment covariances (gicp_pcl.cuh)
       rc = launch_raw_cov<PclCov>(h, c, k, smem, st);
       if (rc) return rc;
     } else if (h->cfg.method == B2R_METHOD_VGICP_CUDA) {  // FastVGICPCuda's float32 raw-moment covariances (vgicp_cuda.cuh)
@@ -1020,7 +1031,7 @@ static int gicp_align(b2r_handle* h, const float* guess, b2r_result* out, const 
 }
 
 // ------------------------------------------------------------------------------------------------ pcl GICP align (gicp_pcl.cuh)
-// the two device passes of B2R_METHOD_GICP_PCL over the handle's current source and target (covariances built)
+// the two device passes of B2R_METHOD_GICP_PCL / _GICP_OMP over the handle's current source and target (covariances built)
 struct HandleGicpPclPasses {
   b2r_handle* h;
   explicit HandleGicpPclPasses(b2r_handle* h_) : h(h_) {}
@@ -1033,7 +1044,7 @@ struct HandleGicpPclPasses {
     gicp_pcl_fill_args(h->cfg, s, t, G, T, R, W.corr.p, W.M.p, W.A);
     double cnt = 0.0;
     W.corr_valid = false;
-    rc = gicp_pcl_run<1>(W, true, &h->tel, h->st, &cnt);
+    rc = gicp_pcl_run<1>(W, true, h->cfg.method, &h->tel, h->st, &cnt);
     if (rc) return rc;
     W.m = (uint64_t)cnt;
     W.corr_valid = true;
@@ -1044,7 +1055,7 @@ struct HandleGicpPclPasses {
   int cost(const float* T, double* sums) {
     GicpPclArgs& A = h->gp_work.A;
     for (int i = 0; i < 12; i++) A.T[i] = T[i];
-    return gicp_pcl_run<kGicpPclSums>(h->gp_work, false, &h->tel, h->st, sums);
+    return gicp_pcl_run<kGicpPclSums>(h->gp_work, false, h->cfg.method, &h->tel, h->st, sums);
   }
 };
 
@@ -1139,7 +1150,7 @@ static int align_impl(b2r_handle* h, const float guess[16], b2r_result* out, con
   int rc = need_source(h);
   if (rc != B2R_OK) {}  // reported below like every failed align
   else if (gicp_family(h->cfg.method)) rc = gicp_align(h, guess, out, between);
-  else if (h->cfg.method == B2R_METHOD_GICP_PCL) rc = gicp_pcl_align(h, guess, out);
+  else if (gicp_pcl_family(h->cfg.method)) rc = gicp_pcl_align(h, guess, out);
   else if (h->cfg.method == B2R_METHOD_ICP_PCL) rc = icp_align(h, guess, out);
   else {
     float Tfinal[16];
@@ -1271,7 +1282,7 @@ extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
   if (need_source(h)) return B2R_ESTATE;
   if (!h->corr_valid) return fail(B2R_ESTATE, "no linearisation has run since the clouds were set");
   if (n != SRC(h).n) return fail(B2R_EINVAL, "n does not match the source cloud");
-  if (h->cfg.method == B2R_METHOD_GICP_PCL) return gicp_pcl_fetch_correspondences(h, out, nullptr, n);
+  if (gicp_pcl_family(h->cfg.method)) return gicp_pcl_fetch_correspondences(h, out, nullptr, n);
   if (h->cfg.method == B2R_METHOD_ICP_PCL) return fail(B2R_ESTATE, "pcl ICP handle: use b2r_icp_pcl_correspondences_at");
   // a non-finite source point is not in the source's search structure (pos_of = -1): no search writes its entry, and like a PCL
   // query that finds nothing it has no correspondence
@@ -1286,7 +1297,7 @@ extern "C" int b2r_get_correspondences(b2r_handle* h, int32_t* out, size_t n) {
 
 extern "C" int b2r_get_covariances(b2r_handle* h, int which, double* out, size_t n) {
   if (!h || !out) return fail(B2R_EINVAL, "NULL argument");
-  if (!cov_family(h->cfg.method)) return fail(B2R_ESTATE, "covariances exist only for the GICP, VGICP, VGICP_CUDA and pcl GICP engines");
+  if (!cov_family(h->cfg.method)) return fail(B2R_ESTATE, "covariances exist only for the GICP, VGICP, VGICP_CUDA, pcl GICP and pclomp GICP engines");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (!which && need_source(h)) return B2R_ESTATE;
   Cloud& c = which ? TGT(h) : SRC(h);
@@ -1381,7 +1392,7 @@ static int gicp_pcl_fetch_correspondences(b2r_handle* h, int32_t* corr, double* 
 
 extern "C" int b2r_gicp_pcl_correspondences_at(b2r_handle* h, const float guess[16], const float T_rel[16], int32_t* corr, double* M, uint64_t* n_corr) {
   if (!h || !guess || !T_rel || !n_corr) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_GICP_PCL) return fail(B2R_ESTATE, "pcl GICP engine (B2R_METHOD_GICP_PCL) required");
+  if (!gicp_pcl_family(h->cfg.method)) return fail(B2R_ESTATE, "pcl GICP engine (B2R_METHOD_GICP_PCL or B2R_METHOD_GICP_OMP) required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (need_source(h)) return B2R_ESTATE;
   Cloud& s = SRC(h);
@@ -1405,7 +1416,7 @@ extern "C" int b2r_gicp_pcl_correspondences_at(b2r_handle* h, const float guess[
 
 extern "C" int b2r_gicp_pcl_cost_at(b2r_handle* h, const float T[16], double* f_sum, double* g_sum, double* dR_sum) {
   if (!h || !T || !f_sum || !g_sum || !dR_sum) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_GICP_PCL) return fail(B2R_ESTATE, "pcl GICP engine (B2R_METHOD_GICP_PCL) required");
+  if (!gicp_pcl_family(h->cfg.method)) return fail(B2R_ESTATE, "pcl GICP engine (B2R_METHOD_GICP_PCL or B2R_METHOD_GICP_OMP) required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   if (need_source(h)) return B2R_ESTATE;
   if (!h->corr_valid || !h->gp_work.corr_valid) return fail(B2R_ESTATE, "no correspondence pass has run since the clouds were set");

@@ -286,7 +286,7 @@ static int batch_build_structures(b2r_batch* b, const int32_t* ids, size_t n_ids
   }
   B2R_CUDA(cudaMemcpyAsync(b->d_knn.p, b->h_knn.p, todo.size() * sizeof(KnnBatchItem), cudaMemcpyHostToDevice, st));
   { TEL_BEGIN(&h->tel, st);
-    if (h->cfg.method == B2R_METHOD_GICP_PCL)  // pcl GICP's raw-moment covariances (gicp_pcl.cuh)
+    if (gicp_pcl_family(h->cfg.method))  // pcl GICP's raw-moment covariances (gicp_pcl.cuh)
       k_pcl_cov_reg_batch<kKnnRegK, PclCov><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
     else if (h->cfg.method == B2R_METHOD_VGICP_CUDA)  // FastVGICPCuda's float32 raw-moment covariances (vgicp_cuda.cuh)
       k_pcl_cov_reg_batch<kKnnRegK, VcudaCov><<<dim3(max_blocks, (unsigned)todo.size()), kKnnThreads, 0, st>>>(b->d_knn.p);
@@ -833,7 +833,10 @@ static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t 
     }
     if (cnt[1]) {
       TEL_BEGIN(&h->tel, st);
-      k_gicp_pcl_cost_batch<<<dim3(max_nb[1], (unsigned)cnt[1]), kGicpPclThreads, 0, st>>>(b->d_gp_args.p + cnt[0]);
+      if (gicp_pcl_base_pose(cfg.method))
+        k_gicp_omp_cost_batch<<<dim3(max_nb[1], (unsigned)cnt[1]), kGicpPclThreads, 0, st>>>(b->d_gp_args.p + cnt[0]);
+      else
+        k_gicp_pcl_cost_batch<<<dim3(max_nb[1], (unsigned)cnt[1]), kGicpPclThreads, 0, st>>>(b->d_gp_args.p + cnt[0]);
       TEL_END(&h->tel, KC_GICP_PCL_COST, 1, st);
       B2R_CUDA(cudaGetLastError());
     }
@@ -974,7 +977,7 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   if (ndt) rc = batch_ndt_maps(b, pairs, n_pairs, fit_only);
   if (rc) return rc;
   const bool vgicp = vgicp_family(h->cfg.method) && !fit_only;
-  const bool gpcl = h->cfg.method == B2R_METHOD_GICP_PCL && !fit_only;  // host-driven rounds, like NDT
+  const bool gpcl = gicp_pcl_family(h->cfg.method) && !fit_only;  // host-driven rounds, like NDT
   if (vgicp) rc = batch_vgicp_maps(b, pairs, n_pairs);
   if (rc) return rc;
   const auto t_b = std::chrono::steady_clock::now();

@@ -6,6 +6,8 @@
 //   k_gicp_pcl_corr                <- the correspondence loop of computeTransformation: q = transformation_ (guess p), exact 1-NN,
 //                                     d2 < corr_dist^2 in float64, M = (R C1 R^T + C2)^-1 with Eigen's 3x3 inverse
 //   k_gicp_pcl_cost                <- OptimizationFunctorWithIndices: the 13 sums behind f, df and fdf at one float32 pose
+//   k_gicp_omp_cost                <- the same for pclomp::GeneralizedIterativeClosestPoint (B2R_METHOD_GICP_OMP, the factory's
+//                                     GICP_OMP branch): the pose applyState(guess, x) moves the raw source point (OmpPose)
 // The k-NN traversal and lists (bvh_group_search, KnnRegs, KnnList) and the fixed reduction tree (block_reduce / finish_partials) are
 // shared with FastGICP's kernels; the BFGS driver (gicp_pcl_compute) runs on the host, one device pass per functor evaluation.
 #pragma once
@@ -223,10 +225,29 @@ __global__ void __launch_bounds__(kGicpPclThreads) k_gicp_pcl_corr_batch(const G
   gicp_pcl_corr_body(A);
 }
 
-// OptimizationFunctorWithIndices' loop body at the pose T over the accepted correspondences: res = (double)(pp - tgt) (float32
-// difference), temp = M res, sums f += res^T temp, g += temp, dR += p_src temp^T (p_src = output_i, promoted)
-__device__ __forceinline__ void gicp_pcl_cost_body(const GicpPclArgs& A) {
+// the pose rule of the cost pass: which point the functor's pose T moves.  pcl GICP (PCL 1.10) transforms the source by the guess
+// first, so T = applyState(I, x) moves output_i = guess p; pclomp's GICP (B2R_METHOD_GICP_OMP) keeps base_transformation_ = guess, so
+// T = applyState(guess, x) moves the raw source point (UPSTREAM-RECALL (DOUBT), tests/gicp_omp_ref.cpp; the host side is
+// gicp_pcl::functor_pose)
+struct PclPose {
+  __device__ __forceinline__ static float3 point(float3 o, float4) { return o; }
+};
+struct OmpPose {
+  __device__ __forceinline__ static float3 point(float3, float4 p) { return make_float3(p.x, p.y, p.z); }
+};
+
+// the fixed-tree reduction of a cost pass's 13 sums (outside the templated body below, so that pcl GICP's kernels keep their shared
+// memory layout)
+__device__ __forceinline__ void gicp_pcl_cost_reduce(double* acc, const GicpPclArgs& A) {
   __shared__ double red[kGicpPclSums * 32];
+  block_reduce<kGicpPclSums>(acc, red);
+  finish_partials<kGicpPclSums>(acc, A.partials, A.out, A.counter, A.flag, A.seq, nullptr, A.nrow, A.round, A.round_n);
+}
+
+// OptimizationFunctorWithIndices' loop body at the pose T over the accepted correspondences: res = (double)(T v - tgt) (float32
+// difference, v = Pose::point), temp = M res, sums f += res^T temp, g += temp, dR += p_src temp^T (p_src = output_i, promoted)
+template <class Pose>
+__device__ __forceinline__ void gicp_pcl_cost_body(const GicpPclArgs& A) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
   double acc[kGicpPclSums];
 #pragma unroll
@@ -235,11 +256,12 @@ __device__ __forceinline__ void gicp_pcl_cost_body(const GicpPclArgs& A) {
   if (ci >= 0) {
     const float4 p = A.src.sp[s];
     const float3 o = gicp_pcl_output(A.G, p.x, p.y, p.z);
+    const float3 v = Pose::point(o, p);
     const float4 q4 = A.tgt.sp[ci];
     const float q[3] = {q4.x, q4.y, q4.z};
-    const double r[3] = {(double)fsub(xform_row(A.T[0], A.T[1], A.T[2], A.T[3], o.x, o.y, o.z), q[0]),
-                         (double)fsub(xform_row(A.T[4], A.T[5], A.T[6], A.T[7], o.x, o.y, o.z), q[1]),
-                         (double)fsub(xform_row(A.T[8], A.T[9], A.T[10], A.T[11], o.x, o.y, o.z), q[2])};
+    const double r[3] = {(double)fsub(xform_row(A.T[0], A.T[1], A.T[2], A.T[3], v.x, v.y, v.z), q[0]),
+                         (double)fsub(xform_row(A.T[4], A.T[5], A.T[6], A.T[7], v.x, v.y, v.z), q[1]),
+                         (double)fsub(xform_row(A.T[8], A.T[9], A.T[10], A.T[11], v.x, v.y, v.z), q[2])};
     const double* M = A.M + (size_t)s * 9;
     double t[3];
 #pragma unroll
@@ -252,17 +274,29 @@ __device__ __forceinline__ void gicp_pcl_cost_body(const GicpPclArgs& A) {
 #pragma unroll
       for (int b = 0; b < 3; b++) acc[4 + a * 3 + b] = dmul(pd[a], t[b]);
   }
-  block_reduce<kGicpPclSums>(acc, red);
-  finish_partials<kGicpPclSums>(acc, A.partials, A.out, A.counter, A.flag, A.seq, nullptr, A.nrow, A.round, A.round_n);
+  gicp_pcl_cost_reduce(acc, A);
 }
 
-__global__ void __launch_bounds__(kGicpPclThreads) k_gicp_pcl_cost(const __grid_constant__ GicpPclArgs A) { gicp_pcl_cost_body(A); }
+__global__ void __launch_bounds__(kGicpPclThreads) k_gicp_pcl_cost(const __grid_constant__ GicpPclArgs A) { gicp_pcl_cost_body<PclPose>(A); }
 
 __global__ void __launch_bounds__(kGicpPclThreads) k_gicp_pcl_cost_batch(const GicpPclArgs* __restrict__ recs) {
   const GicpPclArgs& A = recs[blockIdx.y];
   if (blockIdx.x >= A.nrow) return;
-  gicp_pcl_cost_body(A);
+  gicp_pcl_cost_body<PclPose>(A);
 }
+
+// the same two for pclomp's GICP (OmpPose)
+__global__ void __launch_bounds__(kGicpPclThreads) k_gicp_omp_cost(const __grid_constant__ GicpPclArgs A) { gicp_pcl_cost_body<OmpPose>(A); }
+
+__global__ void __launch_bounds__(kGicpPclThreads) k_gicp_omp_cost_batch(const GicpPclArgs* __restrict__ recs) {
+  const GicpPclArgs& A = recs[blockIdx.y];
+  if (blockIdx.x >= A.nrow) return;
+  gicp_pcl_cost_body<OmpPose>(A);
+}
+
+// does this method's functor evaluate at applyState(guess, x) on the raw source (pclomp's GICP) rather than applyState(I, x) on
+// guess p (pcl GICP)?
+inline bool gicp_pcl_base_pose(int method) { return method == B2R_METHOD_GICP_OMP; }
 
 // ------------------------------------------------------------------------------------------------ host side
 // per-handle workspaces of the two passes
@@ -304,9 +338,9 @@ inline void gicp_pcl_fill_args(const b2r_config& cfg, const Cloud& s, const Clou
   A.corr = corr; A.M = M;
 }
 
-// one pass of either kernel; waits for its message and copies the NV result words to res
+// one pass of either kernel (the cost kernel of the method's pose rule); waits for its message and copies the NV result words to res
 template <int NV>
-inline int gicp_pcl_run(GicpPclWork& W, bool corr_pass, Telemetry* tel, cudaStream_t st, double* res) {
+inline int gicp_pcl_run(GicpPclWork& W, bool corr_pass, int method, Telemetry* tel, cudaStream_t st, double* res) {
   GicpPclArgs& A = W.A;
   A.partials = W.partials.p; A.counter = W.counter.p; A.out = W.msg.d;
   A.flag = reinterpret_cast<unsigned long long*>(W.msg.d + 16);
@@ -314,6 +348,7 @@ inline int gicp_pcl_run(GicpPclWork& W, bool corr_pass, Telemetry* tel, cudaStre
   const unsigned nb = (unsigned)((size_t)A.src.nsup * 1024 / kGicpPclThreads);
   TEL_BEGIN(tel, st);
   if (corr_pass) k_gicp_pcl_corr<<<nb, kGicpPclThreads, 0, st>>>(A);
+  else if (gicp_pcl_base_pose(method)) k_gicp_omp_cost<<<nb, kGicpPclThreads, 0, st>>>(A);
   else k_gicp_pcl_cost<<<nb, kGicpPclThreads, 0, st>>>(A);
   TEL_END(tel, corr_pass ? KC_GICP_PCL_CORR : KC_GICP_PCL_COST, 1, st);
   B2R_CUDA(cudaGetLastError());
@@ -377,6 +412,22 @@ inline void apply_state(const V6& x, float* T) {
   T[12] = T[13] = T[14] = 0.f; T[15] = 1.f;
 }
 
+// the pose the functor evaluates at x (row-major float 4x4).  base == nullptr (pcl GICP): applyState(I, x).  Otherwise pclomp's
+// applyState(base_transformation_ = guess, x): [R(x) R_g | t_g + t(x)], the 3x3 product in float32 ((a0 b0 + a1 b1) + a2 b2), the
+// bottom row the guess's (UPSTREAM-RECALL (DOUBT), tests/gicp_omp_ref.cpp; the device side is OmpPose)
+inline void functor_pose(const V6& x, const float* base, float* T) {
+  apply_state(x, T);
+  if (!base) return;
+  float R[9];
+  for (int i = 0; i < 3; i++)
+    for (int j = 0; j < 3; j++) R[i * 3 + j] = fadd(fadd(fmul(T[i * 4], base[j]), fmul(T[i * 4 + 1], base[4 + j])), fmul(T[i * 4 + 2], base[8 + j]));
+  for (int i = 0; i < 3; i++) {
+    for (int j = 0; j < 3; j++) T[i * 4 + j] = R[i * 3 + j];
+    T[i * 4 + 3] = fadd(base[i * 4 + 3], T[i * 4 + 3]);
+  }
+  for (int j = 0; j < 4; j++) T[12 + j] = base[12 + j];
+}
+
 // computeRDerivative: g[3..5] = <dR/dangle, Rsum> with matricesInnerProd(a, b) = sum_i sum_j a(j, i) b(i, j)
 inline void r_derivative(const V6& x, const double* Rs, V6& g) {
   const double phi = x[3], theta = x[4], psi = x[5];
@@ -405,13 +456,15 @@ inline void r_derivative(const V6& x, const double* Rs, V6& g) {
 struct Functor {
   Replay* R = nullptr;
   int m = 0;
+  float base[16];            // the guess, when the pose rule is pclomp's (has_base)
+  bool has_base = false;
   float lastT[16];
   double last[kGicpPclSums];
   bool have = false;
   int evaluations = 0, passes = 0;
   void sums(const V6& x, double* s) {
     float T[16];
-    apply_state(x, T);
+    functor_pose(x, has_base ? base : nullptr, T);
     evaluations++;
     if (!(have && std::memcmp(T, lastT, sizeof(T)) == 0)) {
       if (R->idx == R->log.size()) {
@@ -669,7 +722,8 @@ struct Bfgs {
 
 }  // namespace gicp_pcl
 
-// GeneralizedIterativeClosestPoint::computeTransformation (PCL 1.10) as a resumable state machine.  next() names the pass the
+// GeneralizedIterativeClosestPoint::computeTransformation (PCL 1.10, and pclomp's copy of it for B2R_METHOD_GICP_OMP, whose cost
+// passes are at applyState(guess, x): Functor::base) as a resumable state machine.  next() names the pass the
 // registration needs — correspondences at (guess, T()) or a cost pass at T() — and consume_*() hands it the result, so one pair runs
 // alone (the single handle) or beside many others whose passes share launches (the batch), through the same statements.
 // Inside BFGS the state is checkpointed before every minimizeOneStep: a step that needs a cost pass unwinds and is re-run from its
@@ -702,6 +756,10 @@ class GicpPclPairState {
                        std::asin(-(double)w.Tcur[8]), (double)std::atan2(w.Tcur[4], w.Tcur[0])};
     w.bfgs = gicp_pcl::Bfgs();
     w.bfgs.fn.m = (int)m;
+    if (gicp_pcl_base_pose(cfg_.method)) {  // pclomp: the functor's poses are applyState(guess, x)
+      std::memcpy(w.bfgs.fn.base, G_, sizeof(G_));
+      w.bfgs.fn.has_base = true;
+    }
     w.phase = P_INIT;
     rep_.log.clear();
     advance();

@@ -18,7 +18,7 @@ library; nothing here computes.
 import ctypes as C
 import numpy as np
 from . import _capi
-from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL, B2R_METHOD_VGICP_CUDA  # noqa: F401
+from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL, B2R_METHOD_VGICP_CUDA, B2R_METHOD_GICP_OMP  # noqa: F401
 
 
 def _cloud(a):
@@ -286,7 +286,7 @@ class Registration:
         return H, b, cost.value, nc.value, vox[:n_source]
 
     def gicpPclCorrespondencesAt(self, guess, T_rel, n_source):
-        """(pcl GICP) one correspondence pass at (guess, T_rel): (target index of every source point (n,) int32, -1 = none,
+        """(pcl GICP, pclomp GICP) one correspondence pass at (guess, T_rel): (target index of every source point (n,) int32, -1 = none,
         Mahalanobis matrices (n, 3, 3), NaN where there is none, accepted count)"""
         g = _colmajor(guess, np.float32)
         t = _colmajor(T_rel, np.float32)
@@ -299,7 +299,7 @@ class Registration:
         return corr[:n_source], M[:n_source], nc.value
 
     def gicpPclCostAt(self, T):
-        """(pcl GICP) one cost pass at T over the last correspondences: (sum res^T M res, sum M res (3,), sum p (M res)^T (3, 3))"""
+        """(pcl GICP, pclomp GICP: T moves the raw source point) one cost pass at T over the last correspondences: (sum res^T M res, sum M res (3,), sum p (M res)^T (3, 3))"""
         t = _colmajor(T, np.float32)
         f = C.c_double()
         g = np.empty(3, np.float64)

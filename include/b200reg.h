@@ -66,6 +66,13 @@ extern "C" {
                                    ndt_resolution (reg_resolution) with cells floor(p / res - 0.5), DIRECT1 voxel correspondences and
                                    float32 terms weighted sqrt(num_points), summed in float64; reads max_iterations / k_correspondences /
                                    transformation_epsilon, not max_correspondence_distance */
+/* id 7 is left unassigned (an unknown method: b2r_config_default returns B2R_EINVAL for it) */
+#define B2R_METHOD_GICP_OMP 8 /* pclomp::GeneralizedIterativeClosestPoint semantics (ndt_omp's copy of PCL's GICP, registrations.cpp:76-86,
+                                 opted into as B200_GICP_OMP): B2R_METHOD_GICP_PCL's covariances, correspondences, BFGS and outer loop,
+                                 reading the same fields, except the pose every functor evaluation (cost pass) uses: applyState(guess, x)
+                                 = [R(x) R_guess | t_guess + t(x)] applied to the raw source point, where pcl GICP applies applyState(I, x)
+                                 to guess * p.  With a translated guess the end pose differs from GICP's by about (R(x*) - I) t_guess.
+                                 This pose rule is recalled, not read from the sources (DOUBT) */
 
 typedef struct b2r_handle b2r_handle;
 
@@ -85,7 +92,7 @@ typedef struct b2r_config {
   int32_t ndt_mt_interval_flag;       /* 0 = ndt_omp polarity (More-Thuente loop never entered), 1 = active line search */
   int32_t ndt_fixed_iterations;       /* >0: exactly this many iterations (BASELINE config 3), convergence test off */
   float grid_cell_min;                /* engine tuning: smallest search-grid cell, power of two (default 0.5 m) */
-  int32_t max_optimizer_iterations;   /* reg_max_optimizer_iterations      (20)   pcl GICP max_inner_iterations_ (B2R_METHOD_GICP_PCL) */
+  int32_t max_optimizer_iterations;   /* reg_max_optimizer_iterations      (20)   pcl GICP max_inner_iterations_ (B2R_METHOD_GICP_PCL, _GICP_OMP) */
   int32_t use_reciprocal_correspondences; /* reg_use_reciprocal_correspondences (false): 0 or 1, read by B2R_METHOD_ICP_PCL only */
 } b2r_config;
 
@@ -109,8 +116,9 @@ int b2r_config_default(b2r_config* cfg, int method);
  * "NDT_OMP"/"B200_NDT" -> NDT engine, "NDT" -> pcl NDT engine (B2R_METHOD_NDT_PCL), "FAST_VGICP"/"B200_VGICP" -> VGICP engine
  * (B2R_METHOD_VGICP), "GICP"/"B200_GICP_PCL" and every other name that reaches the reference's GICP branch (contains "GICP" but not
  * "OMP") -> pcl GICP engine (B2R_METHOD_GICP_PCL), "B200_ICP" -> pcl ICP engine (B2R_METHOD_ICP_PCL; reg_use_reciprocal_correspondences
- * must be true / false / 1 / 0, else B2R_EINVAL), "B200_VGICP_CUDA" -> FastVGICPCuda engine (B2R_METHOD_VGICP_CUDA).
- * ICP / GICP_OMP / FAST_VGICP_CUDA and unknown names are not re-created: returns
+ * must be true / false / 1 / 0, else B2R_EINVAL), "B200_VGICP_CUDA" -> FastVGICPCuda engine (B2R_METHOD_VGICP_CUDA),
+ * "B200_GICP_OMP" -> pclomp GICP engine (B2R_METHOD_GICP_OMP; the GICP branch's parameters and defaults).
+ * ICP / GICP_OMP (and every other name containing GICP and OMP) / FAST_VGICP_CUDA and unknown names are not re-created: returns
  * B2R_EUNSUPPORTED so the caller keeps the reference's own branch.  (Built without USE_VGICP_CUDA the reference sends FAST_VGICP_CUDA to
  * its GICP branch; this factory refuses it all the same, so the caller decides.) */
 int b2r_select_registration_method(const char* const* keys, const char* const* values, int n_params, int device_id,
@@ -212,14 +220,16 @@ int b2r_vgicp_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int32
  * may be NULL) = the index of the point's voxel in b2r_vgicp_get_voxels' order, or -1 */
 int b2r_vgicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* cost, uint64_t* n_corr, int32_t* voxel_of, size_t n);
 
-/* B2R_METHOD_GICP_PCL: one correspondence pass of pcl GICP's computeTransformation at the guess (applied to the source first,
+/* B2R_METHOD_GICP_PCL / B2R_METHOD_GICP_OMP (the same pass for both): one correspondence pass of pcl GICP's computeTransformation at the guess (applied to the source first,
  * transformPointCloud) and T_rel (transformation_), both column-major float: corr[n] (caller's point order, may be NULL) = the target
  * index of the exact 1-NN when its squared distance < max_correspondence_distance^2, else -1; M[9 n] (may be NULL) = the Mahalanobis
  * matrix (R C1 R^T + C2)^-1, 3x3 row-major, of every accepted point (NaN elsewhere); *n_corr = the accepted count.  The cost tap below
  * reads these correspondences. */
 int b2r_gicp_pcl_correspondences_at(b2r_handle* h, const float guess[16], const float T_rel[16], int32_t* corr, double* M, uint64_t* n_corr);
-/* B2R_METHOD_GICP_PCL: one cost pass (OptimizationFunctorWithIndices) at the column-major float pose T over the last correspondences:
- * *f_sum = sum res^T M res, g_sum[3] = sum M res, dR_sum[9] = sum p_src (M res)^T (row-major), unscaled (the functor divides by m) */
+/* B2R_METHOD_GICP_PCL / B2R_METHOD_GICP_OMP: one cost pass (OptimizationFunctorWithIndices) at the column-major float pose T over the
+ * last correspondences: *f_sum = sum res^T M res, g_sum[3] = sum M res, dR_sum[9] = sum p_src (M res)^T (row-major), unscaled (the
+ * functor divides by m), with p_src = guess * p.  GICP_PCL: res = T (guess * p) - q, T being applyState(I, x) in an align.  GICP_OMP:
+ * res = T p - q on the raw source point p, T being applyState(guess, x) in an align, with the guess of the last correspondence pass */
 int b2r_gicp_pcl_cost_at(b2r_handle* h, const float T[16], double* f_sum, double* g_sum, double* dR_sum);
 
 /* B2R_METHOD_ICP_PCL: one correspondence pass with the source transformed once by the column-major float T (transformPointCloud),
@@ -418,7 +428,7 @@ int b2r_loop_matching(b2r_handle* h, const void* new_keyframe, size_t n_new, siz
  * Newton / More-Thuente driver and each round of derivative passes covers every pair in flight (one host wait per round).
  * Pose, flag, iteration count and fitness are bitwise those of b2r_set_target / b2r_set_source / b2r_align / b2r_fitness on
  * one NDT handle; b2r_batch_last_rounds counts batched rounds and, per pair, derivative / Hessian passes.
- * pcl GICP config (B2R_METHOD_GICP_PCL): every pair runs the single handle's computeTransformation / BFGS driver and each round has at
+ * pcl GICP config (B2R_METHOD_GICP_PCL, and pclomp GICP, B2R_METHOD_GICP_OMP): every pair runs the single handle's computeTransformation / BFGS driver and each round has at
  * most one batched correspondence launch and one batched cost launch (one host wait per round); the records are bitwise the single
  * handle's, and b2r_batch_last_rounds counts, per pair, correspondence and cost passes.
  *
