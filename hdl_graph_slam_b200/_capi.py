@@ -8,7 +8,7 @@ LIB_PATH = os.environ.get("B2R_LIB") or os.path.join(_HERE, "_lib", "libb200reg.
 
 B2R_OK = 0
 B2R_EINVAL, B2R_ENODEVICE, B2R_ECUDA, B2R_ESTATE, B2R_EUNSUPPORTED, B2R_ENCCL = -1, -2, -3, -4, -5, -6
-B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL, B2R_METHOD_VGICP_CUDA, B2R_METHOD_GICP_OMP = 0, 1, 2, 3, 4, 5, 6, 8  # 7 is unassigned
+B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL, B2R_METHOD_VGICP_CUDA, B2R_METHOD_GICP_OMP, B2R_METHOD_NDT_KDTREE = 0, 1, 2, 3, 4, 5, 6, 8, 9  # 7 is unassigned
 B2R_DOWNSAMPLE_NONE, B2R_DOWNSAMPLE_VOXELGRID, B2R_DOWNSAMPLE_APPROX_VOXELGRID = 0, 1, 2
 
 

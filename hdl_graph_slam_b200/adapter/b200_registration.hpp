@@ -99,7 +99,8 @@ public:
                       : cfg.method == B2R_METHOD_GICP_PCL ? "B200_GICP_PCL"
                       : cfg.method == B2R_METHOD_ICP_PCL ? "B200_ICP"
                       : cfg.method == B2R_METHOD_VGICP_CUDA ? "B200_VGICP_CUDA"
-                      : cfg.method == B2R_METHOD_GICP_OMP ? "B200_GICP_OMP" : "B200_NDT";
+                      : cfg.method == B2R_METHOD_GICP_OMP ? "B200_GICP_OMP"
+                      : cfg.method == B2R_METHOD_NDT_KDTREE ? "B200_NDT_KDTREE" : "B200_NDT";
     this->max_iterations_ = cfg.max_iterations;
     this->transformation_epsilon_ = cfg.transformation_epsilon;
     this->corr_dist_threshold_ = cfg.max_correspondence_distance;
@@ -227,6 +228,15 @@ private:
 //       cfg.transformation_epsilon = pnh.param<double>("reg_transformation_epsilon", 0.01);
 //       cfg.max_iterations = pnh.param<int>("reg_maximum_iterations", 64);
 //       cfg.k_correspondences = pnh.param<int>("reg_correspondence_randomness", 20);
+//       cfg.device_id = pnh.param<int>("reg_device_id", 0);
+//       return pcl::Registration<PointT, PointT>::Ptr(new B200Registration<PointT>(cfg));
+//     }
+//     else if(registration_method == "B200_NDT_KDTREE") {  // in place of NDT_OMP with reg_nn_search_method = KDTREE (:112-113)
+//       b2r_config cfg;
+//       b2r_config_default(&cfg, B2R_METHOD_NDT_KDTREE);  // pclomp::NormalDistributionsTransform: radius search over the centroids
+//       cfg.transformation_epsilon = pnh.param<double>("reg_transformation_epsilon", 0.01);
+//       cfg.max_iterations = pnh.param<int>("reg_maximum_iterations", 64);
+//       cfg.ndt_resolution = pnh.param<double>("reg_resolution", 0.5);
 //       cfg.device_id = pnh.param<int>("reg_device_id", 0);
 //       return pcl::Registration<PointT, PointT>::Ptr(new B200Registration<PointT>(cfg));
 //     }

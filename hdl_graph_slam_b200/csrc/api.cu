@@ -183,6 +183,14 @@ extern "C" int b2r_select_registration_method(const char* const* keys, const cha
     std::string sm = s ? s : "DIRECT7";
     if (sm == "KDTREE") return fail(B2R_EUNSUPPORTED, "reg_nn_search_method=KDTREE is not re-created (DIRECT1/DIRECT7 only)");
     c.ndt_search_method = (sm == "DIRECT1") ? 1 : 7;  // registrations.cpp:112-118: anything else -> DIRECT7
+  } else if (method == "B200_NDT_KDTREE") {
+    // registrations.cpp:101-120 with reg_nn_search_method = KDTREE (:112-113): pclomp::NormalDistributionsTransform with resolution,
+    // transformation epsilon and maximum iterations; ndt_search_method is not read.  The KDTREE value of the NDT_OMP / B200_NDT
+    // branch stays refused, so that no existing caller's method changes under it
+    b2r_config_default(&c, B2R_METHOD_NDT_KDTREE);
+    c.ndt_resolution = dparam("reg_resolution", 0.5);
+    c.transformation_epsilon = dparam("reg_transformation_epsilon", 0.01);
+    c.max_iterations = iparam("reg_maximum_iterations", 64);
   } else if (method == "NDT") {
     // registrations.cpp:93-100: pcl::NormalDistributionsTransform with transformation epsilon, maximum iterations and resolution;
     // step size and outlier ratio stay PCL's defaults, and neither reg_nn_search_method nor reg_num_threads is read
@@ -1573,7 +1581,7 @@ extern "C" int b2r_ndt_hessian_at(b2r_handle* h, const double p[6], double* H) {
 
 extern "C" int b2r_ndt_get_centroids(b2r_handle* h, size_t capacity, size_t* n_centroids, int64_t* keys, float* xyz) {
   if (!h || !n_centroids) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_NDT_PCL) return fail(B2R_ESTATE, "pcl NDT engine (B2R_METHOD_NDT_PCL) required");
+  if (!ndt_radius_family(h->cfg.method)) return fail(B2R_ESTATE, "pcl NDT or KDTREE NDT engine (B2R_METHOD_NDT_PCL or B2R_METHOD_NDT_KDTREE) required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   int rc = ndt_ensure_map(h->cfg, TGT(h), h->ndt_work, h->st);
   if (rc) return rc;
@@ -1582,7 +1590,7 @@ extern "C" int b2r_ndt_get_centroids(b2r_handle* h, size_t capacity, size_t* n_c
 
 extern "C" int b2r_ndt_neighbors_at(b2r_handle* h, const double p[6], uint32_t* counts, size_t capacity, int64_t* keys, size_t* total) {
   if (!h || !p || !total) return fail(B2R_EINVAL, "NULL argument");
-  if (h->cfg.method != B2R_METHOD_NDT_PCL) return fail(B2R_ESTATE, "pcl NDT engine (B2R_METHOD_NDT_PCL) required");
+  if (!ndt_radius_family(h->cfg.method)) return fail(B2R_ESTATE, "pcl NDT or KDTREE NDT engine (B2R_METHOD_NDT_PCL or B2R_METHOD_NDT_KDTREE) required");
   B2R_CUDA(cudaSetDevice(h->cfg.device_id));
   *total = 0;
   if (need_source(h)) return B2R_ESTATE;

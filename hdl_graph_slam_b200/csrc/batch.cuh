@@ -70,7 +70,7 @@ struct b2r_batch {
   DevBuf<char> ndt_ws;              // per pair in flight: chunk rows, group rows, counters, ticket counter; fitness partials
   DevBuf<NdtArgs> d_ndt_args;       // the round's pass records, grouped by pass kind
   PinnedBuf<NdtArgs> h_ndt_args;    // staging
-  DevBuf<NdtPclArgs> d_pcl_args;    // the same records with the radius-search inputs (B2R_METHOD_NDT_PCL)
+  DevBuf<NdtPclArgs> d_pcl_args;    // the same records with the radius-search inputs (B2R_METHOD_NDT_PCL, _NDT_KDTREE)
   PinnedBuf<NdtPclArgs> h_pcl_args;
   MappedBuf<double> h_ndt_msg;      // one result message per record of the round, then the round's flag (8 doubles)
   DevBuf<unsigned int> d_ndt_round; // messages of the current round (the last one publishes the flag and re-arms it)
@@ -598,8 +598,11 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
   b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
   const b2r_config& cfg = h->cfg;
-  // pcl::NormalDistributionsTransform: the Hessian-only pass is the derivative pass with the Hessian (ndt_run_pass)
+  // pcl::NormalDistributionsTransform: the Hessian-only pass is the derivative pass with the Hessian (ndt_run_pass).  NDT_OMP's KDTREE
+  // runs its own three kernels; both read the radius-search records
   const bool pcl = cfg.method == B2R_METHOD_NDT_PCL;
+  const bool kd = cfg.method == B2R_METHOD_NDT_KDTREE;
+  const bool radius = pcl || kd;
   auto kind_of_pass = [&](int k) { return (pcl && k == NDT_PASS_HESS) ? (int)NDT_PASS_DERIV_HESS : k; };
   std::vector<NdtPairState> S(m);
   std::vector<size_t> active, off(m, 0), fit_off(m, 0);
@@ -625,7 +628,7 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
   B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
   B2R_CUDA(b->d_ndt_args.reserve(m));
   B2R_CUDA(b->h_ndt_args.alloc(m));
-  if (pcl) { B2R_CUDA(b->d_pcl_args.reserve(m)); B2R_CUDA(b->h_pcl_args.alloc(m)); }
+  if (radius) { B2R_CUDA(b->d_pcl_args.reserve(m)); B2R_CUDA(b->h_pcl_args.alloc(m)); }
   if (b->h_ndt_msg.cap < m * kNdtMsg + 8) {
     B2R_CUDA(b->h_ndt_msg.alloc(m * kNdtMsg + 8));
     std::memset(b->h_ndt_msg.p, 0, b->h_ndt_msg.cap * sizeof(double));
@@ -651,7 +654,7 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
     unsigned G[3] = {0, 0, 0};
     for (int k = 0; k < 2; k++)
       if (cnt[k]) {
-        const unsigned res = pcl ? ndt_pcl_resident_blocks(k == 0) : ndt_resident_blocks(k == 0);
+        const unsigned res = pcl ? ndt_pcl_resident_blocks(k == 0) : kd ? ndt_kdtree_resident_blocks(k == 0) : ndt_resident_blocks(k == 0);
         G[k] = std::max(1u, std::min(max_nb[k], (unsigned)((4ull * res + cnt[k] - 1) / cnt[k])));
       }
     G[2] = max_nb[2];
@@ -678,9 +681,9 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       A.seq = seq;
       A.round = b->d_ndt_round.p;
       A.round_n = (unsigned)order.size();
-      if (pcl) ndt_pcl_fill_args(cfg, t, A, b->h_pcl_args.p[r]);
+      if (radius) ndt_pcl_fill_args(cfg, t, A, b->h_pcl_args.p[r]);
     }
-    if (pcl) {
+    if (radius) {
       B2R_CUDA(cudaMemcpyAsync(b->d_pcl_args.p, b->h_pcl_args.p, order.size() * sizeof(NdtPclArgs), cudaMemcpyHostToDevice, st));
       h->tel.h2d += order.size() * sizeof(NdtPclArgs);
     } else {
@@ -694,6 +697,9 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       TEL_BEGIN(&h->tel, st);
       if (pcl && k == NDT_PASS_DERIV_HESS) k_ndt_pcl_derivatives_batch<true><<<grid, kNdtThreads, 0, st>>>(b->d_pcl_args.p + r0);
       else if (pcl) k_ndt_pcl_derivatives_batch<false><<<grid, kNdtThreads, 0, st>>>(b->d_pcl_args.p + r0);
+      else if (kd && k == NDT_PASS_DERIV_HESS) k_ndt_kdtree_derivatives_batch<true><<<grid, kNdtThreads, 0, st>>>(b->d_pcl_args.p + r0);
+      else if (kd && k == NDT_PASS_DERIV) k_ndt_kdtree_derivatives_batch<false><<<grid, kNdtThreads, 0, st>>>(b->d_pcl_args.p + r0);
+      else if (kd) k_ndt_kdtree_hessian_batch<<<grid, kNdtThreads, 0, st>>>(b->d_pcl_args.p + r0);
       else if (k == NDT_PASS_DERIV_HESS) k_ndt_derivatives_batch<true><<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
       else if (k == NDT_PASS_DERIV) k_ndt_derivatives_batch<false><<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);
       else k_ndt_hessian_batch<<<grid, kNdtThreads, 0, st>>>(b->d_ndt_args.p + r0);

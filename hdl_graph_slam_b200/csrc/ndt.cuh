@@ -58,7 +58,7 @@ struct NdtVoxelMap {
   DevBuf<unsigned long long> table;  // (pos << 32) | key, kNdtEmpty = free
   unsigned int mask = 0;
   size_t n = 0;
-  // B2R_METHOD_NDT_PCL targets only (ndt_pcl.cuh): the leaf centroids and their bucket CSR
+  // B2R_METHOD_NDT_PCL / _NDT_KDTREE targets only (ndt_pcl.cuh): the leaf centroids and their bucket CSR
   DevBuf<float4> cent;                   // per sorted position of a voxel's first point: its centroid (x, y, z, bits(position))
   DevBuf<unsigned long long> bkey, bkey_sorted;  // bucket key per position (kPclNoBucket: no centroid there), and sorted
   DevBuf<int> bpos_in, bpos;             // positions, and positions in bucket order
@@ -67,7 +67,7 @@ struct NdtVoxelMap {
   unsigned int bmask = 0;
 };
 
-inline bool ndt_family(int method) { return method == B2R_METHOD_NDT || method == B2R_METHOD_NDT_PCL; }
+inline bool ndt_family(int method) { return method == B2R_METHOD_NDT || method == B2R_METHOD_NDT_PCL || method == B2R_METHOD_NDT_KDTREE; }
 
 struct NdtWork {
   DevBuf<double> partials;
@@ -276,6 +276,107 @@ __device__ __forceinline__ void ndt_rows_sum(const double* rows, int R, double* 
   s += __shfl_xor_sync(0xffffffffu, s, 2);
   s += __shfl_xor_sync(0xffffffffu, s, 1);
   if (row < R && part == 0) dst[row] = s;
+}
+
+// computePointDerivatives(x) of the original point, float32: x . j_ang rows (the non-constant entries of J) and x . h_ang rows
+// (the angular block of point_hessian_: a = (0, ha1, ha2), b, c alike, d, e, f full)
+struct NdtOmpPoint {
+  float j13, j23, j04, j14, j24, j05, j15, j25;
+  float ha1, ha2, hb1, hb2, hc1, hc2, hd0, hd1, hd2, he0, he1, he2, hf0, hf1, hf2;
+};
+
+// the point derivatives as ndt_derivatives_body computes them inline (the h entries only with the Hessian: the term reads them only then)
+template <bool HESS>
+__device__ __forceinline__ void ndt_omp_point(const NdtArgs& A, float x, float y, float z, NdtOmpPoint& pd) {
+  pd.j13 = dot3f(A.jang[0], x, y, z); pd.j23 = dot3f(A.jang[1], x, y, z);
+  pd.j04 = dot3f(A.jang[2], x, y, z); pd.j14 = dot3f(A.jang[3], x, y, z); pd.j24 = dot3f(A.jang[4], x, y, z);
+  pd.j05 = dot3f(A.jang[5], x, y, z); pd.j15 = dot3f(A.jang[6], x, y, z); pd.j25 = dot3f(A.jang[7], x, y, z);
+  if (HESS) {
+    pd.ha1 = dot3f(A.hang[0], x, y, z); pd.ha2 = dot3f(A.hang[1], x, y, z);
+    pd.hb1 = dot3f(A.hang[2], x, y, z); pd.hb2 = dot3f(A.hang[3], x, y, z);
+    pd.hc1 = dot3f(A.hang[4], x, y, z); pd.hc2 = dot3f(A.hang[5], x, y, z);
+    pd.hd0 = dot3f(A.hang[6], x, y, z); pd.hd1 = dot3f(A.hang[7], x, y, z); pd.hd2 = dot3f(A.hang[8], x, y, z);
+    pd.he0 = dot3f(A.hang[9], x, y, z); pd.he1 = dot3f(A.hang[10], x, y, z); pd.he2 = dot3f(A.hang[11], x, y, z);
+    pd.hf0 = dot3f(A.hang[12], x, y, z); pd.hf1 = dot3f(A.hang[13], x, y, z); pd.hf2 = dot3f(A.hang[14], x, y, z);
+  }
+}
+
+// ndt_omp's float32 updateDerivatives for one (point, cell), in exactly the operation order of oracle/ndt.cpp::ndt_point_cell:
+// q = (float)((double)x' - mean), C = (float)icov, exp as (float)exp((double)x).  acc: score, g[6], the upper triangle of H in
+// float64 registers; low: this thread's float64 column of the strict lower triangle (stride kNdtRow).  A term that fails the range
+// check adds nothing, not even its score.  The KDTREE pass (ndt_kdtree.cuh) runs it; ndt_derivatives_body keeps its own inline copy
+// of these very statements: calling this helper there moved the register assignment of k_ndt_derivatives_batch and made an NDT_OMP
+// loop batch 2.5-3.5 % slower on an H100, with bit-identical sums.
+template <bool HESS>
+__device__ __forceinline__ void ndt_omp_term(double d1, float d2f, const NdtCell* L, float xt, float yt, float zt, const NdtOmpPoint& pd,
+                                             double* acc, double* low) {
+  const float j13 = pd.j13, j23 = pd.j23, j04 = pd.j04, j14 = pd.j14, j24 = pd.j24, j05 = pd.j05, j15 = pd.j15, j25 = pd.j25;
+  const float q0 = (float)((double)xt - L->mean[0]), q1 = (float)((double)yt - L->mean[1]), q2 = (float)((double)zt - L->mean[2]);
+  float C[9];
+#pragma unroll
+  for (int k = 0; k < 9; k++) C[k] = L->icov[k];
+  // qC = q^T C ; gq[0..2] == qC
+  float gq[6];
+#pragma unroll
+  for (int j = 0; j < 3; j++) gq[j] = fadd(fadd(fmul(q0, C[0 * 3 + j]), fmul(q1, C[1 * 3 + j])), fmul(q2, C[2 * 3 + j]));
+  const float qCq = fadd(fadd(fmul(q0, gq[0]), fmul(q1, gq[1])), fmul(q2, gq[2]));
+  const float arg = fmul(fmul(-d2f, qCq), 0.5f);
+  float exv = (float)exp((double)arg);
+  const float score_inc = (float)(-d1 * (double)exv);
+  exv = fmul(d2f, exv);
+  if (exv > 1.f || exv < 0.f || exv != exv) return;  // contributes nothing (score_inc dropped as well)
+  exv = (float)((double)exv * d1);
+  // CJ columns 3..5 (columns 0..2 are C itself)
+  float CJ3[3], CJ4[3], CJ5[3];
+#pragma unroll
+  for (int r = 0; r < 3; r++) {
+    CJ3[r] = fadd(fmul(C[r * 3 + 1], j13), fmul(C[r * 3 + 2], j23));
+    CJ4[r] = fadd(fadd(fmul(C[r * 3 + 0], j04), fmul(C[r * 3 + 1], j14)), fmul(C[r * 3 + 2], j24));
+    CJ5[r] = fadd(fadd(fmul(C[r * 3 + 0], j05), fmul(C[r * 3 + 1], j15)), fmul(C[r * 3 + 2], j25));
+  }
+  gq[3] = fadd(fadd(fmul(q0, CJ3[0]), fmul(q1, CJ3[1])), fmul(q2, CJ3[2]));
+  gq[4] = fadd(fadd(fmul(q0, CJ4[0]), fmul(q1, CJ4[1])), fmul(q2, CJ4[2]));
+  gq[5] = fadd(fadd(fmul(q0, CJ5[0]), fmul(q1, CJ5[1])), fmul(q2, CJ5[2]));
+  acc[0] += (double)score_inc;
+#pragma unroll
+  for (int k = 0; k < 6; k++) acc[1 + k] += (double)fmul(exv, gq[k]);
+  if (HESS) {
+    // All 36 entries of H exactly as ndt_omp writes them: its float32 expression is not symmetric to the last bit
+    // ((-d2 g_i) g_j vs (-d2 g_j) g_i, J_j^T C J_i vs J_i^T C J_j) and the Newton iteration is sensitive to it.  The 21 upper
+    // entries accumulate in float64 registers, the 15 strictly lower ones in a float64 shared-memory column per thread (43
+    // register accumulators would spill).  The term J_jj^T C J_ii is P[jj][ii] with
+    // P[a][b] = J[:,a] . CJ[:,b], CJ[r][b]: b<3 -> C[r][b]; b=3 -> CJ3[r]; b=4 -> CJ4[r]; b=5 -> CJ5[r]
+#define B2R_CJ(r, b) ((b) < 3 ? C[(r) * 3 + (b)] : ((b) == 3 ? CJ3[r] : ((b) == 4 ? CJ4[r] : CJ5[r])))
+    // second-derivative terms qC . v_ij  (i,j in 3..5); a=(0,ha1,ha2) b=(0,hb1,hb2) c=(0,hc1,hc2) d,e,f full
+    const float xa = fadd(fadd(fmul(gq[0], 0.f), fmul(gq[1], pd.ha1)), fmul(gq[2], pd.ha2));
+    const float xb = fadd(fadd(fmul(gq[0], 0.f), fmul(gq[1], pd.hb1)), fmul(gq[2], pd.hb2));
+    const float xc = fadd(fadd(fmul(gq[0], 0.f), fmul(gq[1], pd.hc1)), fmul(gq[2], pd.hc2));
+    const float xd = fadd(fadd(fmul(gq[0], pd.hd0), fmul(gq[1], pd.hd1)), fmul(gq[2], pd.hd2));
+    const float xe = fadd(fadd(fmul(gq[0], pd.he0), fmul(gq[1], pd.he1)), fmul(gq[2], pd.he2));
+    const float xf = fadd(fadd(fmul(gq[0], pd.hf0), fmul(gq[1], pd.hf1)), fmul(gq[2], pd.hf2));
+    const float XH[3][3] = {{xa, xb, xc}, {xb, xd, xe}, {xc, xe, xf}};
+    int hk = 7, lk = 0;
+#pragma unroll
+    for (int ii = 0; ii < 6; ii++) {
+#pragma unroll
+      for (int jj = 0; jj < 6; jj++) {
+        float u = fmul(fmul(-d2f, gq[ii]), gq[jj]);
+        const float xh = (ii >= 3 && jj >= 3) ? XH[ii - 3][jj - 3] : 0.f;
+        u = fadd(u, xh);
+        // P[jj][ii] = J[:,jj] . CJ[:,ii]
+        float pj;
+        if (jj < 3) pj = B2R_CJ(jj, ii);
+        else if (jj == 3) pj = fadd(fmul(j13, B2R_CJ(1, ii)), fmul(j23, B2R_CJ(2, ii)));
+        else if (jj == 4) pj = fadd(fadd(fmul(j04, B2R_CJ(0, ii)), fmul(j14, B2R_CJ(1, ii))), fmul(j24, B2R_CJ(2, ii)));
+        else pj = fadd(fadd(fmul(j05, B2R_CJ(0, ii)), fmul(j15, B2R_CJ(1, ii))), fmul(j25, B2R_CJ(2, ii)));
+        u = fadd(u, pj);
+        const double w = (double)fmul(exv, u);
+        if (jj >= ii) { acc[hk] += w; hk++; }                     // upper triangle + diagonal: registers
+        else { low[lk * kNdtRow] += w; lk++; }                    // strict lower triangle: this thread's shared-memory column
+      }
+    }
+#undef B2R_CJ
+  }
 }
 
 template <bool HESS>
@@ -557,6 +658,56 @@ template <bool HESS>
 __global__ void __launch_bounds__(kNdtThreads, 4) k_ndt_derivatives_batch(const NdtArgs* __restrict__ recs) { ndt_derivatives_body<HESS>(recs[blockIdx.y]); }
 
 
+// computeHessian's per-point setup, float64, of the original point: point_gradient_'s angular entries into J (the caller's, holding
+// the identity block) and the angular vectors a .. f of point_hessian_
+__device__ __forceinline__ void ndt_hess_point(const NdtArgs& A, float xf, float yf, float zf, double (&J)[3][6], double* va, double* vb, double* vc,
+                                               double* vd, double* ve, double* vf) {
+  const double x = (double)xf, y = (double)yf, z = (double)zf;
+#define B2R_DJ(r) (x * A.jang_d[r][0] + y * A.jang_d[r][1] + z * A.jang_d[r][2])
+#define B2R_DH(r) (x * A.hang_d[r][0] + y * A.hang_d[r][1] + z * A.hang_d[r][2])
+  J[1][3] = B2R_DJ(0); J[2][3] = B2R_DJ(1); J[0][4] = B2R_DJ(2); J[1][4] = B2R_DJ(3); J[2][4] = B2R_DJ(4);
+  J[0][5] = B2R_DJ(5); J[1][5] = B2R_DJ(6); J[2][5] = B2R_DJ(7);
+  va[0] = 0; va[1] = B2R_DH(0); va[2] = B2R_DH(1); vb[0] = 0; vb[1] = B2R_DH(2); vb[2] = B2R_DH(3); vc[0] = 0; vc[1] = B2R_DH(4); vc[2] = B2R_DH(5);
+  vd[0] = B2R_DH(6); vd[1] = B2R_DH(7); vd[2] = B2R_DH(8); ve[0] = B2R_DH(9); ve[1] = B2R_DH(10); ve[2] = B2R_DH(11);
+  vf[0] = B2R_DH(12); vf[1] = B2R_DH(13); vf[2] = B2R_DH(14);
+#undef B2R_DJ
+#undef B2R_DH
+}
+
+// updateHessian for one (point, voxel), float64 (oracle/ndt.cpp::hessian_only): all 36 entries into acc.  A term that fails the
+// range check adds nothing.  The KDTREE pass (ndt_kdtree.cuh) runs it with ndt_hess_point's setup; ndt_hessian_body keeps its own
+// inline copy of both: calling them there moved the register assignment of k_ndt_hessian[_batch] and made an NDT_OMP odometry with the
+// line search active about 7 % slower on an H100, with bit-identical results.
+__device__ __forceinline__ void ndt_hess_term(const NdtArgs& A, const NdtVoxel* L, float xt, float yt, float zt, const double (&J)[3][6], const double* va,
+                                              const double* vb, const double* vc, const double* vd, const double* ve, const double* vf, double* acc) {
+  const double q[3] = {(double)xt - L->mean[0], (double)yt - L->mean[1], (double)zt - L->mean[2]};
+  const double* C = L->icov;
+  double Cq[3];
+  for (int r = 0; r < 3; r++) Cq[r] = C[r * 3 + 0] * q[0] + C[r * 3 + 1] * q[1] + C[r * 3 + 2] * q[2];
+  double ex = A.d2 * exp(-A.d2 * (q[0] * Cq[0] + q[1] * Cq[1] + q[2] * Cq[2]) / 2);
+  if (ex > 1 || ex < 0 || ex != ex) return;
+  ex *= A.d1;
+  double CJ[3][6], qCJ[6];
+  for (int r = 0; r < 3; r++)
+    for (int k = 0; k < 6; k++) CJ[r][k] = C[r * 3 + 0] * J[0][k] + C[r * 3 + 1] * J[1][k] + C[r * 3 + 2] * J[2][k];
+  for (int k = 0; k < 6; k++) qCJ[k] = q[0] * CJ[0][k] + q[1] * CJ[1][k] + q[2] * CJ[2][k];
+#pragma unroll
+  for (int ii = 0; ii < 6; ii++)
+#pragma unroll
+    for (int jj = 0; jj < 6; jj++) {
+      double xh = 0;
+      if (ii >= 3 && jj >= 3) {
+        const int key = (ii - 3) * 3 + (jj - 3);
+        const double* v = (key == 0) ? va : (key == 1 || key == 3) ? vb : (key == 2 || key == 6) ? vc : (key == 4) ? vd : (key == 5 || key == 7) ? ve : vf;
+        double Cv[3];
+        for (int r = 0; r < 3; r++) Cv[r] = C[r * 3 + 0] * v[0] + C[r * 3 + 1] * v[1] + C[r * 3 + 2] * v[2];
+        xh = q[0] * Cv[0] + q[1] * Cv[1] + q[2] * Cv[2];
+      }
+      const double jcj = J[0][jj] * CJ[0][ii] + J[1][jj] * CJ[1][ii] + J[2][jj] * CJ[2][ii];
+      acc[ii * 6 + jj] += ex * (-A.d2 * qCJ[ii] * qCJ[jj] + xh + jcj);
+    }
+}
+
 // float64 Hessian-only pass (ndt_omp computeHessian/updateHessian); nrow = the source's 128-point blocks
 __device__ __forceinline__ void ndt_hessian_body(const NdtArgs& A, unsigned int nrow) {
   __shared__ double red[36 * 32];
@@ -637,6 +788,7 @@ __global__ void __launch_bounds__(kNdtThreads) k_ndt_hessian_batch(const NdtArgs
 
 }  // namespace b2r
 #include "ndt_pcl.cuh"
+#include "ndt_kdtree.cuh"
 namespace b2r {
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -699,7 +851,7 @@ inline int ndt_ensure_map(const b2r_config& cfg, Cloud& c, NdtWork& W, cudaStrea
     k_vox_gather<<<nb, 256, 0, st>>>(c.raw_view, c.stride_f, n, M.keys.p, B->vals_b.p, M.sorted.p);
     k_vox_finalize<<<(n + 127) / 128, 128, 0, st>>>(M.keys.p, M.sorted.p, M.vox.p, M.cells.p, M.table.p, M.mask, n);
   }
-  if (cfg.method == B2R_METHOD_NDT_PCL) {
+  if (ndt_radius_family(cfg.method)) {
     int rc2 = ndt_pcl_build(M, B, n, st);
     if (rc2) return rc2;
   }
@@ -1004,6 +1156,38 @@ inline int ndt_run_pass(const b2r_config& cfg, Cloud& src, Cloud& tgt, NdtWork& 
     int rc = wait_host_result(W.h_flag, A.seq, W.h_out.p, kNdtAcc, true, st);
     if (rc) return rc;
     ndt_read_pass(W.h_out.p, hess, false, out);
+    return B2R_OK;
+  }
+  if (cfg.method == B2R_METHOD_NDT_KDTREE) {
+    // NDT_OMP's KDTREE: the derivative passes are ndt_omp's float32 term over the radius neighbours, the Hessian-only pass its own
+    // float64 kernel over the same neighbours
+    NdtPclArgs P;
+    ndt_pcl_fill_args(cfg, tgt, A, P);
+    if (hessian_only) {
+      { TEL_BEGIN(W.tel, st);
+        k_ndt_kdtree_hessian<<<nb, kNdtThreads, 0, st>>>(P);
+        TEL_END(W.tel, KC_NDT_HESS, 1, st); }
+      if (W.tel) W.tel->d2h += 36 * sizeof(double);
+      B2R_CUDA(cudaGetLastError());
+      int rc = wait_host_result(W.h_flag, A.seq, W.h_out.p, 36, false, st);
+      if (rc) return rc;
+      ndt_read_pass(W.h_out.p, true, true, out);
+      return B2R_OK;
+    }
+    { TEL_BEGIN(W.tel, st);
+      const unsigned ng = std::min(nb, ndt_kdtree_resident_blocks(compute_hessian));
+      P.A.qbase = W.qnext;
+      W.qnext += (unsigned long long)nb + ng;
+      if (compute_hessian) k_ndt_kdtree_derivatives<true><<<ng, kNdtThreads, 0, st>>>(P);
+      else k_ndt_kdtree_derivatives<false><<<ng, kNdtThreads, 0, st>>>(P);
+      TEL_END(W.tel, KC_NDT_DERIV, 1, st);
+      if (cudaPeekAtLastError() != cudaSuccess) W.qnext = P.A.qbase;
+    }
+    if (W.tel) W.tel->d2h += kNdtAcc * sizeof(double) + 8;
+    B2R_CUDA(cudaGetLastError());
+    int rc = wait_host_result(W.h_flag, A.seq, W.h_out.p, kNdtAcc, true, st);
+    if (rc) return rc;
+    ndt_read_pass(W.h_out.p, compute_hessian, false, out);
     return B2R_OK;
   }
   if (hessian_only) {

@@ -288,9 +288,32 @@ __device__ __forceinline__ void ndt_chunk_finish(const NdtArgs& A, int chunk, in
   }
 }
 
+// The term rule of pcl::NormalDistributionsTransform (B2R_METHOD_NDT_PCL): computePointDerivatives of the original point promoted
+// to double, and ndt_pcl_term over the voxel's float64 record at the neighbour's sorted position s.
+struct NdtPclTermRule {
+  template <bool HESS>
+  struct Point { double jx[8], hx[15]; };
+  template <bool HESS>
+  static __device__ __forceinline__ void point(const NdtArgs& A, float x, float y, float z, Point<HESS>& pd) {
+    const double xd = x, yd = y, zd = z;
+#pragma unroll
+    for (int r = 0; r < 8; r++) pd.jx[r] = dadd(dadd(dmul(xd, A.jang_d[r][0]), dmul(yd, A.jang_d[r][1])), dmul(zd, A.jang_d[r][2]));
+    if (HESS) {
+#pragma unroll
+      for (int r = 0; r < 15; r++) pd.hx[r] = dadd(dadd(dmul(xd, A.hang_d[r][0]), dmul(yd, A.hang_d[r][1])), dmul(zd, A.hang_d[r][2]));
+    }
+  }
+  template <bool HESS>
+  static __device__ __forceinline__ void term(const NdtArgs& A, unsigned int s, float xt, float yt, float zt, const Point<HESS>& pd, double* acc,
+                                              double* low) {
+    ndt_pcl_term<HESS>(A, A.vox + s, (double)xt, (double)yt, (double)zt, pd.jx, pd.hx, acc, low);
+  }
+};
+
 // computeDerivatives over the Hilbert-sorted source: one thread per point, its radius neighbours in ascending (d2, leaf) order,
-// then the chunk row and the fixed two-level tree (ndt_chunk_finish), so the sums are bitwise reproducible.
-template <bool HESS>
+// then the chunk row and the fixed two-level tree (ndt_chunk_finish), so the sums are bitwise reproducible.  Rule: the per-point
+// derivatives and the per-(point, neighbour) term (NdtPclTermRule here; ndt_kdtree.cuh's NdtKdtreeTermRule for NDT_OMP's KDTREE).
+template <class Rule, bool HESS>
 __device__ __forceinline__ void ndt_pcl_derivatives_body(const NdtPclArgs& P) {
   const NdtArgs& A = P.A;
   __shared__ __align__(16) double s_tile[14 * kNdtRow];
@@ -319,22 +342,15 @@ __device__ __forceinline__ void ndt_pcl_derivatives_body(const NdtPclArgs& P) {
       const float yt = xform_row(A.Tf[4], A.Tf[5], A.Tf[6], A.Tf[7], x, y, z);
       const float zt = xform_row(A.Tf[8], A.Tf[9], A.Tf[10], A.Tf[11], x, y, z);
       if (finite3(xt, yt, zt)) {
-        // computePointDerivatives(x): the original point promoted to double
-        const double xd = x, yd = y, zd = z;
-        double jx[8], hx[15];
-#pragma unroll
-        for (int r = 0; r < 8; r++) jx[r] = dadd(dadd(dmul(xd, A.jang_d[r][0]), dmul(yd, A.jang_d[r][1])), dmul(zd, A.jang_d[r][2]));
-        if (HESS) {
-#pragma unroll
-          for (int r = 0; r < 15; r++) hx[r] = dadd(dadd(dmul(xd, A.hang_d[r][0]), dmul(yd, A.hang_d[r][1])), dmul(zd, A.hang_d[r][2]));
-        }
+        // computePointDerivatives(x): the original point
+        typename Rule::template Point<HESS> pd;
+        Rule::template point<HESS>(A, x, y, z, pd);
         unsigned long long buf[kPclNb];
         long long after = -1;
         for (;;) {
           const int total = pcl_collect(P, V, xt, yt, zt, after, buf);
           const int m = min(total, kPclNb);
-          for (int t = 0; t < m; t++)
-            ndt_pcl_term<HESS>(A, A.vox + (unsigned int)buf[t], (double)xt, (double)yt, (double)zt, jx, hx, acc, &s_low[0][threadIdx.x]);
+          for (int t = 0; t < m; t++) Rule::template term<HESS>(A, (unsigned int)buf[t], xt, yt, zt, pd, acc, &s_low[0][threadIdx.x]);
           npairs += (unsigned int)m;
           if (total <= kPclNb) break;
           after = (long long)buf[kPclNb - 1];
@@ -346,11 +362,15 @@ __device__ __forceinline__ void ndt_pcl_derivatives_body(const NdtPclArgs& P) {
 }
 
 template <bool HESS>
-__global__ void __launch_bounds__(kNdtThreads) k_ndt_pcl_derivatives(const __grid_constant__ NdtPclArgs P) { ndt_pcl_derivatives_body<HESS>(P); }
+__global__ void __launch_bounds__(kNdtThreads) k_ndt_pcl_derivatives(const __grid_constant__ NdtPclArgs P) {
+  ndt_pcl_derivatives_body<NdtPclTermRule, HESS>(P);
+}
 
 // many pairs: blockIdx.y = the pair's record, each pair with its own tickets, rows and counters (as k_ndt_derivatives_batch)
 template <bool HESS>
-__global__ void __launch_bounds__(kNdtThreads) k_ndt_pcl_derivatives_batch(const NdtPclArgs* __restrict__ recs) { ndt_pcl_derivatives_body<HESS>(recs[blockIdx.y]); }
+__global__ void __launch_bounds__(kNdtThreads) k_ndt_pcl_derivatives_batch(const NdtPclArgs* __restrict__ recs) {
+  ndt_pcl_derivatives_body<NdtPclTermRule, HESS>(recs[blockIdx.y]);
+}
 
 // b2r_ndt_neighbors_at: the radius neighbours of each point of the source in the caller's order (counts, then positions)
 __global__ void k_ndt_pcl_neighbors(const __grid_constant__ NdtPclArgs P, const float* __restrict__ raw, int stride_f, int n, unsigned int* counts,

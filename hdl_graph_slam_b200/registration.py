@@ -18,7 +18,7 @@ library; nothing here computes.
 import ctypes as C
 import numpy as np
 from . import _capi
-from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL, B2R_METHOD_VGICP_CUDA, B2R_METHOD_GICP_OMP  # noqa: F401
+from ._capi import Config, Result, Pair, OdometryParams, OdometryStatus, Stats, check, B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL, B2R_METHOD_VGICP_CUDA, B2R_METHOD_GICP_OMP, B2R_METHOD_NDT_KDTREE  # noqa: F401
 
 
 def _cloud(a):

@@ -73,6 +73,11 @@ extern "C" {
                                  = [R(x) R_guess | t_guess + t(x)] applied to the raw source point, where pcl GICP applies applyState(I, x)
                                  to guess * p.  With a translated guess the end pose differs from GICP's by about (R(x*) - I) t_guess.
                                  This pose rule is recalled, not read from the sources (DOUBT) */
+#define B2R_METHOD_NDT_KDTREE 9 /* pclomp::NormalDistributionsTransform with reg_nn_search_method = KDTREE (registrations.cpp:112-113,
+                                   opted into as B200_NDT_KDTREE): B2R_METHOD_NDT's voxel map, float32 term, float64 Hessian-only pass and
+                                   Newton / More-Thuente driver over B2R_METHOD_NDT_PCL's neighbourhood (every voxel centroid within
+                                   ndt_resolution, float32 d2 < (float)r^2, no nr_points check); reads ndt_resolution / ndt_step_size /
+                                   ndt_outlier_ratio / ndt_mt_interval_flag / ndt_fixed_iterations, not ndt_search_method */
 
 typedef struct b2r_handle b2r_handle;
 
@@ -117,8 +122,9 @@ int b2r_config_default(b2r_config* cfg, int method);
  * (B2R_METHOD_VGICP), "GICP"/"B200_GICP_PCL" and every other name that reaches the reference's GICP branch (contains "GICP" but not
  * "OMP") -> pcl GICP engine (B2R_METHOD_GICP_PCL), "B200_ICP" -> pcl ICP engine (B2R_METHOD_ICP_PCL; reg_use_reciprocal_correspondences
  * must be true / false / 1 / 0, else B2R_EINVAL), "B200_VGICP_CUDA" -> FastVGICPCuda engine (B2R_METHOD_VGICP_CUDA),
- * "B200_GICP_OMP" -> pclomp GICP engine (B2R_METHOD_GICP_OMP; the GICP branch's parameters and defaults).
- * ICP / GICP_OMP (and every other name containing GICP and OMP) / FAST_VGICP_CUDA and unknown names are not re-created: returns
+ * "B200_GICP_OMP" -> pclomp GICP engine (B2R_METHOD_GICP_OMP; the GICP branch's parameters and defaults), "B200_NDT_KDTREE" ->
+ * NDT_OMP's KDTREE search (B2R_METHOD_NDT_KDTREE; reg_resolution, reg_transformation_epsilon, reg_maximum_iterations).
+ * NDT_OMP / B200_NDT with reg_nn_search_method = KDTREE, ICP / GICP_OMP (and every other name containing GICP and OMP) / FAST_VGICP_CUDA and unknown names are not re-created: returns
  * B2R_EUNSUPPORTED so the caller keeps the reference's own branch.  (Built without USE_VGICP_CUDA the reference sends FAST_VGICP_CUDA to
  * its GICP branch; this factory refuses it all the same, so the caller decides.) */
 int b2r_select_registration_method(const char* const* keys, const char* const* values, int n_params, int device_id,
@@ -195,18 +201,19 @@ int b2r_get_covariances(b2r_handle* h, int which, double* out, size_t n);
 int b2r_gicp_linearize_at(b2r_handle* h, const double T[16], double* H, double* b, double* err);
 /* one compute_error at pose T with the correspondences of the last linearisation (GICP handle only: B2R_ESTATE on any other method) */
 int b2r_gicp_error_at(b2r_handle* h, const double T[16], double* err);
-/* NDT voxel table of the target (either NDT method): returns count through *n_voxels; arrays may be NULL.  keys ascending. */
+/* NDT voxel table of the target (any NDT method): returns count through *n_voxels; arrays may be NULL.  keys ascending. */
 int b2r_ndt_get_voxels(b2r_handle* h, size_t capacity, size_t* n_voxels, int64_t* keys, int32_t* npts, double* mean, double* icov,
                        int32_t min_b[3], int32_t div_b[3]);
 /* one computeDerivatives pass at p = (tx,ty,tz,rx,ry,rz): score, g[6], H[36] row-major, number of (point,cell) pairs
- * (B2R_METHOD_NDT_PCL: (point, radius neighbour) pairs) */
+ * (B2R_METHOD_NDT_PCL / _NDT_KDTREE: (point, radius neighbour) pairs) */
 int b2r_ndt_derivatives_at(b2r_handle* h, const double p[6], double* score, double* g, double* H, uint64_t* n_pairs);
-/* one float64 computeHessian pass at p (the pass the align runs after an active More-Thuente line search): H[36] row-major */
+/* one float64 computeHessian pass at p (the pass the align runs after an active More-Thuente line search): H[36] row-major
+ * (B2R_METHOD_NDT_KDTREE: over the radius neighbours) */
 int b2r_ndt_hessian_at(b2r_handle* h, const double p[6], double* H);
-/* B2R_METHOD_NDT_PCL: the searchable centroid cloud of the target (VoxelGridCovariance::filter(true)): the leaf key and float32
+/* B2R_METHOD_NDT_PCL / _NDT_KDTREE: the searchable centroid cloud of the target (VoxelGridCovariance::filter(true)): the leaf key and float32
  * centroid (xyz: 3 floats each) of every leaf with at least 6 points, keys ascending; *n_centroids = the count; arrays may be NULL */
 int b2r_ndt_get_centroids(b2r_handle* h, size_t capacity, size_t* n_centroids, int64_t* keys, float* xyz);
-/* B2R_METHOD_NDT_PCL: the radiusSearch(T(p) x, resolution) of every source point, in the caller's point order: counts[i] (n source
+/* B2R_METHOD_NDT_PCL / _NDT_KDTREE: the radiusSearch(T(p) x, resolution) of every source point, in the caller's point order: counts[i] (n source
  * entries, may be NULL) and one flat array of the neighbours' leaf keys, ascending within each point (CSR by counts; the first
  * `capacity` entries are written, keys may be NULL); *total = the number of (point, neighbour) pairs */
 int b2r_ndt_neighbors_at(b2r_handle* h, const double p[6], uint32_t* counts, size_t capacity, int64_t* keys, size_t* total);

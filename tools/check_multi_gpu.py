@@ -16,7 +16,7 @@ dev = torch.device("cuda", local)
 dist.init_process_group("nccl", device_id=dev)
 n_groups = int(sys.argv[1]) if len(sys.argv) > 1 else 6
 sensor = sys.argv[2] if len(sys.argv) > 2 else "vlp16_16k"
-method = sys.argv[3] if len(sys.argv) > 3 else "FAST_GICP"  # registration_method of both batches (e.g. FAST_VGICP, GICP, B200_VGICP_CUDA, B200_GICP_OMP)
+method = sys.argv[3] if len(sys.argv) > 3 else "FAST_GICP"  # registration_method of both batches (e.g. FAST_VGICP, GICP, B200_VGICP_CUDA, B200_GICP_OMP, B200_NDT_KDTREE)
 groups, guesses, group_first = batch.loop_workload(n_groups, sensor)
 n_pairs = group_first[-1]
 
