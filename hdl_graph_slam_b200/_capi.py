@@ -10,6 +10,7 @@ B2R_OK = 0
 B2R_EINVAL, B2R_ENODEVICE, B2R_ECUDA, B2R_ESTATE, B2R_EUNSUPPORTED, B2R_ENCCL = -1, -2, -3, -4, -5, -6
 B2R_METHOD_GICP, B2R_METHOD_NDT, B2R_METHOD_NDT_PCL, B2R_METHOD_VGICP, B2R_METHOD_GICP_PCL, B2R_METHOD_ICP_PCL, B2R_METHOD_VGICP_CUDA, B2R_METHOD_GICP_OMP, B2R_METHOD_NDT_KDTREE = 0, 1, 2, 3, 4, 5, 6, 8, 9  # 7 is unassigned
 B2R_DOWNSAMPLE_NONE, B2R_DOWNSAMPLE_VOXELGRID, B2R_DOWNSAMPLE_APPROX_VOXELGRID = 0, 1, 2
+FLOOR_REASONS = ("OK", "EMPTY_INPUT", "TOO_FEW_FILTERED", "NO_MODEL", "TOO_FEW_INLIERS", "NOT_VERTICAL")  # B2R_FLOOR_* codes 0..5
 
 
 class Config(C.Structure):
@@ -42,6 +43,17 @@ class PrefilterParams(C.Structure):
                 ("distance_far_thresh", C.c_double), ("downsample_method", C.c_int32), ("downsample_resolution", C.c_float),
                 ("outlier_removal_method", C.c_int32), ("statistical_mean_k", C.c_int32), ("statistical_stddev", C.c_double),
                 ("radius_radius", C.c_double), ("radius_min_neighbors", C.c_int32), ("reserved", C.c_int32)]
+
+
+class FloorParams(C.Structure):
+    _fields_ = [("tilt_deg", C.c_double), ("sensor_height", C.c_double), ("height_clip_range", C.c_double), ("floor_pts_thresh", C.c_int32),
+                ("use_normal_filtering", C.c_int32), ("floor_normal_thresh", C.c_double), ("normal_filter_thresh", C.c_double)]
+
+
+class FloorResult(C.Structure):
+    _fields_ = [("detected", C.c_int32), ("reason", C.c_int32), ("coeffs", C.c_float * 4), ("n_filtered", C.c_uint64), ("n_inliers", C.c_uint64),
+                ("ransac_iterations", C.c_int32), ("model_indices", C.c_int32 * 3), ("ransac_batches", C.c_int32), ("ransac_hypotheses", C.c_int32),
+                ("readbacks", C.c_int32), ("reserved", C.c_int32)]
 
 
 class KeyframeSnapshot(C.Structure):
@@ -135,6 +147,8 @@ SYMBOLS = [
     ("b2r_deskew", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_double, _F32P, _VP]),
     ("b2r_prefilter_params_default", C.c_int, [C.POINTER(PrefilterParams)]),
     ("b2r_prefilter", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_int, C.POINTER(PrefilterParams), _VP, C.POINTER(_VP), C.POINTER(_SZ)]),
+    ("b2r_floor_params_default", C.c_int, [C.POINTER(FloorParams)]),
+    ("b2r_floor_detect", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_int, C.POINTER(FloorParams), C.POINTER(FloorResult), _VP, _VP, C.POINTER(_VP), C.POINTER(_VP)]),
     ("b2r_ingest_pointcloud2", C.c_int, [_VP, _VP, _SZ, C.POINTER(PointLayout), C.POINTER(_VP)]),
     ("b2r_pcd_read_header", C.c_int, [C.c_char_p, C.POINTER(PointLayout), C.POINTER(_SZ), C.POINTER(_SZ)]),
     ("b2r_ingest_pcd", C.c_int, [_VP, C.c_char_p, C.POINTER(_VP), C.POINTER(_SZ)]),

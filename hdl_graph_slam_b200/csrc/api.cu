@@ -37,6 +37,7 @@
 #include "ingest.cuh"
 #include "loop_gate.cuh"
 #include "odometry_gate.cuh"
+#include "floor.cuh"
 
 #ifndef B2R_PREFETCH_KNN_BLOCKS_DEFAULT
 #define B2R_PREFETCH_KNN_BLOCKS_DEFAULT 0  // 0 = no cap on the prefetch stream's k-NN kernel
@@ -112,6 +113,7 @@ struct b2r_handle {
   DevBuf<char> icp_ws;              // B2R_METHOD_ICP_PCL: the pair's workspace (icp_pair_ws)
   DevBuf<IcpPairDev> icp_pair;      // B2R_METHOD_ICP_PCL: the pair's record
   PinnedBuf<IcpPairDev> icp_h;      // its host copy
+  FloorWork floor;                  // b2r_floor_detect's clouds and scratch (floor.cuh)
   Telemetry tel;
 };
 
@@ -1723,19 +1725,23 @@ static int pf_reserve(b2r_handle* h, size_t n, int sf) {
 }
 
 // records d_in[0..n) with flags (already on the device) -> d_out, *m = kept count
-static int pf_compact(b2r_handle* h, const float* d_in, size_t n, int sf, float* d_out, size_t* m) {
+// scratch: blocks (one int per 1024 records), total (device int), h_total (host-mapped int, its device alias h_total_d)
+static int compact_records(b2r_handle* h, const unsigned char* flags, int* blocks, int* total, int* h_total, int* h_total_d, const float* d_in,
+                           size_t n, int sf, float* d_out, size_t* m) {
   const unsigned nb = (unsigned)((n + kCompactBlock - 1) / kCompactBlock);
-  unsigned char* flags = h->pf_flags.p;
   { TEL_BEGIN(&h->tel, h->st);
-    k_compact_count<<<nb, kCompactBlock, 0, h->st>>>(flags, (int)n, h->pf_blocks.p);
-    k_compact_scan<<<1, 1024, 0, h->st>>>(h->pf_blocks.p, (int)nb, h->pf_total.p, h->pf_h_total.d);
-    k_compact_scatter<<<nb, kCompactBlock, 0, h->st>>>(d_in, sf, flags, (int)n, h->pf_blocks.p, d_out);
+    k_compact_count<<<nb, kCompactBlock, 0, h->st>>>(flags, (int)n, blocks);
+    k_compact_scan<<<1, 1024, 0, h->st>>>(blocks, (int)nb, total, h_total_d);
+    k_compact_scatter<<<nb, kCompactBlock, 0, h->st>>>(d_in, sf, flags, (int)n, blocks, d_out);
     TEL_END(&h->tel, KC_MISC, 3, h->st); }
   B2R_CUDA(cudaGetLastError());
   B2R_CUDA(cudaStreamSynchronize(h->st));
   h->tel.d2h += 4;
-  *m = (size_t)h->pf_h_total.p[0];
+  *m = (size_t)h_total[0];
   return B2R_OK;
+}
+static int pf_compact(b2r_handle* h, const float* d_in, size_t n, int sf, float* d_out, size_t* m) {
+  return compact_records(h, h->pf_flags.p, h->pf_blocks.p, h->pf_total.p, h->pf_h_total.p, h->pf_h_total.d, d_in, n, sf, d_out, m);
 }
 
 // PrefilteringNodelet::distance_filter (apps/prefiltering_nodelet.cpp:164-180)
@@ -1945,6 +1951,173 @@ extern "C" int b2r_prefilter(b2r_handle* h, const void* points, size_t n, size_t
   if (d_out) *d_out = cur;
   if (out_host) return pf_download(h, cur, m, stride_bytes, out_host);
   B2R_CUDA(cudaStreamSynchronize(h->st));
+  return B2R_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ floor detection (SURVEY.md §8f row 5)
+extern "C" int b2r_floor_params_default(b2r_floor_params* p) {
+  if (!p) return fail(B2R_EINVAL, "NULL argument");
+  std::memset(p, 0, sizeof(*p));
+  p->tilt_deg = 0.0;              // floor_detection_nodelet.cpp:57
+  p->sensor_height = 2.0;         // :58
+  p->height_clip_range = 1.0;     // :59
+  p->floor_pts_thresh = 512;      // :60
+  p->floor_normal_thresh = 10.0;  // :61
+  p->use_normal_filtering = 1;    // :62
+  p->normal_filter_thresh = 20.0; // :63
+  return B2R_OK;
+}
+
+// hypotheses per RANSAC batch (B2R_FLOOR_HYPOTHESES, read once per process); the answer does not depend on it.  16: the synthetic
+// scans of tools/floor_time.py stop after 2-6 hypotheses, and the one-thread draw of each further hypothesis costs more than a round
+// trip saves (BASELINE.md §3)
+static int floor_hypotheses() {
+  static const int b = [] { const char* e = getenv("B2R_FLOOR_HYPOTHESES"); const int v = e ? atoi(e) : 0; return v > 0 ? std::min(v, 65535) : 16; }();
+  return b;
+}
+
+// FloorDetectionNodelet::detect (apps/floor_detection_nodelet.cpp:110-180), see floor.cuh
+extern "C" int b2r_floor_detect(b2r_handle* h, const void* points, size_t n, size_t stride_bytes, int device_input, const b2r_floor_params* p,
+                                b2r_floor_result* r, void* filtered_host, void* inliers_host, const void** d_filtered, const void** d_inliers) {
+  if (!h || !p || !r || (n && !points)) return fail(B2R_EINVAL, "NULL argument");
+  if (stride_bytes < 12 || stride_bytes > 48 || (stride_bytes & 3)) return fail(B2R_EINVAL, "stride must be a multiple of 4 in [12, 48]");
+  if (n > (size_t)0x3fffffff) return fail(B2R_EINVAL, "too many points");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  std::memset(r, 0, sizeof(*r));
+  r->model_indices[0] = r->model_indices[1] = r->model_indices[2] = -1;
+  if (d_filtered) *d_filtered = nullptr;
+  if (d_inliers) *d_inliers = nullptr;
+  if (n == 0) { r->reason = B2R_FLOOR_EMPTY_INPUT; return B2R_OK; }  // cloud_callback returns on an empty cloud (:76-78)
+  FloorWork& F = h->floor;
+  const int sf = (int)(stride_bytes / 4);
+  const size_t nrec = n * sf + 8;
+  B2R_CUDA(F.tilted.reserve(nrec)); B2R_CUDA(F.band.reserve(nrec)); B2R_CUDA(F.kept.reserve(nrec)); B2R_CUDA(F.filtered.reserve(nrec));
+  B2R_CUDA(F.inliers.reserve(nrec)); B2R_CUDA(F.flags.reserve(n + 8)); B2R_CUDA(F.blocks.reserve((n + kCompactBlock - 1) / kCompactBlock + 8));
+  if (!F.total.p) {
+    B2R_CUDA(F.total.alloc(4)); B2R_CUDA(F.h_total.alloc(4)); B2R_CUDA(F.rng.alloc(1));
+  }
+  auto compact = [&](const float* in, size_t m, float* out, size_t* kept) {
+    r->readbacks++;  // the kept count
+    return compact_records(h, F.flags.p, F.blocks.p, F.total.p, F.h_total.p, F.h_total.d, in, m, sf, out, kept);
+  };
+  const float* in = (const float*)points;
+  if (!device_input) {
+    B2R_CUDA(F.in.reserve(nrec));
+    B2R_CUDA(cudaMemcpyAsync(F.in.p, points, n * stride_bytes, cudaMemcpyHostToDevice, h->st));
+    h->tel.h2d += n * stride_bytes;
+    in = F.in.p;
+  }
+  // 1-2. tilt and the height band (:112-119)
+  float T[16], Ti[16];
+  floor_tilt_matrix(p->tilt_deg, T);
+  mat4_inv_rigid_general(T, Ti);
+  FloorBandArg A;
+  for (int i = 0; i < 12; i++) A.Tf[i] = T[i];
+  A.d_hi = (float)(p->sensor_height + p->height_clip_range);
+  A.d_lo = (float)(p->sensor_height - p->height_clip_range);
+  const unsigned nb256 = (unsigned)((n + 255) / 256);
+  k_floor_band<<<nb256, 256, 0, h->st>>>(in, sf, (int)n, A, F.tilted.p, F.flags.p);
+  size_t m = 0;
+  int rc = compact(F.tilted.p, n, F.band.p, &m);
+  if (rc) return rc;
+  // 3. normal filter (:121-123)
+  const float* tilted_kept = F.band.p;
+  if (p->use_normal_filtering && m) {
+    Cloud& c = F.band_cloud;
+    c.n = m; c.stride_f = sf; c.invalidate();
+    c.raw_view = F.band.p;
+    rc = build_bvh(h, c, h->bc[0], h->st);
+    if (rc) return rc;
+    B2R_CUDA(cudaMemsetAsync(F.flags.p, 0, m, h->st));
+    const size_t padded = (size_t)c.nsup * 1024;
+    k_floor_normal_flags<<<(unsigned)(padded / kKnnThreads), kKnnThreads, 0, h->st>>>(c.bvh(), F.band.p, sf, std::cos(p->normal_filter_thresh * M_PI / 180.0),
+                                                                                      F.flags.p);
+    size_t mk = 0;
+    rc = compact(F.band.p, m, F.kept.p, &mk);
+    if (rc) return rc;
+    m = mk;
+    tilted_kept = F.kept.p;
+  }
+  // 4. back by tilt_matrix.inverse() (:125)
+  if (m) {
+    XfArgPF X;
+    for (int i = 0; i < 12; i++) X.Tf[i] = Ti[i];
+    k_transform_records<<<(unsigned)((m + 255) / 256), 256, 0, h->st>>>(tilted_kept, sf, (int)m, X, F.filtered.p);
+    B2R_CUDA(cudaGetLastError());
+  }
+  r->n_filtered = m;
+  if (d_filtered) *d_filtered = m ? F.filtered.p : nullptr;
+  if (filtered_host && m) {
+    B2R_CUDA(cudaMemcpyAsync(filtered_host, F.filtered.p, m * stride_bytes, cudaMemcpyDeviceToHost, h->st));
+    h->tel.d2h += m * stride_bytes;
+  }
+  // 5. too few points for RANSAC (:133): size_t against int, so a negative threshold rejects every cloud
+  if (m < static_cast<size_t>(p->floor_pts_thresh)) {
+    B2R_CUDA(cudaStreamSynchronize(h->st));
+    if (filtered_host && m) r->readbacks++;
+    r->reason = B2R_FLOOR_TOO_FEW_FILTERED;
+    return B2R_OK;
+  }
+  // 6. RANSAC (:138-144): B hypotheses drawn and counted on the device per batch, computeModel's loop replayed here
+  const int B = floor_hypotheses();
+  B2R_CUDA(F.hyp.reserve(B)); B2R_CUDA(F.h_hyp.reserve(B)); B2R_CUDA(F.counts.reserve(B)); B2R_CUDA(F.h_counts.reserve(B));
+  B2R_CUDA(F.shuffled.reserve(m + 8));
+  if (m) k_floor_iota<<<(unsigned)((m + 255) / 256), 256, 0, h->st>>>(F.shuffled.p, (int)m);
+  RansacReplay loop;
+  loop.init(m);
+  FloorHyp best;
+  best.ok = 0;
+  const unsigned gx = (unsigned)std::max<size_t>(1, std::min<size_t>((m + kRansacCountThreads - 1) / kRansacCountThreads, (size_t)std::max(1, h->n_sm * 8 / B)));
+  for (int batch = 0; loop.wants_more(); batch++) {
+    k_ransac_samples<<<1, 1, 0, h->st>>>(F.filtered.p, sf, (int)m, F.rng.p, F.shuffled.p, B, batch == 0, F.hyp.p);
+    B2R_CUDA(cudaMemsetAsync(F.counts.p, 0, B * sizeof(int), h->st));
+    if (m) k_ransac_count<<<dim3(gx, (unsigned)B), kRansacCountThreads, 0, h->st>>>(F.filtered.p, sf, (int)m, F.hyp.p, F.counts.p);
+    B2R_CUDA(cudaGetLastError());
+    B2R_CUDA(cudaMemcpyAsync(F.h_hyp.p, F.hyp.p, B * sizeof(FloorHyp), cudaMemcpyDeviceToHost, h->st));
+    B2R_CUDA(cudaMemcpyAsync(F.h_counts.p, F.counts.p, B * sizeof(int), cudaMemcpyDeviceToHost, h->st));
+    B2R_CUDA(cudaStreamSynchronize(h->st));
+    h->tel.d2h += B * (sizeof(FloorHyp) + sizeof(int));
+    r->ransac_batches++;
+    r->readbacks++;
+    r->ransac_hypotheses += B;
+    for (int j = 0; j < B; j++) {
+      const int prev_best = loop.best;
+      const bool more = loop.step(F.h_hyp.p[j], F.h_counts.p[j]);
+      if (loop.best != prev_best) best = F.h_hyp.p[j];  // also when this hypothesis was the last one the loop runs
+      if (!more) break;
+    }
+  }
+  // getSamples with fewer indices than the sample size sets iterations = INT_MAX - 1 before the loop breaks
+  r->ransac_iterations = m < 3 ? INT_MAX - 1 : loop.iterations;
+  if (!best.ok) {  // computeModel found no model: its inlier list is empty
+    r->reason = B2R_FLOOR_NO_MODEL;
+    return B2R_OK;
+  }
+  for (int i = 0; i < 3; i++) r->model_indices[i] = best.idx[i];
+  for (int i = 0; i < 4; i++) r->coeffs[i] = best.c[i];
+  k_ransac_inlier_flags<<<(unsigned)((m + 255) / 256), 256, 0, h->st>>>(F.filtered.p, sf, (int)m, best, F.flags.p);
+  size_t ni = 0;
+  rc = compact(F.filtered.p, m, F.inliers.p, &ni);
+  if (rc) return rc;
+  r->n_inliers = ni;
+  if (d_inliers) *d_inliers = ni ? F.inliers.p : nullptr;
+  if (inliers_host && ni) {
+    B2R_CUDA(cudaMemcpyAsync(inliers_host, F.inliers.p, ni * stride_bytes, cudaMemcpyDeviceToHost, h->st));
+    B2R_CUDA(cudaStreamSynchronize(h->st));
+    r->readbacks++;
+    h->tel.d2h += ni * stride_bytes;
+  }
+  // 7. inlier gate, verticality, upward normal (:147-166)
+  if (ni < static_cast<size_t>(p->floor_pts_thresh)) { r->reason = B2R_FLOOR_TOO_FEW_INLIERS; return B2R_OK; }
+  float ref[3];  // (tilt_matrix.inverse() * UnitZ).head<3>()
+  for (int i = 0; i < 3; i++) ref[i] = ((Ti[i * 4 + 0] * 0.0f + Ti[i * 4 + 1] * 0.0f) + Ti[i * 4 + 2] * 1.0f) + Ti[i * 4 + 3] * 0.0f;
+  // 3-float dots as Eigen's unrolled reduction of a fixed-size 3-vector associates them: a0 b0 + (a1 b1 + a2 b2)
+  const double dot = (double)(r->coeffs[0] * ref[0] + (r->coeffs[1] * ref[1] + r->coeffs[2] * ref[2]));
+  if (std::abs(dot) < std::cos(p->floor_normal_thresh * M_PI / 180.0)) { r->reason = B2R_FLOOR_NOT_VERTICAL; return B2R_OK; }
+  if (r->coeffs[0] * 0.0f + (r->coeffs[1] * 0.0f + r->coeffs[2] * 1.0f) < 0.0f)
+    for (int i = 0; i < 4; i++) r->coeffs[i] *= -1.0f;
+  r->detected = 1;
+  r->reason = B2R_FLOOR_OK;
   return B2R_OK;
 }
 

@@ -520,4 +520,76 @@ B2R_HD bool gicp_is_converged(const double* D, double rot_eps, double trans_eps)
   return (mr > mt ? mr : mt) < 1;
 }
 
+// ---- pcl::eigen33 (PCL 1.10 common/impl/eigen.hpp), the smallest-eigenvalue form NormalEstimation::solvePlaneParameters calls, in
+// float32 as upstream types it for a Matrix3f: scale by the largest |entry| (1 when it is <= FLT_MIN), computeRoots (closed form,
+// roots sorted ascending; the quadratic computeRoots2 when |c0| < FLT_EPSILON or the smallest root is <= 0), subtract the smallest
+// root from the diagonal, and return the row cross product with the largest squared norm over its square root.  Every float32
+// operation is correctly rounded and unfused in the order upstream writes it.  atan2f / cosf / sinf are evaluated as
+// (float)f((double)x) on host and device alike (glibc's float routines cannot be reproduced on the device).  Squared norms associate
+// x x + (y y + z z): Eigen 3.3 reduces a fixed-size 3-vector with redux_novec_unroller, which splits at Length / 2 = 1.  A, v row-major / xyz; a NaN entry gives a NaN vector.
+B2R_HD void pcl_compute_roots2(float b, float c, float* r) {
+  r[0] = 0.0f;
+  float d = (float)dsub((double)fmul(b, b), dmul(4.0, (double)c));  // Scalar(b * b - 4.0 * c): b * b in float32, the rest in float64
+  if (d < 0.0f) d = 0.0f;
+  const float sd = fsqrt_rn(d);
+  r[2] = fmul(0.5f, fadd(b, sd));
+  r[1] = fmul(0.5f, fsub(b, sd));
+}
+B2R_HD void pcl_compute_roots(const float* m, float* r) {
+  const float m00 = m[0], m01 = m[1], m02 = m[2], m11 = m[4], m12 = m[5], m22 = m[8];
+  const float c0 = fsub(fsub(fsub(fadd(fmul(fmul(m00, m11), m22), fmul(fmul(fmul(2.0f, m01), m02), m12)), fmul(fmul(m00, m12), m12)),
+                             fmul(fmul(m11, m02), m02)), fmul(fmul(m22, m01), m01));
+  const float c1 = fsub(fadd(fsub(fadd(fsub(fmul(m00, m11), fmul(m01, m01)), fmul(m00, m22)), fmul(m02, m02)), fmul(m11, m22)), fmul(m12, m12));
+  const float c2 = fadd(fadd(m00, m11), m22);
+  if (fabsf(c0) < 1.1920929e-07f) {  // Eigen::NumTraits<float>::epsilon()
+    pcl_compute_roots2(c2, c1, r);
+    return;
+  }
+  const float s_inv3 = (float)(1.0 / 3.0);
+  const float s_sqrt3 = fsqrt_rn(3.0f);
+  const float c2_over_3 = fmul(c2, s_inv3);
+  float a_over_3 = fmul(fsub(c1, fmul(c2, c2_over_3)), s_inv3);
+  if (a_over_3 > 0.0f) a_over_3 = 0.0f;
+  const float half_b = fmul(0.5f, fadd(c0, fmul(c2_over_3, fsub(fmul(fmul(2.0f, c2_over_3), c2_over_3), c1))));
+  float q = fadd(fmul(half_b, half_b), fmul(fmul(a_over_3, a_over_3), a_over_3));
+  if (q > 0.0f) q = 0.0f;
+  const float rho = fsqrt_rn(-a_over_3);
+  const float theta = fmul((float)atan2((double)fsqrt_rn(-q), (double)half_b), s_inv3);
+  const float cos_theta = (float)cos((double)theta), sin_theta = (float)sin((double)theta);
+  r[0] = fadd(c2_over_3, fmul(fmul(2.0f, rho), cos_theta));
+  r[1] = fsub(c2_over_3, fmul(rho, fadd(cos_theta, fmul(s_sqrt3, sin_theta))));
+  r[2] = fsub(c2_over_3, fmul(rho, fsub(cos_theta, fmul(s_sqrt3, sin_theta))));
+  float t;
+  if (r[0] >= r[1]) { t = r[0]; r[0] = r[1]; r[1] = t; }
+  if (r[1] >= r[2]) {
+    t = r[1]; r[1] = r[2]; r[2] = t;
+    if (r[0] >= r[1]) { t = r[0]; r[0] = r[1]; r[1] = t; }
+  }
+  if (r[0] <= 0.0f) pcl_compute_roots2(c2, c1, r);
+}
+B2R_HD void pcl_eigen33(const float* A, float* v) {
+  float scale = fabsf(A[0]);
+  for (int i = 1; i < 9; i++) scale = fabsf(A[i]) > scale ? fabsf(A[i]) : scale;
+  if (scale <= 1.17549435e-38f) scale = 1.0f;  // std::numeric_limits<float>::min()
+  float S[9];
+  for (int i = 0; i < 9; i++) S[i] = fdiv_rn(A[i], scale);
+  float r[3];
+  pcl_compute_roots(S, r);
+  S[0] = fsub(S[0], r[0]); S[4] = fsub(S[4], r[0]); S[8] = fsub(S[8], r[0]);
+  float V[3][3];  // row0 x row1, row0 x row2, row1 x row2
+  const int ra[3] = {0, 0, 1}, rb[3] = {1, 2, 2};
+  float len[3];
+  for (int k = 0; k < 3; k++) {
+    const float* a = S + ra[k] * 3;
+    const float* b = S + rb[k] * 3;
+    V[k][0] = fsub(fmul(a[1], b[2]), fmul(a[2], b[1]));
+    V[k][1] = fsub(fmul(a[2], b[0]), fmul(a[0], b[2]));
+    V[k][2] = fsub(fmul(a[0], b[1]), fmul(a[1], b[0]));
+    len[k] = fadd(fmul(V[k][0], V[k][0]), fadd(fmul(V[k][1], V[k][1]), fmul(V[k][2], V[k][2])));
+  }
+  const int k = (len[0] >= len[1] && len[0] >= len[2]) ? 0 : (len[1] >= len[0] && len[1] >= len[2]) ? 1 : 2;
+  const float sl = fsqrt_rn(len[k]);
+  v[0] = fdiv_rn(V[k][0], sl); v[1] = fdiv_rn(V[k][1], sl); v[2] = fdiv_rn(V[k][2], sl);
+}
+
 }  // namespace b2r

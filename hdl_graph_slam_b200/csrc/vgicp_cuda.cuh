@@ -89,25 +89,34 @@ __device__ __forceinline__ void vcuda_eigen3(const float* Ain, float* w, float* 
 #undef B2R_SWAPCOL
 }
 
+// The float32 raw-moment covariance of kk neighbours in list order, row-major into C: sums of p and of p_a p_b, / kk, then
+// cov = E[ab] - E[a]E[b].  Statement for statement this is also pcl::computeMeanAndCovarianceMatrix's dense path (PCL 1.10), the
+// moments of NormalEstimation in floor.cuh.
+template <class PtAt>
+__device__ __forceinline__ void raw_moment_cov_f32(int kk, PtAt pt_at, float* C) {
+  float m[3] = {0.f, 0.f, 0.f}, s[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // s: xx xy xz yy yz zz
+  for (int j = 0; j < kk; j++) {
+    const float3 p = pt_at(j);
+    m[0] = __fadd_rn(m[0], p.x); m[1] = __fadd_rn(m[1], p.y); m[2] = __fadd_rn(m[2], p.z);
+    s[0] = __fadd_rn(s[0], __fmul_rn(p.x, p.x)); s[1] = __fadd_rn(s[1], __fmul_rn(p.x, p.y)); s[2] = __fadd_rn(s[2], __fmul_rn(p.x, p.z));
+    s[3] = __fadd_rn(s[3], __fmul_rn(p.y, p.y)); s[4] = __fadd_rn(s[4], __fmul_rn(p.y, p.z)); s[5] = __fadd_rn(s[5], __fmul_rn(p.z, p.z));
+  }
+  const float kf = (float)kk;
+#pragma unroll
+  for (int a = 0; a < 3; a++) m[a] = __fdiv_rn(m[a], kf);
+  const float c00 = __fsub_rn(__fdiv_rn(s[0], kf), __fmul_rn(m[0], m[0])), c01 = __fsub_rn(__fdiv_rn(s[1], kf), __fmul_rn(m[0], m[1]));
+  const float c02 = __fsub_rn(__fdiv_rn(s[2], kf), __fmul_rn(m[0], m[2])), c11 = __fsub_rn(__fdiv_rn(s[3], kf), __fmul_rn(m[1], m[1]));
+  const float c12 = __fsub_rn(__fdiv_rn(s[4], kf), __fmul_rn(m[1], m[2])), c22 = __fsub_rn(__fdiv_rn(s[5], kf), __fmul_rn(m[2], m[2]));
+  C[0] = c00; C[1] = c01; C[2] = c02; C[3] = c01; C[4] = c11; C[5] = c12; C[6] = c02; C[7] = c12; C[8] = c22;
+}
+
 // FastVGICPCuda's covariance of one point over its kk neighbours (covariance_estimation + covariance_regularization PLANE).  Stores
 // xx, xy, xz, yy, yz, zz, each a float32 value widened.
 struct VcudaCov {
   template <class PtAt>
   __device__ __forceinline__ static void store(int kk, PtAt pt_at, double* __restrict__ o) {
-    float m[3] = {0.f, 0.f, 0.f}, s[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // s: xx xy xz yy yz zz
-    for (int j = 0; j < kk; j++) {
-      const float3 p = pt_at(j);
-      m[0] = __fadd_rn(m[0], p.x); m[1] = __fadd_rn(m[1], p.y); m[2] = __fadd_rn(m[2], p.z);
-      s[0] = __fadd_rn(s[0], __fmul_rn(p.x, p.x)); s[1] = __fadd_rn(s[1], __fmul_rn(p.x, p.y)); s[2] = __fadd_rn(s[2], __fmul_rn(p.x, p.z));
-      s[3] = __fadd_rn(s[3], __fmul_rn(p.y, p.y)); s[4] = __fadd_rn(s[4], __fmul_rn(p.y, p.z)); s[5] = __fadd_rn(s[5], __fmul_rn(p.z, p.z));
-    }
-    const float kf = (float)kk;
-#pragma unroll
-    for (int a = 0; a < 3; a++) m[a] = __fdiv_rn(m[a], kf);
-    const float c00 = __fsub_rn(__fdiv_rn(s[0], kf), __fmul_rn(m[0], m[0])), c01 = __fsub_rn(__fdiv_rn(s[1], kf), __fmul_rn(m[0], m[1]));
-    const float c02 = __fsub_rn(__fdiv_rn(s[2], kf), __fmul_rn(m[0], m[2])), c11 = __fsub_rn(__fdiv_rn(s[3], kf), __fmul_rn(m[1], m[1]));
-    const float c12 = __fsub_rn(__fdiv_rn(s[4], kf), __fmul_rn(m[1], m[2])), c22 = __fsub_rn(__fdiv_rn(s[5], kf), __fmul_rn(m[2], m[2]));
-    const float C[9] = {c00, c01, c02, c01, c11, c12, c02, c12, c22};
+    float C[9];
+    raw_moment_cov_f32(kk, pt_at, C);
     float w[3], V[9];
     vcuda_eigen3(C, w, V);
     // (1e-3 u0_a u0_b + u1_a u1_b) + u2_a u2_b for a <= b

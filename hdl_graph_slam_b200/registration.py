@@ -383,6 +383,34 @@ class Registration:
         check(self._lib.b2r_prefilter(self._h, C.c_void_p(ptr), n, stride_bytes, int(device), C.byref(p), None, C.byref(dptr), C.byref(m)))
         return None, dptr.value, m.value
 
+    def floor_detect(self, cloud=None, ptr=None, n=0, stride_bytes=32, device=False, want_host=True, **params):
+        """FloorDetectionNodelet::detect (b2r_floor_detect) on a host array `cloud`, or on `n` records at `ptr` (a device pointer when
+        device=True).  Returns a dict: detected, reason (name), coeffs, n_filtered, n_inliers, ransac_iterations, model_indices,
+        ransac_batches, ransac_hypotheses, readbacks, the filtered and inlier clouds as host arrays (when want_host) and their device pointers."""
+        if cloud is not None:
+            a, n, stride_bytes = _cloud(cloud)
+            ptr, device = a.ctypes.data, False
+        p = _capi.FloorParams()
+        check(self._lib.b2r_floor_params_default(C.byref(p)))
+        for k, v in params.items():
+            if not hasattr(p, k):
+                raise TypeError(f"unknown floor parameter {k}")
+            setattr(p, k, v)
+        r = _capi.FloorResult()
+        sf = stride_bytes // 4
+        filt = np.zeros((max(n, 1), sf), np.float32) if want_host else None
+        inl = np.zeros((max(n, 1), sf), np.float32) if want_host else None
+        df, di = C.c_void_p(), C.c_void_p()
+        check(self._lib.b2r_floor_detect(self._h, C.c_void_p(ptr), n, stride_bytes, int(device), C.byref(p), C.byref(r),
+                                         filt.ctypes.data_as(C.c_void_p) if want_host else None, inl.ctypes.data_as(C.c_void_p) if want_host else None,
+                                         C.byref(df), C.byref(di)))
+        return {"detected": bool(r.detected), "reason": _capi.FLOOR_REASONS[r.reason], "coeffs": np.array(r.coeffs[:], np.float32),
+                "n_filtered": r.n_filtered, "n_inliers": r.n_inliers, "ransac_iterations": r.ransac_iterations,
+                "model_indices": tuple(r.model_indices[:]), "ransac_batches": r.ransac_batches, "ransac_hypotheses": r.ransac_hypotheses,
+                "readbacks": r.readbacks,
+                "filtered": filt[: r.n_filtered] if want_host else None, "inliers": inl[: r.n_inliers] if want_host else None,
+                "d_filtered": df.value, "d_inliers": di.value}
+
     def ingestPointCloud2(self, blob, n_points, point_step, off_x=0, off_y=4, off_z=8, off_intensity=0xffffffff, intensity_datatype=7, is_bigendian=False):
         """sensor_msgs/PointCloud2 data[] -> device PointXYZI records (b2r_ingest_pointcloud2); returns the device pointer"""
         buf = np.frombuffer(blob, np.uint8) if not isinstance(blob, np.ndarray) else blob.view(np.uint8).reshape(-1)

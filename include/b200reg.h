@@ -322,6 +322,50 @@ int b2r_prefilter_params_default(b2r_prefilter_params* p);
 int b2r_prefilter(b2r_handle* h, const void* points, size_t n, size_t stride_bytes, int device_input, const b2r_prefilter_params* p,
                   void* out_host, const void** d_out, size_t* n_out);
 
+/* replaces FloorDetectionNodelet::detect (apps/floor_detection_nodelet.cpp:110-180) on the cloud of its cloud_callback (:72-103):
+ * tilt, the height band of two plane clips, the k = 10 normal filter, the back-transform, the size gate, PCL 1.10's seeded RANSAC
+ * plane fit (threshold 0.1) replayed hypothesis for hypothesis, the inlier gate, the verticality check and the upward flip.
+ * points: host records, or device records when device_input != 0 (e.g. b2r_prefilter's *d_out); stride 12..48 bytes, x y z first,
+ * every other field copied.  The call uses its own device buffers: no registration cloud, prefilter or voxel-grid output changes.
+ *   filtered_host  (capacity n records, may be NULL) <- /floor_detection/floor_filtered_points (:127-130)
+ *   inliers_host   (capacity n records, may be NULL) <- /floor_detection/floor_points (:168-177); filled whenever RANSAC found a
+ *                  model (result->n_inliers records), which the reference publishes only when the floor is detected
+ *   d_filtered / d_inliers (may be NULL) <- the same clouds in engine-owned device memory, valid until the next floor call on this
+ *                  handle; NULL when empty.
+ * Returns B2R_OK whenever the arguments are valid; result->detected says whether a FloorCoeffs message carries coefficients. */
+#define B2R_FLOOR_OK 0
+#define B2R_FLOOR_EMPTY_INPUT 1       /* no message at all (:76-78) */
+#define B2R_FLOOR_TOO_FEW_FILTERED 2  /* filtered->size() < floor_pts_thresh (:133; size_t against int: a negative threshold always) */
+#define B2R_FLOOR_NO_MODEL 3          /* RANSAC selected no sample (fewer than 3 points, or 1000 collinear draws) (:141) */
+#define B2R_FLOOR_TOO_FEW_INLIERS 4   /* inliers->indices.size() < floor_pts_thresh (:147) */
+#define B2R_FLOOR_NOT_VERTICAL 5      /* |coeffs.head<3>() . tilt^-1 UnitZ| < cos(floor_normal_thresh) (:152-161) */
+typedef struct b2r_floor_params {
+  double tilt_deg;                /* "tilt_deg" (0.0)                                     floor_detection_nodelet.cpp:57 */
+  double sensor_height;           /* "sensor_height" (2.0)                                :58                            */
+  double height_clip_range;       /* "height_clip_range" (1.0)                            :59                            */
+  int32_t floor_pts_thresh;       /* "floor_pts_thresh" (512)                             :60                            */
+  int32_t use_normal_filtering;   /* "use_normal_filtering" (true)                        :62                            */
+  double floor_normal_thresh;     /* "floor_normal_thresh" (10.0 deg)                     :61                            */
+  double normal_filter_thresh;    /* "normal_filter_thresh" (20.0 deg)                    :63                            */
+} b2r_floor_params;
+typedef struct b2r_floor_result {
+  int32_t detected;               /* detect() returned coefficients                                                     */
+  int32_t reason;                 /* B2R_FLOOR_*                                                                        */
+  float coeffs[4];                /* the published plane (normal up, :164-166); RANSAC's model when not detected        */
+  uint64_t n_filtered;            /* points after the band, normal filter and back-transform (:116-125)                */
+  uint64_t n_inliers;             /* selectWithinDistance of the best model (:143-144)                                  */
+  int32_t ransac_iterations;      /* RandomSampleConsensus::iterations_ at the end of computeModel (INT_MAX - 1 when the
+                                     filtered cloud has fewer than 3 points: getSamples sets it so)                      */
+  int32_t model_indices[3];       /* getModel(): the best sample's indices into the filtered cloud (-1: none)          */
+  int32_t ransac_batches;         /* device round trips of the RANSAC replay                                           */
+  int32_t ransac_hypotheses;      /* hypotheses drawn and counted on the device                                        */
+  int32_t readbacks;              /* times the call waited for data from the device: kept counts, RANSAC batches, copies */
+  int32_t reserved;
+} b2r_floor_result;
+int b2r_floor_params_default(b2r_floor_params* p);
+int b2r_floor_detect(b2r_handle* h, const void* points, size_t n, size_t stride_bytes, int device_input, const b2r_floor_params* p,
+                     b2r_floor_result* result, void* filtered_host, void* inliers_host, const void** d_filtered, const void** d_inliers);
+
 /* replaces MapCloudGenerator::generate(keyframes, resolution) (src/hdl_graph_slam/map_cloud_generator.cpp:13-51; called at
  * apps/hdl_graph_slam_nodelet.cpp:528,989): every keyframe cloud transformed by its optimised pose (float32), all concatenated;
  * resolution <= 0 returns that cloud (intensity kept), otherwise the centres of the occupied voxels of a
