@@ -51,9 +51,9 @@ struct b2r_batch {
   PinnedBuf<PairDev> h_pairs;       // staging
   PinnedBuf<PairReport> h_reports;  // staging
   PinnedBuf<VgicpMapDev> h_vmaps;   // staging (VGICP)
-  DevBuf<char> vfit_ws;             // VGICP getFitnessScore: per pair the reduction partials, counter and sums
-  DevBuf<VgicpFitItem> d_vfit;      // VGICP getFitnessScore: one record per pair of the call
-  PinnedBuf<VgicpFitItem> h_vfit;   // staging (filled once per call, so no chunk overwrites a record still being copied)
+  DevBuf<char> fit_ws;              // getFitnessScore after the rounds (batch_fitness): per pair the reduction partials, counter and sums
+  DevBuf<FitItem> d_fit;            // getFitnessScore after the rounds: one record per pair of the call
+  PinnedBuf<FitItem> h_fit;         // staging (filled once per call, so no chunk overwrites a record still being copied)
   MappedBuf<unsigned long long> h_word;  // [0..kLanes) = the lanes' words, [kLanes] = sum of the pairs' executed rounds
   size_t max_chunk = 1024;  // pairs in flight per launch sequence (~7.7 MB of workspace per 64k-point pair)
   int copies = 1;           // lanes per query of the batched 1-NN search
@@ -66,21 +66,21 @@ struct b2r_batch {
   DevBuf<KnnBatchItem> d_knn;       // descriptor list of one batched k-NN covariance launch
   PinnedBuf<KnnBatchItem> h_knn;    // staging
   PinnedBuf<b2r_result> h_gather;
+  // host-driven methods (NDT, pcl GICP, pcl ICP: batch_run_*_chunk).  A batch serves one method, so they share the workspace
+  DevBuf<char> method_ws;           // per pair in flight: ndt_pair_ws, gicp_pcl_pair_ws or icp_pair_ws
+  // the round channel of the NDT and pcl GICP rounds (batch_round_channel)
+  MappedBuf<double> h_msg;          // one result message per record of the round, then the round's flag (8 doubles)
+  DevBuf<unsigned int> d_round;     // messages of the current round (the last one publishes the flag and re-arms it)
+  unsigned long long msg_seq = 0;
   // NDT batch (batch_run_ndt_chunk)
-  DevBuf<char> ndt_ws;              // per pair in flight: chunk rows, group rows, counters, ticket counter; fitness partials
   DevBuf<NdtArgs> d_ndt_args;       // the round's pass records, grouped by pass kind
   PinnedBuf<NdtArgs> h_ndt_args;    // staging
   DevBuf<NdtPclArgs> d_pcl_args;    // the same records with the radius-search inputs (B2R_METHOD_NDT_PCL, _NDT_KDTREE)
   PinnedBuf<NdtPclArgs> h_pcl_args;
-  MappedBuf<double> h_ndt_msg;      // one result message per record of the round, then the round's flag (8 doubles)
-  DevBuf<unsigned int> d_ndt_round; // messages of the current round (the last one publishes the flag and re-arms it)
-  unsigned long long ndt_seq = 0;
-  // pcl GICP batch (batch_run_gicp_pcl_chunk): its rounds publish through h_ndt_msg / d_ndt_round / ndt_seq like the NDT rounds
-  DevBuf<char> gp_ws;               // per pair in flight: correspondences, M, reduction partials and counter; fitness partials
+  // pcl GICP batch (batch_run_gicp_pcl_chunk)
   DevBuf<GicpPclArgs> d_gp_args;    // the round's pass records: correspondence passes first, then cost passes
   PinnedBuf<GicpPclArgs> h_gp_args; // staging
   // pcl ICP batch (batch_run_icp_chunk)
-  DevBuf<char> icp_ws;              // per pair in flight: icp_pair_ws, then its k_fitness partials and counter
   DevBuf<IcpPairDev> d_icp;         // the pair records
   PinnedBuf<IcpPairDev> h_icp;      // their host copies
   // telemetry of the last b2r_batch_align
@@ -119,7 +119,7 @@ extern "C" int b2r_batch_create(const b2r_config* cfg, b2r_batch** out) {
   if (b->h_word.alloc(8) != cudaSuccess) return fail(B2R_ECUDA, "host allocation failed");
   for (int i = 0; i < 8; i++) b->h_word.p[i] = 0;
   if (b->fork_ev.create() != cudaSuccess) return fail(B2R_ECUDA, "event creation failed");
-  if (b->d_ndt_round.alloc(1) != cudaSuccess || cudaMemset(b->d_ndt_round.p, 0, sizeof(unsigned int)) != cudaSuccess)
+  if (b->d_round.alloc(1) != cudaSuccess || cudaMemset(b->d_round.p, 0, sizeof(unsigned int)) != cudaSuccess)
     return fail(B2R_ECUDA, "device allocation failed");
   for (int l = 0; l < b2r_batch::kLanes; l++) {
     b2r_batch::Lane& L = b->lane[l];
@@ -473,9 +473,9 @@ static int batch_vgicp_maps(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs)
   return B2R_OK;
 }
 
-// getFitnessScore at the final pose of every pair of the call (reports d_rep[0..m) on the device): one k_vgicp_fitness launch covers
+// getFitnessScore at the final pose of every pair of the call (reports d_rep[0..m) on the device): one k_fitness_batch launch covers
 // every pair with the kernel, grid and reduction of b2r_fitness, so each score is bitwise b2r_fitness's; no host round trip.
-static int batch_vgicp_fitness(b2r_batch* b, const b2r_pair* pairs, size_t m, double fit_max_range, PairReport* d_rep) {
+static int batch_fitness(b2r_batch* b, const b2r_pair* pairs, size_t m, double fit_max_range, PairReport* d_rep) {
   b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
   std::vector<size_t> live, off;
@@ -484,7 +484,7 @@ static int batch_vgicp_fitness(b2r_batch* b, const b2r_pair* pairs, size_t m, do
   for (size_t i = 0; i < m; i++) {
     const Cloud& s = *b->clouds[pairs[i].source];
     const Cloud& t = *b->clouds[pairs[i].target];
-    if (s.n == 0 || t.n == 0) continue;  // degenerate_report: DBL_MAX already
+    if (s.n == 0 || t.n == 0) continue;  // degenerate_report / method_report: DBL_MAX already
     const size_t nb = (size_t)s.nsup * 1024 / kLinThreads;
     live.push_back(i);
     off.push_back(ws);
@@ -492,17 +492,17 @@ static int batch_vgicp_fitness(b2r_batch* b, const b2r_pair* pairs, size_t m, do
     max_nb = std::max(max_nb, (unsigned)nb);
   }
   if (live.empty()) return B2R_OK;
-  B2R_CUDA(b->vfit_ws.reserve(ws + 256));
-  B2R_CUDA(b->d_vfit.reserve(live.size()));
-  if (b->h_vfit.cap < live.size()) B2R_CUDA(b->h_vfit.alloc(live.size() + live.size() / 4 + 16));
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->vfit_ws.p), 256));
+  B2R_CUDA(b->fit_ws.reserve(ws + 256));
+  B2R_CUDA(b->d_fit.reserve(live.size()));
+  if (b->h_fit.cap < live.size()) B2R_CUDA(b->h_fit.alloc(live.size() + live.size() / 4 + 16));
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->fit_ws.p), 256));
   B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));  // the reduction counters start at zero (and re-arm themselves)
   for (size_t k = 0; k < live.size(); k++) {
     const size_t i = live[k];
     const Cloud& s = *b->clouds[pairs[i].source];
     const Cloud& t = *b->clouds[pairs[i].target];
     const size_t nb = (size_t)s.nsup * 1024 / kLinThreads;
-    VgicpFitItem& it = b->h_vfit.p[k];
+    FitItem& it = b->h_fit.p[k];
     std::memset(&it, 0, sizeof(it));
     it.A.src = s.bvh(); it.A.tgt = t.bvh();
     it.A.max_range = fit_max_range; it.A.inlier_thresh_sq = 0.25f;
@@ -513,16 +513,16 @@ static int batch_vgicp_fitness(b2r_batch* b, const b2r_pair* pairs, size_t m, do
     it.rep = d_rep + i;
     it.nblk = (unsigned)nb;
   }
-  B2R_CUDA(cudaMemcpyAsync(b->d_vfit.p, b->h_vfit.p, live.size() * sizeof(VgicpFitItem), cudaMemcpyHostToDevice, st));
-  h->tel.h2d += live.size() * sizeof(VgicpFitItem);
+  B2R_CUDA(cudaMemcpyAsync(b->d_fit.p, b->h_fit.p, live.size() * sizeof(FitItem), cudaMemcpyHostToDevice, st));
+  h->tel.h2d += live.size() * sizeof(FitItem);
   for (size_t k0 = 0; k0 < live.size(); k0 += 65535) {  // grid.y limit
     const unsigned ny = (unsigned)std::min<size_t>(65535, live.size() - k0);
     TEL_BEGIN(&h->tel, st);
-    k_vgicp_fitness<<<dim3(max_nb, ny), kLinThreads, 0, st>>>(b->d_vfit.p + k0);
+    k_fitness_batch<<<dim3(max_nb, ny), kLinThreads, 0, st>>>(b->d_fit.p + k0);
     TEL_END(&h->tel, KC_FITNESS, 1, st);
     B2R_CUDA(cudaGetLastError());
   }
-  k_vgicp_fitness_store<<<(unsigned)((live.size() + 255) / 256), 256, 0, st>>>(b->d_vfit.p, (int)live.size());
+  k_fitness_batch_store<<<(unsigned)((live.size() + 255) / 256), 256, 0, st>>>(b->d_fit.p, (int)live.size());
   B2R_CUDA(cudaGetLastError());
   return B2R_OK;
 }
@@ -544,38 +544,33 @@ static int batch_ndt_maps(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, b
   return B2R_OK;
 }
 
-// getFitnessScore at each pair's final pose (T[i]: row-major, the first 12 floats are read): the kernel and reduction of b2r_fitness,
-// one launch per pair, one wait for all.  base + fit_off[i]: the pair's k_fitness partials, then its counter (zeroed); base + fit_out:
-// 3 doubles per pair.  fit[3 i ..] = sum d2, count, inliers.
-static int batch_fitness_at(b2r_batch* b, const b2r_pair* pairs, size_t m, const std::vector<const float*>& T, char* base,
-                            const std::vector<size_t>& fit_off, size_t fit_out, double fit_max_range, std::vector<double>& fit) {
-  b2r_handle* h = b->eng.get();
-  cudaStream_t st = h->st;
-  double* d_fit = reinterpret_cast<double*>(base + fit_out);
-  for (size_t i = 0; i < m; i++) {
-    Cloud& s = *b->clouds[pairs[i].source];
-    Cloud& t = *b->clouds[pairs[i].target];
-    if (s.n == 0 || t.n == 0) continue;
-    const size_t nb = (size_t)s.nsup * 1024 / kLinThreads;
-    FitArgs A;
-    A.src = s.bvh(); A.tgt = t.bvh();
-    for (int k = 0; k < 12; k++) A.Tf[k] = T[i][k];
-    A.max_range = fit_max_range; A.inlier_thresh_sq = 0.25f;
-    A.partials = reinterpret_cast<double*>(base + fit_off[i]);
-    A.counter = reinterpret_cast<unsigned int*>(base + fit_off[i] + align_up(nb * 3 * sizeof(double), 256));
-    A.out = d_fit + 3 * i;
-    TEL_BEGIN(&h->tel, st);
-    k_fitness<<<(unsigned)nb, kLinThreads, 0, st>>>(A);
-    TEL_END(&h->tel, KC_FITNESS, 1, st);
-    B2R_CUDA(cudaGetLastError());
-  }
-  B2R_CUDA(cudaMemcpyAsync(fit.data(), d_fit, m * 3 * sizeof(double), cudaMemcpyDeviceToHost, st));
-  B2R_CUDA(cudaStreamSynchronize(st));
-  h->tel.d2h += m * 3 * sizeof(double);
-  return B2R_OK;
+// The report of a pair of a host-driven method: T_row is the registration's pose (row-major), or nullptr for a pair that never
+// started, which reports the caller's guess exactly as given.  With want_fitness the score is DBL_MAX until batch_fitness, which
+// runs after the rounds, overwrites it for every pair with points on both sides.
+static void method_report(PairReport& R, const float* T_row, const float* guess_col, bool converged, int iterations, int rounds,
+                          bool want_fitness) {
+  std::memset(&R, 0, sizeof(R));
+  for (int r = 0; r < 4; r++)
+    for (int c = 0; c < 4; c++) R.r.T[c * 4 + r] = T_row ? T_row[r * 4 + c] : guess_col[c * 4 + r];
+  R.r.fitness = want_fitness ? DBL_MAX : NAN;
+  R.r.converged = converged ? 1 : 0;
+  R.r.iterations = iterations;
+  R.rounds = rounds;
 }
 
-constexpr int kNdtMsg = 48;  // doubles per result message: kNdtAcc sums (or 36 Hessian entries), pair count, checksum
+constexpr int kRoundMsg = 48;  // doubles per result message: kNdtAcc sums (or 36 Hessian entries, or kGicpPclSums), pair count, checksum
+
+// The round channel of the NDT and pcl GICP rounds, sized for m messages: the flag behind the last message (host and device address)
+static int batch_round_channel(b2r_batch* b, size_t m, unsigned long long** flag, unsigned long long** flag_dev) {
+  if (b->h_msg.cap < m * kRoundMsg + 8) {
+    B2R_CUDA(b->h_msg.alloc(m * kRoundMsg + 8));
+    std::memset(b->h_msg.p, 0, b->h_msg.cap * sizeof(double));
+  }
+  const size_t flag_at = b->h_msg.cap - 8;  // behind the last message the buffer holds
+  *flag = reinterpret_cast<unsigned long long*>(b->h_msg.p + flag_at);
+  *flag_dev = reinterpret_cast<unsigned long long*>(b->h_msg.d + flag_at);
+  return B2R_OK;
+}
 
 // per pair in flight: [chunks + 1][kNdtAcc] chunk rows (also the Hessian pass's [blocks][36]), [groups][kNdtAcc] group rows,
 // group counters, then counter / pair count / ticket counter — all zero at the start of a chunk of pairs
@@ -594,7 +589,7 @@ static NdtPairWs ndt_pair_ws(const Cloud& s) {
 // pairs[0..m) of an NDT batch -> rep[0..m) (host).  Every pair runs ndt_align's driver (NdtPairState); a round gathers the pass
 // each active pair asks for into at most three launches (derivatives with Hessian, without, float64 Hessian only), waits once for
 // the round's flag and hands every pair its result.  A pair reduces through its own rows and counters, exactly as alone.
-static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, double fit_max_range, PairReport* rep) {
+static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, PairReport* rep) {
   b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
   const b2r_config& cfg = h->cfg;
@@ -605,14 +600,12 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
   const bool radius = pcl || kd;
   auto kind_of_pass = [&](int k) { return (pcl && k == NDT_PASS_HESS) ? (int)NDT_PASS_DERIV_HESS : k; };
   std::vector<NdtPairState> S(m);
-  std::vector<size_t> active, off(m, 0), fit_off(m, 0);
+  std::vector<size_t> active, off(m, 0);
   size_t ws = 0;
   for (size_t i = 0; i < m; i++) {
     Cloud& s = *b->clouds[pairs[i].source];
     Cloud& t = *b->clouds[pairs[i].target];
     if (s.n == 0 || t.n == 0) continue;  // ndt_align: initCompute fails silently (identity, not converged, no iteration)
-    fit_off[i] = ws;
-    ws += align_up((size_t)s.nsup * 1024 / kLinThreads * 3 * sizeof(double), 256) + 256;  // k_fitness partials, then its counter
     int rc = ndt_sync_geom(*t.ndt, h->ndt_work, st);
     if (rc) return rc;
     if (t.ndt->h_geom.empty) continue;  // no finite target point: as above
@@ -621,21 +614,15 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
     off[i] = ws;
     ws += ndt_pair_ws(s).bytes;
   }
-  const size_t fit_out = ws;  // 3 doubles per pair: the fitness sums
-  ws += align_up(m * 3 * sizeof(double), 256);
-  B2R_CUDA(b->ndt_ws.reserve(ws + 256));
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->ndt_ws.p), 256));
+  B2R_CUDA(b->method_ws.reserve(ws + 256));
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->method_ws.p), 256));
   B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
   B2R_CUDA(b->d_ndt_args.reserve(m));
   B2R_CUDA(b->h_ndt_args.alloc(m));
   if (radius) { B2R_CUDA(b->d_pcl_args.reserve(m)); B2R_CUDA(b->h_pcl_args.alloc(m)); }
-  if (b->h_ndt_msg.cap < m * kNdtMsg + 8) {
-    B2R_CUDA(b->h_ndt_msg.alloc(m * kNdtMsg + 8));
-    std::memset(b->h_ndt_msg.p, 0, b->h_ndt_msg.cap * sizeof(double));
-  }
-  const size_t flag_at = b->h_ndt_msg.cap - 8;  // behind the last message the buffer holds
-  unsigned long long* flag = reinterpret_cast<unsigned long long*>(b->h_ndt_msg.p + flag_at);
-  unsigned long long* flag_dev = reinterpret_cast<unsigned long long*>(b->h_ndt_msg.d + flag_at);
+  unsigned long long *flag, *flag_dev;
+  int rc = batch_round_channel(b, m, &flag, &flag_dev);
+  if (rc) return rc;
   std::vector<unsigned long long> qnext(m, 0);
   std::vector<size_t> order;
   std::vector<int> kind_of;
@@ -658,7 +645,7 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
         G[k] = std::max(1u, std::min(max_nb[k], (unsigned)((4ull * res + cnt[k] - 1) / cnt[k])));
       }
     G[2] = max_nb[2];
-    const unsigned long long seq = ++b->ndt_seq;
+    const unsigned long long seq = ++b->msg_seq;
     for (size_t r = 0; r < order.size(); r++) {
       const size_t i = order[r];
       const int k = kind_of[r];
@@ -676,10 +663,10 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       A.queue = reinterpret_cast<unsigned long long*>(p + w.small + 24);
       A.qbase = qnext[i];
       if (k != NDT_PASS_HESS) qnext[i] += (unsigned long long)(s.nsup * 1024 / kNdtThreads) + G[k];  // chunks + one closing draw per block
-      A.out = b->h_ndt_msg.d + r * kNdtMsg;
+      A.out = b->h_msg.d + r * kRoundMsg;
       A.flag = flag_dev;
       A.seq = seq;
-      A.round = b->d_ndt_round.p;
+      A.round = b->d_round.p;
       A.round_n = (unsigned)order.size();
       if (radius) ndt_pcl_fill_args(cfg, t, A, b->h_pcl_args.p[r]);
     }
@@ -707,12 +694,12 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       B2R_CUDA(cudaGetLastError());
       r0 += cnt[k];
     }
-    h->tel.d2h += order.size() * kNdtMsg * sizeof(double);
+    h->tel.d2h += order.size() * kRoundMsg * sizeof(double);
     b->last_rounds++;
     for (size_t r = 0; r < order.size(); r++) {  // the first wait covers the round; the rest only check each message
       const int k = kind_of[r];
-      const double* msg = b->h_ndt_msg.p + r * kNdtMsg;
-      int rc = (k == NDT_PASS_HESS) ? wait_host_result(flag, seq, msg, 36, false, st) : wait_host_result(flag, seq, msg, kNdtAcc, true, st);
+      const double* msg = b->h_msg.p + r * kRoundMsg;
+      rc = (k == NDT_PASS_HESS) ? wait_host_result(flag, seq, msg, 36, false, st) : wait_host_result(flag, seq, msg, kNdtAcc, true, st);
       if (rc) return rc;
       NdtPass P;
       ndt_read_pass(msg, k != NDT_PASS_DERIV, k == NDT_PASS_HESS, &P);
@@ -723,24 +710,8 @@ static int batch_run_ndt_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
       if (S[i].next() != NDT_PASS_DONE) active[keep++] = i;
     active.resize(keep);
   }
-  std::vector<double> fit(m * 3, 0.0);
-  if (want_fitness) {
-    std::vector<const float*> T(m);
-    for (size_t i = 0; i < m; i++) T[i] = S[i].Tfinal;
-    int rc = batch_fitness_at(b, pairs, m, T, base, fit_off, fit_out, fit_max_range, fit);
-    if (rc) return rc;
-  }
-  for (size_t i = 0; i < m; i++) {
-    PairReport& R = rep[i];
-    std::memset(&R, 0, sizeof(R));
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) R.r.T[c * 4 + r] = S[i].Tfinal[r * 4 + c];
-    const double nr = fit[3 * i + 1];
-    R.r.fitness = !want_fitness ? NAN : (nr > 0 ? fit[3 * i] / nr : DBL_MAX);
-    R.r.converged = S[i].converged ? 1 : 0;
-    R.r.iterations = S[i].nr_iterations;
-    R.rounds = S[i].passes;
-  }
+  for (size_t i = 0; i < m; i++)  // a pair that never started reports NdtPairState's identity
+    method_report(rep[i], S[i].Tfinal, nullptr, S[i].converged, S[i].nr_iterations, S[i].passes, want_fitness);
   return B2R_OK;
 }
 
@@ -760,43 +731,34 @@ static GicpPclPairWs gicp_pcl_pair_ws(const Cloud& s) {
 // pairs[0..m) of a pcl GICP batch -> rep[0..m) (host).  Every pair runs the single handle's GicpPclPairState; a round gathers the
 // pass each active pair asks for into at most two launches (correspondence passes, cost passes; blockIdx.y = pair), waits once for
 // the round's flag and hands every pair its result.  A pair reduces through its own partials and counter, exactly as alone.
-static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, double fit_max_range, PairReport* rep) {
+static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, PairReport* rep) {
   b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
   const b2r_config& cfg = h->cfg;
   std::vector<GicpPclPairState> S(m);
   std::vector<char> started(m, 0);
-  std::vector<float> G(m * 16);
-  std::vector<size_t> active, off(m, 0), fit_off(m, 0);
+  std::vector<size_t> active, off(m, 0);
   size_t ws = 0;
   for (size_t i = 0; i < m; i++) {
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) G[i * 16 + r * 4 + c] = pairs[i].guess[c * 4 + r];
     Cloud& s = *b->clouds[pairs[i].source];
     Cloud& t = *b->clouds[pairs[i].target];
     if (s.n == 0 || t.n == 0) continue;  // initCompute fails: the guess, not converged, no iteration (as gicp_pcl_align)
-    fit_off[i] = ws;
-    ws += align_up((size_t)s.nsup * 1024 / kLinThreads * 3 * sizeof(double), 256) + 256;
-    S[i].start(cfg, &G[i * 16]);
+    float G[16];
+    colmajor_to_row_f(pairs[i].guess, G);
+    S[i].start(cfg, G);
     started[i] = 1;
     active.push_back(i);
     off[i] = ws;
     ws += gicp_pcl_pair_ws(s).bytes;
   }
-  const size_t fit_out = ws;
-  ws += align_up(m * 3 * sizeof(double), 256);
-  B2R_CUDA(b->gp_ws.reserve(ws + 256));
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->gp_ws.p), 256));
+  B2R_CUDA(b->method_ws.reserve(ws + 256));
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->method_ws.p), 256));
   B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
   B2R_CUDA(b->d_gp_args.reserve(m));
   if (b->h_gp_args.cap < m) B2R_CUDA(b->h_gp_args.alloc(m));
-  if (b->h_ndt_msg.cap < m * kNdtMsg + 8) {
-    B2R_CUDA(b->h_ndt_msg.alloc(m * kNdtMsg + 8));
-    std::memset(b->h_ndt_msg.p, 0, b->h_ndt_msg.cap * sizeof(double));
-  }
-  const size_t flag_at = b->h_ndt_msg.cap - 8;
-  unsigned long long* flag = reinterpret_cast<unsigned long long*>(b->h_ndt_msg.p + flag_at);
-  unsigned long long* flag_dev = reinterpret_cast<unsigned long long*>(b->h_ndt_msg.d + flag_at);
+  unsigned long long *flag, *flag_dev;
+  int rc = batch_round_channel(b, m, &flag, &flag_dev);
+  if (rc) return rc;
   std::vector<size_t> order;
   std::vector<int> kind_of;
   while (!active.empty()) {
@@ -809,7 +771,7 @@ static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t 
           order.push_back(i); kind_of.push_back(k); cnt[k]++;
           max_nb[k] = std::max(max_nb[k], (unsigned)((size_t)b->clouds[pairs[i].source]->nsup * 1024 / kGicpPclThreads));
         }
-    const unsigned long long seq = ++b->ndt_seq;
+    const unsigned long long seq = ++b->msg_seq;
     for (size_t r = 0; r < order.size(); r++) {
       const size_t i = order[r];
       Cloud& s = *b->clouds[pairs[i].source];
@@ -822,10 +784,10 @@ static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t 
       gicp_pcl_fill_args(cfg, s, t, S[i].guess(), S[i].T(), R, reinterpret_cast<int*>(p + w.corr), reinterpret_cast<double*>(p + w.M), A);
       A.partials = reinterpret_cast<double*>(p + w.partials);
       A.counter = reinterpret_cast<unsigned int*>(p + w.counter);
-      A.out = b->h_ndt_msg.d + r * kNdtMsg;
+      A.out = b->h_msg.d + r * kRoundMsg;
       A.flag = flag_dev;
       A.seq = seq;
-      A.round = b->d_ndt_round.p;
+      A.round = b->d_round.p;
       A.round_n = (unsigned)order.size();
       A.nrow = (unsigned)((size_t)s.nsup * 1024 / kGicpPclThreads);
     }
@@ -849,14 +811,14 @@ static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t 
     h->tel.d2h += order.size() * (kGicpPclSums + 2) * sizeof(double);
     b->last_rounds++;
     for (size_t r = 0; r < order.size(); r++) {  // the first wait covers the round; the rest only check each message
-      const double* msg = b->h_ndt_msg.p + r * kNdtMsg;
+      const double* msg = b->h_msg.p + r * kRoundMsg;
       GicpPclPairState& P = S[order[r]];
       if (kind_of[r] == 0) {
-        int rc = wait_host_result(flag, seq, msg, 1, false, st);
+        rc = wait_host_result(flag, seq, msg, 1, false, st);
         if (rc) return rc;
         P.consume_corr((uint64_t)msg[0]);
       } else {
-        int rc = wait_host_result(flag, seq, msg, kGicpPclSums, false, st);
+        rc = wait_host_result(flag, seq, msg, kGicpPclSums, false, st);
         if (rc) return rc;
         P.consume_cost(msg);
       }
@@ -866,51 +828,31 @@ static int batch_run_gicp_pcl_chunk(b2r_batch* b, const b2r_pair* pairs, size_t 
       if (S[i].next() != GicpPclPairState::DONE) active[keep++] = i;
     active.resize(keep);
   }
-  std::vector<const float*> T(m);
-  for (size_t i = 0; i < m; i++) T[i] = started[i] ? S[i].Tfinal : &G[i * 16];
-  std::vector<double> fit(m * 3, 0.0);
-  if (want_fitness) {
-    int rc = batch_fitness_at(b, pairs, m, T, base, fit_off, fit_out, fit_max_range, fit);
-    if (rc) return rc;
-  }
   for (size_t i = 0; i < m; i++) {
-    PairReport& R = rep[i];
-    std::memset(&R, 0, sizeof(R));
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) R.r.T[c * 4 + r] = T[i][r * 4 + c];
-    const double nr = fit[3 * i + 1];
-    R.r.fitness = !want_fitness ? NAN : (nr > 0 ? fit[3 * i] / nr : DBL_MAX);
-    R.r.converged = (started[i] && S[i].converged) ? 1 : 0;
-    R.r.iterations = started[i] ? S[i].nr_iterations : 0;
-    R.rounds = started[i] ? S[i].corr_passes + S[i].cost_passes : 0;
+    const GicpPclPairState& P = S[i];
+    if (started[i]) method_report(rep[i], P.Tfinal, nullptr, P.converged, P.nr_iterations, P.corr_passes + P.cost_passes, want_fitness);
+    else method_report(rep[i], nullptr, pairs[i].guess, false, 0, 0, want_fitness);
   }
   return B2R_OK;
 }
 
 // pairs[0..m) of a pcl ICP batch -> rep[0..m) (host).  Every pair runs the single handle's device loop; one launch per pass covers
 // every pair (blockIdx.y = pair), so a round is 2 launches (4 with the reciprocal check) whatever the number of pairs.
-static int batch_run_icp_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, double fit_max_range, PairReport* rep) {
+static int batch_run_icp_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bool want_fitness, PairReport* rep) {
   b2r_handle* h = b->eng.get();
   cudaStream_t st = h->st;
-  std::vector<size_t> active, off(m, 0), fit_off(m, 0);
-  std::vector<float> G(m * 16);
+  std::vector<size_t> active, off(m, 0);
   size_t ws = 0;
   for (size_t i = 0; i < m; i++) {
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) G[i * 16 + r * 4 + c] = pairs[i].guess[c * 4 + r];
     Cloud& s = *b->clouds[pairs[i].source];
     Cloud& t = *b->clouds[pairs[i].target];
     if (s.n == 0 || t.n == 0) continue;  // initCompute fails: the guess, not converged, no iteration (as icp_align)
-    fit_off[i] = ws;
-    ws += align_up((size_t)s.nsup * 1024 / kLinThreads * 3 * sizeof(double), 256) + 256;
     off[i] = ws;
     ws += icp_pair_ws(s).bytes;
     active.push_back(i);
   }
-  const size_t fit_out = ws;
-  ws += align_up(m * 3 * sizeof(double), 256);
-  B2R_CUDA(b->icp_ws.reserve(ws + 256));
-  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->icp_ws.p), 256));
+  B2R_CUDA(b->method_ws.reserve(ws + 256));
+  char* base = reinterpret_cast<char*>(align_up(reinterpret_cast<size_t>(b->method_ws.p), 256));
   B2R_CUDA(cudaMemsetAsync(base, 0, ws, st));
   const size_t na = active.size();
   if (na) {
@@ -927,26 +869,13 @@ static int batch_run_icp_chunk(b2r_batch* b, const b2r_pair* pairs, size_t m, bo
     if (rc) return rc;
     b->last_rounds += (unsigned long long)rounds;
   }
-  std::vector<const float*> T(m);
-  std::vector<int> slot(m, -1);
-  for (size_t k = 0; k < na; k++) slot[active[k]] = (int)k;
-  for (size_t i = 0; i < m; i++) T[i] = slot[i] >= 0 ? b->h_icp.p[slot[i]].T : &G[i * 16];
-  std::vector<double> fit(m * 3, 0.0);
-  if (want_fitness) {
-    int rc = batch_fitness_at(b, pairs, m, T, base, fit_off, fit_out, fit_max_range, fit);
-    if (rc) return rc;
-  }
-  for (size_t i = 0; i < m; i++) {
-    PairReport& R = rep[i];
-    std::memset(&R, 0, sizeof(R));
-    for (int r = 0; r < 4; r++)
-      for (int c = 0; c < 4; c++) R.r.T[c * 4 + r] = T[i][r * 4 + c];
-    const double nr = fit[3 * i + 1];
-    R.r.fitness = !want_fitness ? NAN : (nr > 0 ? fit[3 * i] / nr : DBL_MAX);
-    const IcpPairDev* P = slot[i] >= 0 ? &b->h_icp.p[slot[i]] : nullptr;
-    R.r.converged = (P && P->converged) ? 1 : 0;
-    R.r.iterations = P ? P->iterations : 0;
-    R.rounds = P ? P->rounds : 0;
+  for (size_t i = 0, k = 0; i < m; i++) {  // active[k]: ascending
+    if (k < na && active[k] == i) {
+      const IcpPairDev& P = b->h_icp.p[k++];
+      method_report(rep[i], P.T, nullptr, P.converged != 0, P.iterations, P.rounds, want_fitness);
+    } else {
+      method_report(rep[i], nullptr, pairs[i].guess, false, 0, 0, want_fitness);
+    }
   }
   return B2R_OK;
 }
@@ -983,7 +912,10 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   if (ndt) rc = batch_ndt_maps(b, pairs, n_pairs, fit_only);
   if (rc) return rc;
   const bool vgicp = vgicp_family(h->cfg.method) && !fit_only;
-  const bool gpcl = gicp_pcl_family(h->cfg.method) && !fit_only;  // host-driven rounds, like NDT
+  const bool gpcl = gicp_pcl_family(h->cfg.method);
+  // NDT, pcl GICP and ICP aligns run their rounds from the host and leave their reports in h_reports; a stand-alone fitness
+  // evaluation is the GICP engine's search on every method
+  const bool host_driven = !fit_only && (ndt || gpcl || icp);
   if (vgicp) rc = batch_vgicp_maps(b, pairs, n_pairs);
   if (rc) return rc;
   const auto t_b = std::chrono::steady_clock::now();
@@ -991,22 +923,21 @@ static int batch_run(b2r_batch* b, const b2r_pair* pairs, size_t n_pairs, bool w
   rc = batch_host_staging(b, std::max(chunk, n_pairs));
   if (rc) return rc;
   B2R_CUDA(b->d_reports.reserve(n_pairs + 1));
-  // a VGICP round carries no fitness sums: its scores come from batch_vgicp_fitness after the rounds
+  // a VGICP round carries no fitness sums: its scores come from batch_fitness after the rounds
   const LmCfg cfg = make_lm_cfg(h->cfg, want_fitness && !vgicp, fit_max_range);
   b->last_rounds = b->last_pair_rounds = 0;
   for (size_t c0 = 0; c0 < n_pairs; c0 += chunk) {
     const size_t m = std::min(chunk, n_pairs - c0);
-    // an NDT align runs its own rounds; a stand-alone fitness evaluation is the same search on either engine
-    if (ndt && !fit_only) rc = batch_run_ndt_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
-    else if (gpcl) rc = batch_run_gicp_pcl_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
-    else if (icp && !fit_only) rc = batch_run_icp_chunk(b, pairs + c0, m, want_fitness, fit_max_range, b->h_reports.p + c0);
-    else rc = batch_run_chunk(b, pairs + c0, m, cfg, b->d_reports.p + c0, fit_only);
+    if (!host_driven) rc = batch_run_chunk(b, pairs + c0, m, cfg, b->d_reports.p + c0, fit_only);
+    else if (ndt) rc = batch_run_ndt_chunk(b, pairs + c0, m, want_fitness, b->h_reports.p + c0);
+    else if (gpcl) rc = batch_run_gicp_pcl_chunk(b, pairs + c0, m, want_fitness, b->h_reports.p + c0);
+    else rc = batch_run_icp_chunk(b, pairs + c0, m, want_fitness, b->h_reports.p + c0);
     if (rc) return rc;
   }
-  if (vgicp && want_fitness) rc = batch_vgicp_fitness(b, pairs, n_pairs, fit_max_range, b->d_reports.p);
-  if (rc) return rc;
-  if ((ndt && !fit_only) || gpcl || (icp && !fit_only))  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
+  if (host_driven)  // the reports go where the GICP engine leaves them: b2r_batch_loop_detect packs and gathers them on the device
     B2R_CUDA(cudaMemcpyAsync(b->d_reports.p, b->h_reports.p, n_pairs * sizeof(PairReport), cudaMemcpyHostToDevice, h->st));
+  if (want_fitness && (vgicp || host_driven)) rc = batch_fitness(b, pairs, n_pairs, fit_max_range, b->d_reports.p);
+  if (rc) return rc;
   if (dbg) {
     const auto t_c = std::chrono::steady_clock::now();
     fprintf(stderr, "[b2r rank %d] batch_run: build enqueue %.3f ms, rounds (host follows the device) %.3f ms, %llu rounds\n", b->rank,

@@ -3,12 +3,14 @@
 // k_fitness      <- pcl::Registration::getFitnessScore(max_range) (called at apps/scan_matching_odometry_nodelet.cpp:307,
 //                   include/hdl_graph_slam/loop_detector.hpp:146; in-tree twin src/hdl_graph_slam/information_matrix_calculator.cpp:49-80)
 //                   fused with the inlier loop of apps/scan_matching_odometry_nodelet.cpp:309-320
+// k_fitness_batch <- the same score for every pair of a batch call, in one launch (loop_detector.hpp:146)
 // k_nearest      <- getSearchMethodTarget()->nearestKSearch(pt, 1, ...) (apps/scan_matching_odometry_nodelet.cpp:316)
 // k_transform    <- the `aligned` cloud written by align() (pcl::transformPointCloud with final_transformation_)
 #pragma once
 #include "common.cuh"
 #include "bvh.cuh"
 #include "gicp.cuh"
+#include "pair_engine.cuh"  // PairReport
 
 namespace b2r {
 
@@ -23,10 +25,11 @@ struct FitArgs {
   unsigned int* counter;
 };
 
-__global__ void __launch_bounds__(kLinThreads, 4) k_fitness(const __grid_constant__ FitArgs A) {
-  __shared__ double red[3 * 32];
+// one block's share of a fitness launch: its kLinThreads source points at the pose Tf (row-major 3x4), each point's nearest target
+// point, and the block's sums (sum d2, count, inliers) reduced into acc
+__device__ __forceinline__ void fitness_block(const FitArgs& A, const float* Tf, double* acc, double* red) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  double acc[3] = {0.0, 0.0, 0.0};
+  acc[0] = acc[1] = acc[2] = 0.0;
   float4 p = make_float4(0.f, 0.f, 0.f, bits_idx(kPadIdx));
   if (s < A.src.nleaf * kLeaf) p = A.src.sp[s];
   float qx = 0.f, qy = 0.f, qz = 0.f;
@@ -34,9 +37,9 @@ __global__ void __launch_bounds__(kLinThreads, 4) k_fitness(const __grid_constan
   v.reset(INFINITY);
   bool active = false;
   if (idx_bits(p.w) != kPadIdx) {
-    qx = xform_row(A.Tf[0], A.Tf[1], A.Tf[2], A.Tf[3], p.x, p.y, p.z);
-    qy = xform_row(A.Tf[4], A.Tf[5], A.Tf[6], A.Tf[7], p.x, p.y, p.z);
-    qz = xform_row(A.Tf[8], A.Tf[9], A.Tf[10], A.Tf[11], p.x, p.y, p.z);
+    qx = xform_row(Tf[0], Tf[1], Tf[2], Tf[3], p.x, p.y, p.z);
+    qy = xform_row(Tf[4], Tf[5], Tf[6], Tf[7], p.x, p.y, p.z);
+    qz = xform_row(Tf[8], Tf[9], Tf[10], Tf[11], p.x, p.y, p.z);
     active = finite3(qx, qy, qz);
   }
   bvh_group_search(A.tgt, qx, qy, qz, active, v, -1);
@@ -45,7 +48,45 @@ __global__ void __launch_bounds__(kLinThreads, 4) k_fitness(const __grid_constan
     if (v.best_d2() < A.inlier_thresh_sq) acc[2] = 1.0;
   }
   block_reduce<3>(acc, red);
+}
+
+__global__ void __launch_bounds__(kLinThreads, 4) k_fitness(const __grid_constant__ FitArgs A) {
+  __shared__ double red[3 * 32];
+  double acc[3];
+  fitness_block(A, A.Tf, acc, red);
   finish_partials<3>(acc, A.partials, A.out, A.counter);
+}
+
+// getFitnessScore of many pairs at their final poses in ONE launch (blockIdx.y = pair): per pair exactly k_fitness's work, grid
+// (nblk blocks of kLinThreads) and fixed-order reduction, so every score is bitwise b2r_fitness's.  The pose is read from the pair's
+// report on the device (the float T the single handle stores as its final transformation); k_fitness_batch_store writes the score back.
+struct FitItem {
+  FitArgs A;                 // Tf unused: the pose comes from `rep`
+  PairReport* rep;
+  unsigned int nblk;         // = k_fitness's gridDim.x for this source
+  unsigned int pad;
+};
+__global__ void __launch_bounds__(kLinThreads, 4) k_fitness_batch(const FitItem* __restrict__ items) {
+  __shared__ double red[3 * 32];
+  const FitItem& it = items[blockIdx.y];
+  const unsigned int nblk = it.nblk;
+  if (blockIdx.x >= nblk) return;  // before the reduction's block count: only the pair's own nblk blocks take part
+  float Tf[12];
+#pragma unroll
+  for (int r = 0; r < 3; r++)
+#pragma unroll
+    for (int c = 0; c < 4; c++) Tf[r * 4 + c] = it.rep->r.T[c * 4 + r];
+  double acc[3];
+  fitness_block(it.A, Tf, acc, red);
+  finish_partials<3>(acc, it.A.partials, it.A.out, it.A.counter, nullptr, 0, nullptr, nblk);
+}
+
+// score = sum / count, DBL_MAX without a neighbour in range (as b2r_fitness computes it on the host, one IEEE division)
+__global__ void k_fitness_batch_store(const FitItem* __restrict__ items, int n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const double* o = items[i].A.out;
+  items[i].rep->r.fitness = o[1] > 0.0 ? o[0] / o[1] : DBL_MAX;
 }
 
 // queries in caller order (no spatial coherence guaranteed: still exact, only less efficient)

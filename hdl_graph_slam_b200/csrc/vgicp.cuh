@@ -360,56 +360,6 @@ __global__ void __launch_bounds__(kAccThreads, B2R_ACC_MINBLOCKS) k_vgicp_round(
   }
 }
 
-// getFitnessScore of many VGICP pairs at their final poses in ONE launch (blockIdx.y = pair): per pair exactly k_fitness's work, grid
-// (nblk blocks of kLinThreads) and fixed-order reduction, so every score is bitwise b2r_fitness's.  The pose is read from the pair's
-// report on the device (the float T the single handle stores as its final transformation); k_vgicp_fitness_store writes the score back.
-struct VgicpFitItem {
-  FitArgs A;                 // Tf unused: the pose comes from `rep`
-  PairReport* rep;
-  unsigned int nblk;         // = k_fitness's gridDim.x for this source
-  unsigned int pad;
-};
-__global__ void __launch_bounds__(kLinThreads, 4) k_vgicp_fitness(const VgicpFitItem* __restrict__ items) {
-  __shared__ double red[3 * 32];
-  const VgicpFitItem& it = items[blockIdx.y];
-  const unsigned int nblk = it.nblk;
-  if (blockIdx.x >= nblk) return;  // before the reduction's block count: only the pair's own nblk blocks take part
-  const FitArgs& A = it.A;
-  float Tf[12];
-#pragma unroll
-  for (int r = 0; r < 3; r++)
-#pragma unroll
-    for (int c = 0; c < 4; c++) Tf[r * 4 + c] = it.rep->r.T[c * 4 + r];
-  const int s = blockIdx.x * blockDim.x + threadIdx.x;
-  double acc[3] = {0.0, 0.0, 0.0};
-  float4 p = make_float4(0.f, 0.f, 0.f, bits_idx(kPadIdx));
-  if (s < A.src.nleaf * kLeaf) p = A.src.sp[s];
-  float qx = 0.f, qy = 0.f, qz = 0.f;
-  Nn1 v;
-  v.reset(INFINITY);
-  bool active = false;
-  if (idx_bits(p.w) != kPadIdx) {
-    qx = xform_row(Tf[0], Tf[1], Tf[2], Tf[3], p.x, p.y, p.z);
-    qy = xform_row(Tf[4], Tf[5], Tf[6], Tf[7], p.x, p.y, p.z);
-    qz = xform_row(Tf[8], Tf[9], Tf[10], Tf[11], p.x, p.y, p.z);
-    active = finite3(qx, qy, qz);
-  }
-  bvh_group_search(A.tgt, qx, qy, qz, active, v, -1);
-  if (active && v.best_pos >= 0) {
-    if ((double)v.best_d2() <= A.max_range) { acc[0] = (double)v.best_d2(); acc[1] = 1.0; }
-    if (v.best_d2() < A.inlier_thresh_sq) acc[2] = 1.0;
-  }
-  block_reduce<3>(acc, red);
-  finish_partials<3>(acc, A.partials, A.out, A.counter, nullptr, 0, nullptr, nblk);
-}
-
-// score = sum / count, DBL_MAX without a neighbour in range (as b2r_fitness computes it on the host, one IEEE division)
-__global__ void k_vgicp_fitness_store(const VgicpFitItem* __restrict__ items, int n) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const double* o = items[i].A.out;
-  items[i].rep->r.fitness = o[1] > 0.0 ? o[0] / o[1] : DBL_MAX;
-}
 #endif  // __CUDACC__
 
 }  // namespace b2r
