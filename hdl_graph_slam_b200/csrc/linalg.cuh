@@ -2,6 +2,7 @@
 // Eigen is what the upstream CPU packages use, it does not exist here, and nothing of it is needed on a GPU.
 #pragma once
 #include "common.cuh"
+#include "atan2_rn.cuh"
 
 namespace b2r {
 
@@ -525,7 +526,8 @@ B2R_HD bool gicp_is_converged(const double* D, double rot_eps, double trans_eps)
 // roots sorted ascending; the quadratic computeRoots2 when |c0| < FLT_EPSILON or the smallest root is <= 0), subtract the smallest
 // root from the diagonal, and return the row cross product with the largest squared norm over its square root.  Every float32
 // operation is correctly rounded and unfused in the order upstream writes it.  atan2f / cosf / sinf are evaluated as
-// (float)f((double)x) on host and device alike (glibc's float routines cannot be reproduced on the device).  Squared norms associate
+// (float)f((double)x) on host and device alike (glibc's float routines cannot be reproduced on the device); atan2 is atan2_rn.cuh's,
+// because CUDA's and glibc's float64 atan2 round some float32 results differently (cos and sin agree on every |t| <= 1.1).  Squared norms associate
 // x x + (y y + z z): Eigen 3.3 reduces a fixed-size 3-vector with redux_novec_unroller, which splits at Length / 2 = 1.  A, v row-major / xyz; a NaN entry gives a NaN vector.
 B2R_HD void pcl_compute_roots2(float b, float c, float* r) {
   r[0] = 0.0f;
@@ -554,7 +556,7 @@ B2R_HD void pcl_compute_roots(const float* m, float* r) {
   float q = fadd(fmul(half_b, half_b), fmul(fmul(a_over_3, a_over_3), a_over_3));
   if (q > 0.0f) q = 0.0f;
   const float rho = fsqrt_rn(-a_over_3);
-  const float theta = fmul((float)atan2((double)fsqrt_rn(-q), (double)half_b), s_inv3);
+  const float theta = fmul((float)atan2_rn((double)fsqrt_rn(-q), (double)half_b), s_inv3);
   const float cos_theta = (float)cos((double)theta), sin_theta = (float)sin((double)theta);
   r[0] = fadd(c2_over_3, fmul(fmul(2.0f, rho), cos_theta));
   r[1] = fsub(c2_over_3, fmul(rho, fadd(cos_theta, fmul(s_sqrt3, sin_theta))));

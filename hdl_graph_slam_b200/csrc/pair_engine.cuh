@@ -86,7 +86,10 @@ struct PairDev {
 // (msg_mix, the position-dependent checksum term, lives in common.cuh)
 
 // The LM step functions below are __host__ __device__: the device runs them in the last block of k_pair_accumulate, and
-// tests/lm_harness.cu drives the very same state machine on the CPU against the oracle's step_lm (no GPU needed).
+// tests/lm_harness.cu drives their host build on the CPU against the oracle's step_lm (no GPU needed).  The two builds are not the
+// same arithmetic: the device may contract the plain float64 products of ldlt6_solve / se3_exp / mul_iso into FMAs.  Replayed over
+// the same round sums (tests/test_device_numerics_gpu.py) they take the same decisions, with lambda and nu within 1e-12 relative and
+// the pose within 1e-12 of its largest entry.
 // report (16 words) -> dst, checksum -> dst[16]; flag = seq.  No system-scope fences: the host accepts the message only when
 // it is self-consistent (wait_report).
 B2R_HD void publish_report(const PairReport& rep, PairReport* dst, unsigned long long* flag, unsigned long long seq) {

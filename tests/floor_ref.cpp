@@ -23,7 +23,8 @@
 //                row cross products of (A/scale - roots(0) I), the first largest squared norm, divided by its sqrt.
 //                computeRoots2's d = Scalar(b * b - 4.0 * c): b * b in float32, the rest in float64.
 //    trig        ENGINE  atan2f / cosf / sinf of computeRoots as (float)f((double)x): glibc's float routines cannot be reproduced on
-//                the device.
+//                the device.  atan2 is the engine's atan2_rn (csrc/atan2_rn.cuh), shared with the device: CUDA's and glibc's float64
+//                atan2 round some float32 results differently; cos and sin agree on every |t| <= 1.1.
 //    squares     UPSTREAM-RECALL  Vector3f squaredNorm as x x + (y y + z z): Eigen 3.3 reduces a fixed-size 3-vector with
 //                redux_novec_unroller, which splits at Length / 2 = 1 (first element, then the sum of the other two).
 //    keep        UPSTREAM-RECALL  |normalized(n).dot(UnitZ)| > cos(normal_filter_thresh * M_PI / 180.0) in float64, where the dot
@@ -63,6 +64,7 @@
 #include <unordered_map>
 #include <utility>
 #include <vector>
+#include "../hdl_graph_slam_b200/csrc/atan2_rn.cuh"
 
 namespace {
 
@@ -154,7 +156,7 @@ void roots(const float m[3][3], float* r) {
   float q = half_b * half_b + a_over_3 * a_over_3 * a_over_3;
   if (q > 0.f) q = 0.f;
   const float rho = std::sqrt(-a_over_3);
-  const float theta = (float)std::atan2((double)std::sqrt(-q), (double)half_b) * s_inv3;
+  const float theta = (float)b2r::atan2_rn((double)std::sqrt(-q), (double)half_b) * s_inv3;
   const float cos_theta = (float)std::cos((double)theta), sin_theta = (float)std::sin((double)theta);
   r[0] = c2_over_3 + 2.0f * rho * cos_theta;
   r[1] = c2_over_3 - rho * (cos_theta + s_sqrt3 * sin_theta);
