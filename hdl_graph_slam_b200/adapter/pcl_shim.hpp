@@ -1,7 +1,8 @@
-// pcl_shim.hpp — TEST-ONLY stand-in for the handful of PCL / Eigen declarations b200_registration.hpp touches, so the
-// adapter can be syntax-checked in an image without PCL (tests/test_adapter_syntax.py).  Signatures follow PCL 1.10
+// pcl_shim.hpp — TEST-ONLY stand-in for the handful of PCL / Eigen declarations b200_registration.hpp and b200_backend.hpp touch, so
+// the adapters can be syntax-checked in an image without PCL (tests/test_adapter_syntax.py).  Signatures follow PCL 1.10
 // (the distro package of ROS noetic, /root/reference/docker/noetic/Dockerfile:6).  Nothing here is shipped or linked.
 #pragma once
+#include <cstdint>
 #include <limits>
 #include <memory>
 #include <string>
@@ -31,6 +32,9 @@ static_assert(sizeof(PointXYZI) == 32, "pcl::PointXYZI is a 32-byte record");
 template <typename PointT>
 struct PointCloud {
   std::vector<PointT> points;
+  uint32_t width = 0, height = 0;
+  bool is_dense = true;
+  size_t size() const { return points.size(); }
   using Ptr = std::shared_ptr<PointCloud<PointT>>;
   using ConstPtr = std::shared_ptr<const PointCloud<PointT>>;
 };
