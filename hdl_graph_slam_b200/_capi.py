@@ -150,6 +150,7 @@ SYMBOLS = [
     ("b2r_floor_params_default", C.c_int, [C.POINTER(FloorParams)]),
     ("b2r_floor_detect", C.c_int, [_VP, _VP, _SZ, _SZ, C.c_int, C.POINTER(FloorParams), C.POINTER(FloorResult), _VP, _VP, C.POINTER(_VP), C.POINTER(_VP)]),
     ("b2r_ingest_pointcloud2", C.c_int, [_VP, _VP, _SZ, C.POINTER(PointLayout), C.POINTER(_VP)]),
+    ("b2r_ingest_pointcloud2_rows", C.c_int, [_VP, _VP, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(PointLayout), C.POINTER(_VP)]),
     ("b2r_pcd_read_header", C.c_int, [C.c_char_p, C.POINTER(PointLayout), C.POINTER(_SZ), C.POINTER(_SZ)]),
     ("b2r_ingest_pcd", C.c_int, [_VP, C.c_char_p, C.POINTER(_VP), C.POINTER(_SZ)]),
     ("b2r_map_cloud_generate", C.c_int, [_VP, C.POINTER(KeyframeSnapshot), _SZ, _SZ, C.c_double, _VP, _SZ, C.POINTER(_SZ)]),

@@ -40,15 +40,16 @@ struct MatrixXd {
 }  // namespace Eigen
 
 namespace ros {
-// the private namespace of a nodelet: values kept as strings, converted on read as the parameter server would
+// the private namespace of a nodelet: values kept as strings, converted on read as the parameter server would.  Copies share one
+// store, as copies of a roscpp NodeHandle reach the same parameter server.
 class NodeHandle {
 public:
-  void setParam(const std::string& key, const std::string& value) { p_[key] = value; }
-  bool hasParam(const std::string& key) const { return p_.count(key) != 0; }
+  void setParam(const std::string& key, const std::string& value) { (*p_)[key] = value; }
+  bool hasParam(const std::string& key) const { return p_->count(key) != 0; }
   template <typename T>
   T param(const std::string& key, const T& default_val) const {
-    auto it = p_.find(key);
-    if (it == p_.end()) return default_val;
+    auto it = p_->find(key);
+    if (it == p_->end()) return default_val;
     return convert(it->second, default_val);
   }
 
@@ -62,7 +63,7 @@ private:
   }
   static std::string convert(const std::string& s, const std::string&) { return s; }
   static bool convert(const std::string& s, const bool&) { return s == "true" || s == "1"; }
-  std::map<std::string, std::string> p_;
+  std::shared_ptr<std::map<std::string, std::string>> p_ = std::make_shared<std::map<std::string, std::string>>();
 };
 }  // namespace ros
 

@@ -29,8 +29,16 @@ struct alignas(16) PointXYZI {
 };
 static_assert(sizeof(PointXYZI) == 32, "pcl::PointXYZI is a 32-byte record");
 
+// pcl::PCLHeader: stamp in microseconds, as pcl_conversions::toPCL writes it
+struct PCLHeader {
+  uint32_t seq = 0;
+  uint64_t stamp = 0;
+  std::string frame_id;
+};
+
 template <typename PointT>
 struct PointCloud {
+  PCLHeader header;
   std::vector<PointT> points;
   uint32_t width = 0, height = 0;
   bool is_dense = true;

@@ -2171,6 +2171,40 @@ extern "C" int b2r_ingest_pointcloud2(b2r_handle* h, const void* data, size_t n_
   return rc;
 }
 
+// an organized message as fromROSMsg takes it: height rows of row_step bytes, each holding width records of point_step bytes and
+// any padding after them.  The whole height * row_step blob goes up; k_unpack_points_rows skips the padding on the device.
+extern "C" int b2r_ingest_pointcloud2_rows(b2r_handle* h, const void* data, uint32_t width, uint32_t height, uint32_t row_step,
+                                           const b2r_point_layout* layout, const void** d_points) {
+  const size_t n = (size_t)width * height;
+  if (!h || !d_points || (n && !data)) return fail(B2R_EINVAL, "NULL argument");
+  int rc = layout_check(layout);
+  if (rc) return rc;
+  if (n && (uint64_t)row_step < (uint64_t)width * layout->point_step) return fail(B2R_EINVAL, "row_step is shorter than width * point_step");
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  *d_points = nullptr;
+  if (n == 0) return B2R_OK;
+  if (n > (size_t)0x3fffffff) return fail(B2R_EINVAL, "too many points");
+  const size_t bytes = (size_t)height * row_step;
+  B2R_CUDA(h->ingest_blob.reserve(bytes + 16));
+  const bool pinned = is_pinned_host(data);
+  B2R_CUDA(cudaMemcpyAsync(h->ingest_blob.p, data, bytes, cudaMemcpyHostToDevice, h->st));
+  h->tel.h2d += bytes;
+  if (pinned) B2R_CUDA(cudaEventRecord(h->upload_ev, h->st));
+  B2R_CUDA(h->ingest_out.reserve(n * 8 + 8));
+  UnpackRowsArgs A;
+  A.data = reinterpret_cast<const unsigned char*>(h->ingest_blob.p); A.n = (long long)n; A.width = width; A.row_step = row_step;
+  A.point_step = layout->point_step; A.off_x = layout->off_x; A.off_y = layout->off_y; A.off_z = layout->off_z;
+  A.off_i = layout->intensity_datatype == 7 ? layout->off_intensity : 0xffffffffu;  // as ingest_device: only FLOAT32 intensity is mapped
+  A.bigendian = layout->is_bigendian; A.out = h->ingest_out.p;
+  { TEL_BEGIN(&h->tel, h->st);
+    k_unpack_points_rows<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)h->n_sm * 16), 256, 0, h->st>>>(A);
+    TEL_END(&h->tel, KC_MISC, 1, h->st); }
+  B2R_CUDA(cudaGetLastError());
+  *d_points = h->ingest_out.p;
+  if (pinned) B2R_CUDA(cudaEventSynchronize(h->upload_ev));
+  return B2R_OK;
+}
+
 extern "C" int b2r_pcd_read_header(const char* path, b2r_point_layout* layout, size_t* n_points, size_t* data_offset) {
   if (!path || !layout || !n_points) return fail(B2R_EINVAL, "NULL argument");
   FILE* f = fopen(path, "rb");

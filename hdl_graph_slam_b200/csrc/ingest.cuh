@@ -6,6 +6,7 @@
 //                        arbitrary byte offsets of a point_step-long record.  As in PCL, a field is mapped only when its datatype
 //                        and count match the point type's, so intensity is read only when it is FLOAT32; any other intensity
 //                        field is left unmapped and the point keeps intensity 0.  is_bigendian byte-swaps (PCL copies native bytes).
+//   k_unpack_points_rows <- the same for organized messages with padded rows (row_step > width * point_step).
 #pragma once
 #include <cstdio>
 #include <cstring>
@@ -31,6 +32,31 @@ __global__ void k_unpack_points(const __grid_constant__ UnpackArgs A) {
   const bool swap = A.bigendian != 0;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < A.n; i += (long long)gridDim.x * blockDim.x) {
     const unsigned char* r = A.data + (size_t)i * A.point_step;
+    float* o = A.out + (size_t)i * 8;
+    o[0] = __uint_as_float(load_u32(r + A.off_x, swap));
+    o[1] = __uint_as_float(load_u32(r + A.off_y, swap));
+    o[2] = __uint_as_float(load_u32(r + A.off_z, swap));
+    o[3] = 1.0f;
+    o[4] = A.off_i != 0xffffffffu ? __uint_as_float(load_u32(r + A.off_i, swap)) : 0.f;
+    o[5] = 0.f; o[6] = 0.f; o[7] = 0.f;
+  }
+}
+
+// k_unpack_points_rows <- the same mapping for an organized message whose rows are padded (row_step > width * point_step), which
+// fromROSMsg accepts: record i sits at (i / width) * row_step + (i % width) * point_step.  Kept apart from k_unpack_points so the
+// contiguous path's code stays as it is.
+struct UnpackRowsArgs {
+  const unsigned char* data;
+  long long n;
+  unsigned int width, row_step;
+  unsigned int point_step, off_x, off_y, off_z, off_i, bigendian;
+  float* out;
+};
+
+__global__ void k_unpack_points_rows(const __grid_constant__ UnpackRowsArgs A) {
+  const bool swap = A.bigendian != 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < A.n; i += (long long)gridDim.x * blockDim.x) {
+    const unsigned char* r = A.data + (size_t)(i / A.width) * A.row_step + (size_t)(i % A.width) * A.point_step;
     float* o = A.out + (size_t)i * 8;
     o[0] = __uint_as_float(load_u32(r + A.off_x, swap));
     o[1] = __uint_as_float(load_u32(r + A.off_y, swap));

@@ -420,6 +420,19 @@ class Registration:
         check(self._lib.b2r_ingest_pointcloud2(self._h, buf.ctypes.data_as(C.c_void_p), n_points, C.byref(L), C.byref(out)))
         return out.value
 
+    def ingestPointCloud2Rows(self, blob, width, height, row_step, point_step, off_x=0, off_y=4, off_z=8, off_intensity=0xffffffff,
+                              intensity_datatype=7, is_bigendian=False):
+        """organized sensor_msgs/PointCloud2 data[] with rows of row_step bytes (padding after width * point_step allowed) -> device
+        PointXYZI records, width * height of them (b2r_ingest_pointcloud2_rows); returns the device pointer"""
+        buf = np.frombuffer(blob, np.uint8) if not isinstance(blob, np.ndarray) else blob.view(np.uint8).reshape(-1)
+        if width * height and buf.size < height * row_step:
+            raise ValueError("blob is shorter than height * row_step")
+        self._keep["pc2"] = buf
+        L = _capi.PointLayout(point_step, off_x, off_y, off_z, off_intensity, intensity_datatype, int(is_bigendian))
+        out = C.c_void_p()
+        check(self._lib.b2r_ingest_pointcloud2_rows(self._h, buf.ctypes.data_as(C.c_void_p), width, height, row_step, C.byref(L), C.byref(out)))
+        return out.value
+
     def ingestPcd(self, path):
         """binary PCD file -> (device pointer to PointXYZI records, point count) (b2r_ingest_pcd)"""
         out, n = C.c_void_p(), C.c_size_t()

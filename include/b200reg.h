@@ -392,8 +392,9 @@ int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot* keyframes
  *     intensity field of any other datatype is left unmapped and every point gets intensity 0 (PCL warns and does the same).
  *   - is_bigendian is honoured: x, y, z and intensity are byte-swapped.  (PCL copies the bytes as they are, so a big-endian
  *     message on a little-endian host decodes to garbage there; this is a deliberate deviation.)
- *   - Rows must be contiguous: n_points records of point_step bytes back to back, i.e. row_step == width * point_step.  An
- *     organized message with padded rows has to be repacked by the caller first.
+ *   - b2r_ingest_pointcloud2 takes contiguous rows: n_points records of point_step bytes back to back, i.e. row_step == width *
+ *     point_step.  An organized message with padded rows (row_step > width * point_step), which fromROSMsg also accepts, goes to
+ *     b2r_ingest_pointcloud2_rows.
  *   - b2r_ingest_pointcloud2 is synchronous with respect to `data`: when it returns, the copy out of the caller's buffer has
  *     finished (pageable or pinned) and the buffer may be reused. */
 typedef struct b2r_point_layout {
@@ -405,6 +406,13 @@ typedef struct b2r_point_layout {
   uint32_t is_bigendian;       /* PointCloud2.is_bigendian */
 } b2r_point_layout;
 int b2r_ingest_pointcloud2(b2r_handle* h, const void* data, size_t n_points, const b2r_point_layout* layout, const void** d_points);
+/* the same unpacking for an organized message whose rows may be padded: `data` holds height * row_step bytes (all of them are
+ * copied), and record i = r * width + c (row-major, width * height records, NaN records included) is read at byte
+ * r * row_step + c * point_step.  Field mapping, byte order, intensity rules and the lifetime of *d_points are
+ * b2r_ingest_pointcloud2's.  B2R_EINVAL when row_step < width * point_step (for a non-empty message); width * height = 0 succeeds
+ * with *d_points = NULL. */
+int b2r_ingest_pointcloud2_rows(b2r_handle* h, const void* data, uint32_t width, uint32_t height, uint32_t row_step,
+                                const b2r_point_layout* layout, const void** d_points);
 /* header of a binary PCD file (the cloud.pcd KeyFrame::save writes with pcl::io::savePCDFileBinary, keyframe.cpp:57): x, y, z must be
  * F 4 COUNT 1 (else B2R_EINVAL); "intensity" is reported (datatype 7) only when it is F 4 COUNT 1, otherwise off_intensity = 0xffffffff.
  * DATA ascii / binary_compressed: B2R_EUNSUPPORTED.  Without POINTS the count is WIDTH * HEIGHT. */
