@@ -158,6 +158,8 @@ SYMBOLS = [
     ("b2r_odometry_destroy", None, [_VP]),
     ("b2r_odometry_matching", C.c_int, [_VP, C.c_double, _VP, _SZ, _SZ, _F32P, C.POINTER(OdometryStatus)]),
     ("b2r_odometry_matching_device", C.c_int, [_VP, C.c_double, _VP, _SZ, _SZ, _F32P, C.POINTER(OdometryStatus)]),
+    ("b2r_odometry_matching_ros", C.c_int, [_VP, C.c_uint32, C.c_uint32, _VP, _SZ, _SZ, C.c_int, _F32P, C.c_int, C.POINTER(OdometryStatus)]),
+    ("b2r_odometry_aligned", C.c_int, [_VP, C.c_int, _VP, _SZ, _SZ]),
     ("b2r_loop_matching", C.c_int, [_VP, _VP, _SZ, _SZ, C.POINTER(_VP), C.POINTER(_SZ), _SZ, _F32P, C.c_double, C.c_double,
                                     C.POINTER(Result), _I32P]),
     ("b2r_batch_create", C.c_int, [C.POINTER(Config), C.POINTER(_VP)]),

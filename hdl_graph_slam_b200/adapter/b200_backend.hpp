@@ -10,8 +10,8 @@
 // stand-ins adapter/pcl_shim.hpp and adapter/backend_shim.hpp.
 #pragma once
 #include <b200reg.h>
+#include "b200_select.hpp"
 #include <algorithm>
-#include <cstdio>
 #include <deque>
 #include <iostream>
 #include <limits>
@@ -35,22 +35,7 @@ public:
   // pnh: the back end's private namespace, the one LoopDetector(pnh) reads.  A registration_method the engine does not re-create
   // (B2R_EUNSUPPORTED) throws here with the engine's message, so the caller can keep the reference classes.
   explicit B200KeyframeCache(ros::NodeHandle& pnh) {
-    // forward only the parameters that are set: the engine applies each branch's own defaults (registrations.cpp:22-124)
-    std::vector<std::string> keys, values;
-    auto put = [&](const char* k, const std::string& v) { keys.push_back(k); values.push_back(v); };
-    auto num = [](double v) { char s[32]; std::snprintf(s, sizeof s, "%.17g", v); return std::string(s); };
-    for (const char* k : {"registration_method", "reg_nn_search_method"})
-      if (pnh.hasParam(k)) put(k, pnh.param<std::string>(k, ""));
-    for (const char* k : {"reg_resolution", "reg_transformation_epsilon", "reg_max_correspondence_distance"})
-      if (pnh.hasParam(k)) put(k, num(pnh.param<double>(k, 0.0)));
-    for (const char* k : {"reg_maximum_iterations", "reg_correspondence_randomness", "reg_max_optimizer_iterations"})
-      if (pnh.hasParam(k)) put(k, std::to_string(pnh.param<int>(k, 0)));
-    if (pnh.hasParam("reg_use_reciprocal_correspondences"))
-      put("reg_use_reciprocal_correspondences", pnh.param<bool>("reg_use_reciprocal_correspondences", false) ? "true" : "false");
-    std::vector<const char*> k, v;
-    for (size_t i = 0; i < keys.size(); i++) { k.push_back(keys[i].c_str()); v.push_back(values[i].c_str()); }
-    b2r_handle* h = nullptr;
-    check(b2r_select_registration_method(k.data(), v.data(), (int)k.size(), pnh.param<int>("reg_device_id", 0), &h));
+    b2r_handle* h = b200_select::select_registration_method(pnh);
     b2r_config cfg;
     const int rc = b2r_get_config(h, &cfg);
     b2r_destroy(h);

@@ -9,6 +9,8 @@
 //                                      (pcl::IterativeClosestPoint loop: icp_pcl.cuh)
 //   b2r_fitness                     <- getFitnessScore
 //   b2r_odometry_matching           <- ScanMatchingOdometryNodelet::matching  apps/scan_matching_odometry_nodelet.cpp:165-262
+//   b2r_odometry_matching_ros       <- the same with ros::Time stamps and the status chosen per frame (:243, :299)
+//   b2r_odometry_aligned            <- matching's aligned_points cloud                          :254-259
 //   b2r_loop_matching               <- LoopDetector::matching                include/hdl_graph_slam/loop_detector.hpp:117-171
 // There is deliberately NO CPU fallback in this file: every compute step is a CUDA kernel launch.
 #include <cuda_runtime.h>
@@ -90,7 +92,10 @@ struct b2r_handle {
   DevBuf<unsigned char> pf_flags;
   DevBuf<int> pf_blocks;
   DevBuf<char> ingest_blob;         // PointCloud2 / PCD bodies as uploaded, and their PointXYZI unpacking
-  DevBuf<float> ingest_out;
+  // two unpacking buffers, used in turn: a cloud an ingest returns survives the next ingest, so a frame registered by pointer
+  // (b2r_odometry_matching_ros with device = 1) is still intact when the following frame, ingested first, is matched against it
+  DevBuf<float> ingest_out[2];
+  int ingest_slot = 0;
   PinnedBuf<char> ingest_pinned;
   DevBuf<char> map_kf;              // MapCloudGenerator: keyframe descriptors, voxel keys
   DevBuf<unsigned long long> map_keys[2];
@@ -2122,19 +2127,25 @@ extern "C" int b2r_floor_detect(b2r_handle* h, const void* points, size_t n, siz
 }
 
 // ------------------------------------------------------------------------------------------------ wire / disk ingest ("next" row f-4)
+static DevBuf<float>& next_ingest_out(b2r_handle* h) {
+  h->ingest_slot ^= 1;
+  return h->ingest_out[h->ingest_slot];
+}
+
 static int ingest_device(b2r_handle* h, const unsigned char* d_blob, size_t n, const b2r_point_layout& L, const void** d_out) {
-  B2R_CUDA(h->ingest_out.reserve(n * 8 + 8));
+  DevBuf<float>& out = next_ingest_out(h);
+  B2R_CUDA(out.reserve(n * 8 + 8));
   UnpackArgs A;
   A.data = d_blob; A.n = (long long)n; A.point_step = L.point_step; A.off_x = L.off_x; A.off_y = L.off_y; A.off_z = L.off_z;
   // pcl::PointXYZI's intensity is a float: fromPCLPointCloud2 maps an "intensity" field only when it is FLOAT32 (count 1) and
   // leaves the point's intensity at 0 for every other datatype
   A.off_i = L.intensity_datatype == 7 ? L.off_intensity : 0xffffffffu;
-  A.bigendian = L.is_bigendian; A.out = h->ingest_out.p;
+  A.bigendian = L.is_bigendian; A.out = out.p;
   { TEL_BEGIN(&h->tel, h->st);
     k_unpack_points<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)h->n_sm * 16), 256, 0, h->st>>>(A);
     TEL_END(&h->tel, KC_MISC, 1, h->st); }
   B2R_CUDA(cudaGetLastError());
-  *d_out = h->ingest_out.p;
+  *d_out = out.p;
   return B2R_OK;
 }
 static int layout_check(const b2r_point_layout* L) {
@@ -2190,17 +2201,18 @@ extern "C" int b2r_ingest_pointcloud2_rows(b2r_handle* h, const void* data, uint
   B2R_CUDA(cudaMemcpyAsync(h->ingest_blob.p, data, bytes, cudaMemcpyHostToDevice, h->st));
   h->tel.h2d += bytes;
   if (pinned) B2R_CUDA(cudaEventRecord(h->upload_ev, h->st));
-  B2R_CUDA(h->ingest_out.reserve(n * 8 + 8));
+  DevBuf<float>& out = next_ingest_out(h);
+  B2R_CUDA(out.reserve(n * 8 + 8));
   UnpackRowsArgs A;
   A.data = reinterpret_cast<const unsigned char*>(h->ingest_blob.p); A.n = (long long)n; A.width = width; A.row_step = row_step;
   A.point_step = layout->point_step; A.off_x = layout->off_x; A.off_y = layout->off_y; A.off_z = layout->off_z;
   A.off_i = layout->intensity_datatype == 7 ? layout->off_intensity : 0xffffffffu;  // as ingest_device: only FLOAT32 intensity is mapped
-  A.bigendian = layout->is_bigendian; A.out = h->ingest_out.p;
+  A.bigendian = layout->is_bigendian; A.out = out.p;
   { TEL_BEGIN(&h->tel, h->st);
     k_unpack_points_rows<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)h->n_sm * 16), 256, 0, h->st>>>(A);
     TEL_END(&h->tel, KC_MISC, 1, h->st); }
   B2R_CUDA(cudaGetLastError());
-  *d_points = h->ingest_out.p;
+  *d_points = out.p;
   if (pinned) B2R_CUDA(cudaEventSynchronize(h->upload_ev));
   return B2R_OK;
 }
@@ -2413,6 +2425,23 @@ struct b2r_odometry {
   unsigned long long pf_stamp = 0;
   const float* pf_out = nullptr;
   size_t pf_m = 0;
+  // the keyframe's stamp as b2r_odometry_matching_ros gave it (keyframe_ros), for roscpp's exact delta_time
+  bool keyframe_ros = false;
+  uint32_t keyframe_sec = 0, keyframe_nsec = 0;
+  // the last frame's raw records for b2r_odometry_aligned: where matching left them (the source upload, a slot's `in`, or the
+  // caller's device cloud), valid until the next matching call; aligned_ok only after an accepted frame
+  bool aligned_ok = false;
+  const float* raw = nullptr;
+  size_t raw_n = 0, raw_stride = 0;
+  float odom_row[16];
+  DevBuf<float> aligned_out;
+};
+
+// a frame's stamp in the form the caller gave it: a double (b2r_odometry_matching*) or ros::Time's sec / nsec, with t = toSec()
+struct OdomStamp {
+  double t;
+  bool ros;
+  uint32_t sec, nsec;
 };
 
 static bool odometry_downsamples(const b2r_odometry_params& p) {
@@ -2514,8 +2543,8 @@ static int odometry_take(b2r_odometry* o, const void* cloud, size_t n, size_t st
   return odometry_downsample(o, o->cur, o->reg->st, cloud, n, stride, device, d_reg, m_reg);
 }
 
-static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* cloud, size_t n, size_t stride_bytes, const float* msf_delta,
-                                  b2r_odometry_status* out, bool device);
+static int odometry_matching_impl(b2r_odometry* o, const OdomStamp& stamp, const void* cloud, size_t n, size_t stride_bytes, const float* msf_delta,
+                                  b2r_odometry_status* out, bool device, bool want_status);
 extern "C" int b2r_odometry_prefetch(b2r_odometry* o, const void* cloud, size_t n, size_t stride_bytes, int device) {
   if (!o) return fail(B2R_EINVAL, "NULL argument");
   o->next_ptr = cloud; o->next_n = n; o->next_stride = stride_bytes; o->next_device = device != 0; o->next_pending = true;
@@ -2569,18 +2598,49 @@ static int odometry_set_cloud(b2r_odometry* o, bool is_target, const void* cloud
 
 extern "C" int b2r_odometry_matching(b2r_odometry* o, double stamp, const void* cloud, size_t n, size_t stride_bytes,
                                      const float* msf_delta, b2r_odometry_status* out) {
-  return odometry_matching_impl(o, stamp, cloud, n, stride_bytes, msf_delta, out, false);
+  const OdomStamp t = {stamp, false, 0, 0};
+  return odometry_matching_impl(o, t, cloud, n, stride_bytes, msf_delta, out, false, o && o->p.publish_status);
 }
 extern "C" int b2r_odometry_matching_device(b2r_odometry* o, double stamp, const void* d_cloud, size_t n, size_t stride_bytes,
                                             const float* msf_delta, b2r_odometry_status* out) {
-  return odometry_matching_impl(o, stamp, d_cloud, n, stride_bytes, msf_delta, out, true);
+  const OdomStamp t = {stamp, false, 0, 0};
+  return odometry_matching_impl(o, t, d_cloud, n, stride_bytes, msf_delta, out, true, o && o->p.publish_status);
 }
-static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* cloud, size_t n, size_t stride_bytes, const float* msf_delta,
-                                  b2r_odometry_status* out, bool device) {
+extern "C" int b2r_odometry_matching_ros(b2r_odometry* o, uint32_t sec, uint32_t nsec, const void* cloud, size_t n, size_t stride_bytes,
+                                         int device, const float* msf_delta, int want_status, b2r_odometry_status* out) {
+  const OdomStamp t = {(double)sec + 1e-9 * (double)nsec, true, sec, nsec};  // ros::Time::toSec()
+  return odometry_matching_impl(o, t, cloud, n, stride_bytes, msf_delta, out, device != 0, want_status != 0);
+}
+
+extern "C" int b2r_odometry_aligned(b2r_odometry* o, int is_dense, void* out_points, size_t n, size_t stride_bytes) {
+  if (!o || (!out_points && n)) return fail(B2R_EINVAL, "NULL argument");
+  if (!o->aligned_ok) return fail(B2R_ESTATE, "no aligned cloud: the last matching call was a first frame, a rejected frame or an error");
+  if (n != o->raw_n) return fail(B2R_EINVAL, "n does not match the last frame's cloud");
+  if (stride_bytes != o->raw_stride) return fail(B2R_EINVAL, "stride_bytes does not match the last frame's cloud");
+  if (n == 0) return B2R_OK;
+  b2r_handle* h = o->reg;
+  B2R_CUDA(cudaSetDevice(h->cfg.device_id));
+  const int sf = (int)(stride_bytes / 4);
+  B2R_CUDA(o->aligned_out.reserve(n * sf));
+  XfArg X;
+  for (int i = 0; i < 12; i++) X.Tf[i] = o->odom_row[i];
+  { TEL_BEGIN(&h->tel, h->st);
+    k_transform_aligned_records<<<(unsigned)((n + 255) / 256), 256, 0, h->st>>>(o->raw, sf, (int)n, X, is_dense, o->aligned_out.p);
+    TEL_END(&h->tel, KC_MISC, 1, h->st); }
+  B2R_CUDA(cudaGetLastError());
+  B2R_CUDA(cudaMemcpyAsync(out_points, o->aligned_out.p, n * stride_bytes, cudaMemcpyDeviceToHost, h->st));
+  B2R_CUDA(cudaStreamSynchronize(h->st));
+  h->tel.d2h += n * stride_bytes;
+  return B2R_OK;
+}
+
+static int odometry_matching_impl(b2r_odometry* o, const OdomStamp& stamp, const void* cloud, size_t n, size_t stride_bytes, const float* msf_delta,
+                                  b2r_odometry_status* out, bool device, bool want_status) {
   if (!o || !out) return fail(B2R_EINVAL, "NULL argument");
   std::memset(out, 0, sizeof(*out));
   out->matching_error = NAN;
   out->inlier_fraction = NAN;
+  o->aligned_ok = false;
   b2r_handle* reg = o->reg;
   float I[16];
   mat4_identity(I);
@@ -2588,7 +2648,8 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
     o->prev_time_zero = true;
     mat4_identity(o->prev_trans);
     mat4_identity(o->keyframe_pose);
-    o->keyframe_stamp = stamp;
+    o->keyframe_stamp = stamp.t;
+    o->keyframe_ros = stamp.ros; o->keyframe_sec = stamp.sec; o->keyframe_nsec = stamp.nsec;
     size_t n_reg = 0;
     int rc = odometry_set_cloud(o, true, cloud, n, stride_bytes, device, &n_reg);  // keyframe = downsample(cloud)
     if (rc) return rc;
@@ -2603,6 +2664,11 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
   size_t n_reg = 0;  // aligned->size() of :321
   int rc = odometry_set_cloud(o, false, cloud, n, stride_bytes, device, &n_reg);  // :176-177
   if (rc) return rc;
+  // the raw records of `cloud` on the device, for b2r_odometry_aligned: a downsampled frame's host cloud was uploaded into its slot's
+  // `in` (also when the prefetch did it), a device cloud is read where it is; without a downsample the source reads them itself
+  o->raw = odometry_downsamples(o->p) ? (device ? (const float*)cloud : o->vw[o->cur].in.p) : SRC(reg).raw_view;
+  o->raw_n = n;
+  o->raw_stride = stride_bytes;
   // the NEXT frame's upload / BVH / covariances overlap this frame's align on a second stream.  Its downsample waits on the host
   // for the filter's output count; on a GICP handle it is therefore issued from inside the align, once the align's first rounds
   // are on the main stream, so that the wait does not hold them back
@@ -2624,7 +2690,7 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
   out->converged = res.converged;
   out->iterations = res.iterations;
   std::memcpy(out->trans, res.T, sizeof(res.T));
-  if (o->p.publish_status) {  // :298-335
+  if (want_status) {  // :298-335
     double score;
     uint32_t used, inl;
     rc = b2r_fitness(reg, nullptr, DBL_MAX, 0.5f * 0.5f, &score, &used, &inl);
@@ -2634,23 +2700,30 @@ static int odometry_matching_impl(b2r_odometry* o, double stamp, const void* clo
   }
   float trans[16], odom_row[16];
   for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) trans[r * 4 + c] = res.T[c * 4 + r];
-  const OdometryDecision d = odometry_gate(o->p, o->keyframe_pose, o->prev_trans, trans, res.converged != 0, stamp, o->keyframe_stamp, odom_row);
+  // :243 (stamp - keyframe_stamp).toSec(): roscpp's rule when both stamps came as sec / nsec, else the difference of the doubles (a
+  // ros::Time stamp then as its toSec())
+  const double delta_time = stamp.ros && o->keyframe_ros ? ros_delta_time(stamp.sec, stamp.nsec, o->keyframe_sec, o->keyframe_nsec)
+                                                         : stamp.t - o->keyframe_stamp;
+  const OdometryDecision d = odometry_gate_dt(o->p, o->keyframe_pose, o->prev_trans, trans, res.converged != 0, delta_time, odom_row);
   row_to_col(odom_row, out->odom);
   if (d == ODOM_REJECTED) {  // :214-218, :223-233: prev_trans, prev_time and the keyframe stay as they are
     out->frame_rejected = 1;
     return B2R_OK;
   }
-  o->prev_time = stamp;  // :235-236
+  std::memcpy(o->odom_row, odom_row, sizeof(odom_row));
+  o->prev_time = stamp.t;  // :235-236
   o->prev_time_zero = false;
   std::memcpy(o->prev_trans, trans, sizeof(trans));
   if (d == ODOM_KEYFRAME) {  // :241-252
     rc = b2r_promote_source_to_target(reg);  // keyframe = filtered; registration->setInputTarget(keyframe)
     if (rc) return rc;
     std::memcpy(o->keyframe_pose, odom_row, sizeof(odom_row));
-    o->keyframe_stamp = stamp;
+    o->keyframe_stamp = stamp.t;
+    o->keyframe_ros = stamp.ros; o->keyframe_sec = stamp.sec; o->keyframe_nsec = stamp.nsec;
     mat4_identity(o->prev_trans);
     out->keyframe_updated = 1;
   }
+  o->aligned_ok = true;
   return B2R_OK;
 }
 

@@ -119,4 +119,21 @@ __global__ void k_transform(const float* __restrict__ raw, int stride_f, int n, 
                        xform_row(X.Tf[8], X.Tf[9], X.Tf[10], X.Tf[11], x, y, z), 1.0f);
 }
 
+// the `aligned_points` cloud of ScanMatchingOdometryNodelet::matching (:254-259), pcl::transformPointCloud(*cloud, *aligned, odom) of the
+// frame's raw records: the record copied, then xyz as k_transform and 1.0f at float 3.  is_dense == 0: a record with a non-finite x,
+// y or z stays as copied (PCL 1.10's non-dense branch, UPSTREAM-RECALL)
+__global__ void k_transform_aligned_records(const float* __restrict__ in, int stride_f, int n, XfArg X, int is_dense, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float* p = in + (size_t)i * stride_f;
+  float* o = out + (size_t)i * stride_f;
+  for (int k = 0; k < stride_f; k++) o[k] = p[k];
+  const float x = p[0], y = p[1], z = p[2];
+  if (!is_dense && !finite3(x, y, z)) return;
+  o[0] = xform_row(X.Tf[0], X.Tf[1], X.Tf[2], X.Tf[3], x, y, z);
+  o[1] = xform_row(X.Tf[4], X.Tf[5], X.Tf[6], X.Tf[7], x, y, z);
+  o[2] = xform_row(X.Tf[8], X.Tf[9], X.Tf[10], X.Tf[11], x, y, z);
+  if (stride_f > 3) o[3] = 1.0f;
+}
+
 }  // namespace b2r

@@ -6,6 +6,7 @@
 //   odom = keyframe_pose * trans                                                                          :220-221
 //   transform_thresholding         -> delta = prev_trans.inverse() * trans, dx, da, reject               :223-233
 //   keyframe switch                -> delta_trans, delta_angle, delta_time                               :241-252
+//                                     (delta_time of two ros::Time stamps: ros_delta_time; of two doubles: their difference)
 // Arithmetic (DESIGN.md §2 "Documented oracle choices"): everything the reference computes on Eigen::Matrix4f is float32 here too.
 //   4x4 products    float32, each entry ((a0 b0 + a1 b1) + a2 b2) + a3 b3 with separate multiplies and adds (the translation unit
 //                   is compiled with -ffp-contract=off, build.py);
@@ -21,6 +22,7 @@
 // All matrices are ROW-major float[16].
 #pragma once
 #include <cmath>
+#include <cstdint>
 #include <cstring>
 #include "../../include/b200reg.h"
 
@@ -88,12 +90,31 @@ inline bool odometry_step_too_large(const b2r_odometry_params& p, const float* p
   return dx > p.max_acceptable_trans || da > p.max_acceptable_angle;
 }
 
-// :241-244 — does this accepted frame become the keyframe?
-inline bool odometry_wants_keyframe(const b2r_odometry_params& p, const float* trans, double stamp, double keyframe_stamp) {
+// :243 `double delta_time = (stamp - keyframe_stamp).toSec()` on two ros::Time stamps (UPSTREAM-RECALL: roscpp_core's
+// TimeBase::operator- and DurationBase::toSec, not in this tree): seconds and nanoseconds are subtracted as integers, the nanoseconds
+// normalised into [0, 1e9) by borrowing from the seconds, and toSec() = (double)sec + 1e-9 * (double)nsec.  Exact up to that last
+// rounding, unlike the difference of two epoch stamps widened to double, which keeps only about 0.24 us of an epoch stamp.
+inline double ros_delta_time(uint32_t sec, uint32_t nsec, uint32_t ref_sec, uint32_t ref_nsec) {
+  int64_t s = (int64_t)sec - (int64_t)ref_sec;
+  int64_t ns = (int64_t)nsec - (int64_t)ref_nsec;
+  s += ns / 1000000000LL;
+  ns %= 1000000000LL;
+  if (ns < 0) {
+    ns += 1000000000LL;
+    s -= 1;
+  }
+  return (double)s + 1e-9 * (double)ns;
+}
+
+// :241-244 — does this accepted frame become the keyframe?  delta_time: the frame's stamp minus the keyframe's, in seconds
+inline bool odometry_wants_keyframe_dt(const b2r_odometry_params& p, const float* trans, double delta_time) {
   const double delta_trans = translation_norm(trans);
   const double delta_angle = rotation_angle(trans);
-  const double delta_time = stamp - keyframe_stamp;
   return delta_trans > p.keyframe_delta_trans || delta_angle > p.keyframe_delta_angle || delta_time > p.keyframe_delta_time;
+}
+// the same with the two stamps as double seconds, subtracted as doubles
+inline bool odometry_wants_keyframe(const b2r_odometry_params& p, const float* trans, double stamp, double keyframe_stamp) {
+  return odometry_wants_keyframe_dt(p, trans, stamp - keyframe_stamp);
 }
 
 enum OdometryDecision { ODOM_REJECTED = 0, ODOM_ACCEPTED = 1, ODOM_KEYFRAME = 2 };
@@ -102,14 +123,19 @@ enum OdometryDecision { ODOM_REJECTED = 0, ODOM_ACCEPTED = 1, ODOM_KEYFRAME = 2 
 //   ODOM_REJECTED  not converged or thresholded: odom = keyframe_pose * prev_trans, no state changes
 //   ODOM_ACCEPTED  odom = keyframe_pose * trans; the caller sets prev_trans = trans, prev_time = stamp
 //   ODOM_KEYFRAME  as ACCEPTED, and the frame becomes the keyframe: keyframe_pose = odom, keyframe_stamp = stamp, prev_trans = I
-inline OdometryDecision odometry_gate(const b2r_odometry_params& p, const float* keyframe_pose, const float* prev_trans, const float* trans,
-                                      bool converged, double stamp, double keyframe_stamp, float* odom) {
+//   delta_time     the frame's stamp minus the keyframe's (ros_delta_time, or a difference of doubles)
+inline OdometryDecision odometry_gate_dt(const b2r_odometry_params& p, const float* keyframe_pose, const float* prev_trans, const float* trans,
+                                         bool converged, double delta_time, float* odom) {
   if (!converged || (p.transform_thresholding && odometry_step_too_large(p, prev_trans, trans))) {
     mat4_mul(keyframe_pose, prev_trans, odom);
     return ODOM_REJECTED;
   }
   mat4_mul(keyframe_pose, trans, odom);
-  return odometry_wants_keyframe(p, trans, stamp, keyframe_stamp) ? ODOM_KEYFRAME : ODOM_ACCEPTED;
+  return odometry_wants_keyframe_dt(p, trans, delta_time) ? ODOM_KEYFRAME : ODOM_ACCEPTED;
+}
+inline OdometryDecision odometry_gate(const b2r_odometry_params& p, const float* keyframe_pose, const float* prev_trans, const float* trans,
+                                      bool converged, double stamp, double keyframe_stamp, float* odom) {
+  return odometry_gate_dt(p, keyframe_pose, prev_trans, trans, converged, stamp - keyframe_stamp, odom);
 }
 
 }  // namespace b2r

@@ -7,6 +7,7 @@ Names follow the reference so that tests read like its call sites:
                                   apps/scan_matching_odometry_nodelet.cpp:172,177,210,214,220,246,307 and
                                   include/hdl_graph_slam/loop_detector.hpp:122,136,143,146,147,153
   ScanMatchingOdometry.matching <- apps/scan_matching_odometry_nodelet.cpp:165-262
+  ScanMatchingOdometry.aligned  <- its aligned_points cloud (:254-259)
   LoopDetector.matching         <- include/hdl_graph_slam/loop_detector.hpp:117-171
   VoxelGrid.filter              <- pcl::VoxelGrid as set up at apps/prefiltering_nodelet.cpp:54-58
   approximateVoxelGridFilter    <- pcl::ApproximateVoxelGrid as set up at apps/prefiltering_nodelet.cpp:61-63
@@ -555,9 +556,36 @@ class ScanMatchingOdometry:
             dp = d.ctypes.data_as(C.POINTER(C.c_float))
         fn = self._lib.b2r_odometry_matching_device if device else self._lib.b2r_odometry_matching
         check(fn(self._o, float(stamp), C.c_void_p(ptr), n, stride_bytes, dp, C.byref(st)))
-        return dict(odom=_from_colmajor(st.odom), trans=_from_colmajor(st.trans), converged=bool(st.converged), iterations=st.iterations,
-                    keyframe_updated=bool(st.keyframe_updated), frame_rejected=bool(st.frame_rejected), matching_error=st.matching_error,
-                    inlier_fraction=st.inlier_fraction)
+        return _odometry_status(st)
+
+    def matching_ros(self, sec, nsec, cloud, msf_delta=None, want_status=False):
+        """matching() with a ros::Time stamp (sec, nsec): the keyframe test takes roscpp's exact (stamp - keyframe_stamp).toSec(), and
+        the status (matching_error, inlier_fraction) is computed only when want_status is set"""
+        a, n, s = _cloud(cloud)
+        return self.matching_ros_raw(sec, nsec, a.ctypes.data, n, s, msf_delta, want_status)
+
+    def matching_ros_raw(self, sec, nsec, ptr, n, stride_bytes, msf_delta=None, want_status=False, device=False):
+        st = OdometryStatus()
+        dp = None
+        if msf_delta is not None:
+            d = _colmajor(msf_delta)
+            dp = d.ctypes.data_as(C.POINTER(C.c_float))
+        check(self._lib.b2r_odometry_matching_ros(self._o, int(sec), int(nsec), C.c_void_p(ptr), n, stride_bytes, int(device), dp,
+                                                  int(bool(want_status)), C.byref(st)))
+        return _odometry_status(st)
+
+    def aligned(self, n, stride_bytes=32, is_dense=True):
+        """aligned_points of the last matching call: its raw cloud (n records of stride_bytes) under odom, as (n, stride_bytes / 4)
+        float32; raises after a first or rejected frame"""
+        out = np.zeros((n, stride_bytes // 4), np.float32)
+        check(self._lib.b2r_odometry_aligned(self._o, int(bool(is_dense)), out.ctypes.data, n, stride_bytes))
+        return out
+
+
+def _odometry_status(st):
+    return dict(odom=_from_colmajor(st.odom), trans=_from_colmajor(st.trans), converged=bool(st.converged), iterations=st.iterations,
+                keyframe_updated=bool(st.keyframe_updated), frame_rejected=bool(st.frame_rejected), matching_error=st.matching_error,
+                inlier_fraction=st.inlier_fraction)
 
 
 class LoopDetector:

@@ -386,8 +386,10 @@ int b2r_map_cloud_generate(b2r_handle* h, const b2r_keyframe_snapshot* keyframes
  * A sensor_msgs/PointCloud2 data[] blob (or a binary PCD body) goes to the device unconverted and is unpacked there into
  * pcl::PointXYZI records (32 bytes: x y z 1 | intensity 0 0 0) — the work of pcl::fromROSMsg at
  * apps/scan_matching_odometry_nodelet.cpp:118-119 and apps/hdl_graph_slam_nodelet.cpp:153-154, and of pcl::io::loadPCDFile at
- * src/hdl_graph_slam/keyframe.cpp:141.  *d_points is an engine-owned device buffer (valid until the next ingest call on this
- * handle) for b2r_set_source_device / b2r_set_target_device / b2r_prefilter(device_input = 1) / b2r_batch_add_cloud_device.
+ * src/hdl_graph_slam/keyframe.cpp:141.  *d_points is an engine-owned device buffer for b2r_set_source_device /
+ * b2r_set_target_device / b2r_prefilter(device_input = 1) / b2r_batch_add_cloud_device / b2r_odometry_matching_ros(device = 1).  Two
+ * such buffers are used in turn, so it stays valid until the SECOND ingest call after it on this handle: a frame ingested and matched
+ * on the odometry's own handle is still intact while the next frame is ingested and matched against it.
  *   - Field mapping as PCL's fromPCLPointCloud2 does it for PointXYZI: intensity is read only when its datatype is FLOAT32; an
  *     intensity field of any other datatype is left unmapped and every point gets intensity 0 (PCL warns and does the same).
  *   - is_bigendian is honoured: x, y, z and intensity are byte-swapped.  (PCL copies the bytes as they are, so a big-endian
@@ -460,6 +462,25 @@ int b2r_odometry_matching(b2r_odometry* o, double stamp, const void* cloud, size
 /* same, for a cloud already resident in device memory (the HBM-resident measurement of bench.py) */
 int b2r_odometry_matching_device(b2r_odometry* o, double stamp, const void* d_cloud, size_t n, size_t stride_bytes, const float* msf_delta,
                                  b2r_odometry_status* out);
+
+/* matching(stamp, cloud) with the stamp as ros::Time holds it (sec, nsec) and the status chosen per call (want_status: status_pub has
+ * subscribers, :299; the first frame computes none whatever it says).  device != 0: `cloud` is a device pointer, e.g. an ingest buffer of
+ * the odometry's handle.  The keyframe test's delta_time is roscpp's exact (stamp - keyframe_stamp).toSec() (:243): seconds and
+ * nanoseconds subtracted as integers, nanoseconds normalised into [0, 1e9), then sec + 1e-9 * nsec; the double entry points subtract
+ * two doubles instead, which decides differently when the true difference lies within a few hundred nanoseconds of
+ * keyframe_delta_time.  One odometry may mix both forms: the keyframe keeps the form of the call that made it, roscpp's rule applies
+ * when both stamps are sec / nsec, and otherwise the doubles are subtracted, a sec / nsec stamp taken as ros::Time::toSec(). */
+int b2r_odometry_matching_ros(b2r_odometry* o, uint32_t sec, uint32_t nsec, const void* cloud, size_t n, size_t stride_bytes, int device,
+                              const float* msf_delta, int want_status, b2r_odometry_status* out);
+
+/* aligned_points of the last matching call (:254-259): pcl::transformPointCloud(*cloud, *aligned, odom) of the RAW cloud that call was
+ * given (before the odometry's downsample), computed on the device from the records matching left there (no second upload) and written
+ * to `out` as n records of stride_bytes.  Each record is copied, then x, y, z become ((m0 x + m1 y) + m2 z) + m3 under odom (as
+ * b2r_get_aligned) and the float at byte 12 becomes 1.0f (when stride_bytes >= 16).  is_dense == 0 (the input cloud's is_dense): a
+ * record with a non-finite x, y or z stays as it was (PCL 1.10's non-dense branch).  B2R_ESTATE unless the last matching call
+ * succeeded on an accepted frame (not the first, not rejected, :214-233 return before :254); B2R_EINVAL when n or stride_bytes
+ * differs from that call's.  A device cloud given to that call is read again here: keep it unchanged until this returns. */
+int b2r_odometry_aligned(b2r_odometry* o, int is_dense, void* out, size_t n, size_t stride_bytes);
 
 /* announce the cloud of the NEXT matching() call: the following matching() prefetches it (b2r_prefetch_source) right after it
  * has set its own source, so the next frame's preprocessing overlaps this frame's align.  device != 0: device pointer.
