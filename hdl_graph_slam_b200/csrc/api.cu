@@ -2696,7 +2696,8 @@ static int odometry_matching_impl(b2r_odometry* o, const OdomStamp& stamp, const
     rc = b2r_fitness(reg, nullptr, DBL_MAX, 0.5f * 0.5f, &score, &used, &inl);
     if (rc) return rc;
     out->matching_error = score;
-    out->inlier_fraction = n_reg ? (float)inl / (float)n_reg : 0.f;
+    // static_cast<float>(num_inliers) / aligned->size() (:321): an empty registered frame gives 0.f / 0.f = NaN
+    out->inlier_fraction = n_reg ? (float)inl / (float)n_reg : NAN;
   }
   float trans[16], odom_row[16];
   for (int r = 0; r < 4; r++) for (int c = 0; c < 4; c++) trans[r * 4 + c] = res.T[c * 4 + r];
